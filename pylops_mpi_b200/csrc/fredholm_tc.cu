@@ -76,6 +76,17 @@ __device__ __forceinline__ void mma_k16(float (&d)[BN / 2], uint64_t da, uint64_
   else wgmma_m64n128k16_f16<0, 0>(d, da, db, scale_d);
 }
 
+// v * sa * sb for power-of-two scales sa (row of op(G)) and sb (column of x).  sa * sb is exact unless it leaves the
+// normal range, which needs both scales < 1 or both > 1 (tiny or huge maxima on both sides, while the result itself
+// can still be a normal float or zero); then the scale nearer 1 goes first, so that the intermediate lies between v
+// and the result and, for a normal result, only the last product rounds.
+__device__ __forceinline__ float unscale(float v, float sa, float sb) {
+  const float p = sa * sb;
+  if (p >= 0x1p-126f && p <= 0x1p127f) return v * p;
+  const float lo = fminf(sa, sb), hi = fmaxf(sa, sb);
+  return p < 1.f ? (v * hi) * lo : (v * lo) * hi;
+}
+
 template <int MODE>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 fredholm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
@@ -200,8 +211,8 @@ fredholm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
           const float* sb_inv = invB + (size_t)s * nz;
           const float c0 = __ldg(sb_inv + col / zdiv);
           const float c1 = (col + 1 < n) ? __ldg(sb_inv + (col + 1) / zdiv) : 0.f;
-          o.x = fmaf(sml[4 * j + 2 * h], 1.f / 2048.f, acc[4 * j + 2 * h]) * (sa_inv * c0);
-          o.y = fmaf(sml[4 * j + 2 * h + 1], 1.f / 2048.f, acc[4 * j + 2 * h + 1]) * (sa_inv * c1);
+          o.x = unscale(fmaf(sml[4 * j + 2 * h], 1.f / 2048.f, acc[4 * j + 2 * h]), sa_inv, c0);
+          o.y = unscale(fmaf(sml[4 * j + 2 * h + 1], 1.f / 2048.f, acc[4 * j + 2 * h + 1]), sa_inv, c1);
         } else {
           o.x = acc[4 * j + 2 * h] + sml[4 * j + 2 * h];
           o.y = acc[4 * j + 2 * h + 1] + sml[4 * j + 2 * h + 1];
@@ -247,13 +258,14 @@ __device__ __forceinline__ Split<MODE> split(float v, float scale) {
 }
 __device__ __forceinline__ unsigned short neg16(unsigned short h) { return h ^ 0x8000u; }   // bf16 and fp16: sign bit
 
-// power-of-two scale that puts amax just below 2^15 (exponent clamped so scale and 1/scale stay normal floats)
+// power-of-two scale that puts amax just below 2^15 (exponent clamped so scale and 1/scale stay normal floats; every
+// finite float32 amax >= 2^-112 gets its exact scale, the largest ones need e = -113)
 __device__ __forceinline__ void pow2_scale(float amax, float* scale, float* inv) {
   int ex = 0;
   if (amax > 0.f && amax < INFINITY) frexpf(amax, &ex);      // amax = f * 2^ex, f in [0.5, 1)
   else ex = 15;
   int e = 15 - ex;
-  e = e > 100 ? 100 : (e < -100 ? -100 : e);
+  e = e > 126 ? 126 : (e < -126 ? -126 : e);
   *scale = ldexpf(1.f, e);
   *inv = ldexpf(1.f, -e);
 }
