@@ -230,8 +230,6 @@ int b2_fredholm_plan_create(b2_ctx* ctx, const void* G, size_t nsl, size_t nx, s
 int b2_fredholm_plan_destroy(b2_fredholm_plan* plan);
 int b2_fredholm_apply(b2_fredholm_plan* plan, const void* x, void* y, void* const* peers_host, int npeers,
                       int adjoint, void* stream);
-/* profiling aid: parts = 1 packs x only, 2 = product on the planes of the previous pack, 3 = both */
-int b2_fredholm_apply_parts(b2_fredholm_plan* plan, const void* x, void* y, int adjoint, int parts, void* stream);
 /* peer-mappable device buffers (cudaMalloc) and CUDA IPC handle plumbing (64-byte handles) */
 int b2_symm_alloc(size_t bytes, void** out);
 int b2_symm_free(void* p);
@@ -278,7 +276,7 @@ int b2_allgather(b2_comm* comm, const void* send, void* recv, size_t n_per_rank,
 int b2_allgatherv(b2_comm* comm, const void* send, void* recv, const size_t* counts_host,
                   int dtype, void* stream);
 /* same, with explicit placement: rank r's counts[r] elements land at recv + offsets[r] (elements);
- * send may alias its own destination (in-place).  Enables chunked gather overlapped with compute. */
+ * send may alias its own destination (in-place). */
 int b2_allgatherv_at(b2_comm* comm, const void* send, void* recv, const size_t* counts_host,
                      const size_t* offsets_host, int dtype, void* stream);
 int b2_bcast(b2_comm* comm, void* buf, size_t n, int dtype, int root, void* stream);  /* :243-262 */

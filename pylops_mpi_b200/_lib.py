@@ -102,7 +102,6 @@ def _load():
         "b2_fredholm_plan_create": ([vp, vp, sz, sz, sz, sz, i, C.POINTER(vp)], i),
         "b2_fredholm_plan_destroy": ([vp], i),
         "b2_fredholm_apply": ([vp, vp, vp, C.POINTER(vp), i, i, vp], i),
-        "b2_fredholm_apply_parts": ([vp, vp, vp, i, i, vp], i),
         "b2_symm_alloc": ([sz, C.POINTER(vp)], i),
         "b2_symm_free": ([vp], i),
         "b2_ipc_get_handle": ([vp, vp], i),

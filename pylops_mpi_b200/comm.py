@@ -124,6 +124,39 @@ class Comm:
             self._nccl = h
         return self._nccl
 
+    def _symm_map(self, nbytes: int):
+        """COLLECTIVE: every rank allocates ``nbytes`` of IPC-mappable device memory, exports its IPC handle, the
+        handles are allgathered and every rank maps every peer's buffer.  Returns ``(ok, my_ptr, ptrs)`` with
+        ``ptrs[r]`` = rank r's buffer as addressable from this process (``ptrs[rank] == my_ptr``).  A failed
+        allocation or export on any rank fails every rank (the flag travels with the handles); ``ok`` only covers
+        this rank's mapping of its peers, so callers finish with one allgather of ``ok`` to agree."""
+        from . import _lib
+        ok, ptr, mine = 1, C.c_void_p(), b""
+        try:
+            _lib.check(_lib.lib.b2_symm_alloc(max(int(nbytes), 16), C.byref(ptr)), "b2_symm_alloc")
+            if self._size > 1:
+                h = (C.c_char * 64)()
+                _lib.check(_lib.lib.b2_ipc_get_handle(ptr, h), "b2_ipc_get_handle")
+                mine = bytes(h.raw)
+        except Exception:
+            ok = 0
+        handles = self.allgather((ok, mine))
+        if not all(hh[0] for hh in handles):
+            return 0, ptr.value, None
+        ptrs = []
+        try:
+            for r, (_, raw) in enumerate(handles):
+                if r == self._rank:
+                    ptrs.append(ptr.value)
+                else:
+                    q = C.c_void_p()
+                    _lib.check(_lib.lib.b2_ipc_open_handle((C.c_char * 64).from_buffer_copy(raw), C.byref(q)),
+                               "b2_ipc_open_handle")
+                    ptrs.append(q.value)
+        except Exception:
+            return 0, ptr.value, None
+        return 1, ptr.value, ptrs
+
     def _ipc_mailboxes(self, attr: str, nbytes_fn, create_fn):
         """collective lazy setup of an IPC-mapped mailbox group (one symmetric buffer per rank, every
         rank maps every peer's); returns the library handle or None when CUDA IPC is unavailable"""
@@ -131,27 +164,12 @@ class Comm:
             return None
         if getattr(self, attr, None) is None and not getattr(self, attr + "_failed", False):
             from . import _lib
-            ok, ptr, mine, hnd = 1, C.c_void_p(), b"", None
-            try:
-                nbytes = getattr(_lib.lib, nbytes_fn)() if isinstance(nbytes_fn, str) else nbytes_fn()
-                _lib.check(_lib.lib.b2_symm_alloc(nbytes, C.byref(ptr)), "b2_symm_alloc")
-                h = (C.c_char * 64)()
-                _lib.check(_lib.lib.b2_ipc_get_handle(ptr, h), "b2_ipc_get_handle")
-                mine = bytes(h.raw)
-            except Exception:
-                ok = 0
-            handles = self.allgather((ok, mine))
-            boxes = (C.c_void_p * self._size)()
-            if all(hh[0] for hh in handles):
+            nbytes = getattr(_lib.lib, nbytes_fn)() if isinstance(nbytes_fn, str) else nbytes_fn()
+            ok, _, ptrs = self._symm_map(nbytes)
+            hnd = None
+            if ok:
                 try:
-                    for r, (_, raw) in enumerate(handles):
-                        if r == self._rank:
-                            boxes[r] = ptr.value
-                        else:
-                            q = C.c_void_p()
-                            _lib.check(_lib.lib.b2_ipc_open_handle((C.c_char * 64).from_buffer_copy(raw), C.byref(q)),
-                                       "b2_ipc_open_handle")
-                            boxes[r] = q.value
+                    boxes = (C.c_void_p * self._size)(*ptrs)
                     hnd = C.c_void_p()
                     if isinstance(create_fn, str):
                         _lib.check(getattr(_lib.lib, create_fn)(self._rank, self._size, boxes, C.byref(hnd)), create_fn)
@@ -159,8 +177,6 @@ class Comm:
                         create_fn(boxes, hnd)
                 except Exception:
                     ok = 0
-            else:
-                ok = 0
             if min(self.allgather(ok)) == 1:      # every rank zeroed its mailbox and mapped its peers
                 setattr(self, attr, hnd)
             else:
@@ -170,25 +186,14 @@ class Comm:
     def symm_alloc(self, nbytes: int):
         """COLLECTIVE: every rank allocates ``nbytes`` of IPC-mappable device memory and maps every peer's
         buffer; returns ``(my_ptr, ptrs)`` with ``ptrs[r]`` = rank r's buffer as addressable from this process
-        (``ptrs[rank] == my_ptr``).  Used for the peer-memory arenas of the fused compute + collective kernels."""
-        from . import _lib
-        ptr = C.c_void_p()
-        _lib.check(_lib.lib.b2_symm_alloc(max(int(nbytes), 16), C.byref(ptr)), "b2_symm_alloc")
-        if self._size == 1:
-            return ptr.value, [ptr.value]
-        h = (C.c_char * 64)()
-        _lib.check(_lib.lib.b2_ipc_get_handle(ptr, h), "b2_ipc_get_handle")
-        handles = self.allgather(bytes(h.raw))
-        ptrs = []
-        for r, raw in enumerate(handles):
-            if r == self._rank:
-                ptrs.append(ptr.value)
-            else:
-                q = C.c_void_p()
-                _lib.check(_lib.lib.b2_ipc_open_handle((C.c_char * 64).from_buffer_copy(raw), C.byref(q)),
-                           "b2_ipc_open_handle")
-                ptrs.append(q.value)
-        return ptr.value, ptrs
+        (``ptrs[rank] == my_ptr``).  Used for the peer-memory arenas of the fused compute + collective kernels.
+        Raises on every rank when the allocation or the mapping failed on any rank."""
+        ok, ptr, ptrs = self._symm_map(nbytes)
+        if min(self.allgather(ok)) == 0:
+            from . import _lib
+            raise _lib.B200Error(f"symm_alloc of {int(nbytes)} bytes: the allocation or the CUDA IPC mapping "
+                                 f"failed on at least one rank")
+        return ptr, ptrs
 
     @property
     def peer(self):

@@ -663,8 +663,8 @@ static int launch_product(b2_fredholm_plan* pl, int d, float* y, const PeerOut& 
 // y[s] = op(G[s]) x[s] for all slices of the plan; peers_host (npeers <= 8, may be NULL/0): the same logical
 // output position in peer GPUs' IPC-mapped buffers -- the epilogue stores every element there too (fused all-gather).
 // Applies of one plan must be stream-ordered (they share the X' workspace).
-static int fredholm_apply_impl(b2_fredholm_plan* pl, const void* x, void* y, void* const* peers_host, int npeers,
-                               int adjoint, int parts, void* stream) {
+extern "C" int b2_fredholm_apply(b2_fredholm_plan* pl, const void* x, void* y, void* const* peers_host, int npeers,
+                                 int adjoint, void* stream) {
   if (!pl || !x || !y || npeers < 0 || npeers > 8 || (npeers && !peers_host)) return B2_ERR_ARG;
   const int d = adjoint ? 1 : 0;
   cudaStream_t st = (cudaStream_t)stream;
@@ -674,7 +674,7 @@ static int fredholm_apply_impl(b2_fredholm_plan* pl, const void* x, void* y, voi
   dim3 grid(pl->nstrips, (unsigned)pl->nsl, (kcover + PK_ROWS - 1) / PK_ROWS);
   if (grid.z > 65535u) return B2_ERR_ARG;
   const float* xf = (const float*)x;
-  if ((parts & 1) && pl->pack_small && kcover <= PS_K) {
+  if (pl->pack_small && kcover <= PS_K) {
     dim3 gs((nz + PS_Z - 1) / PS_Z, (unsigned)pl->nsl);
     if (pl->mode == MODE_B3) {
       if (pl->cx) pack_x_small_kernel<true, MODE_B3><<<gs, PS_THREADS, 0, st>>>(xf, pl->BT[d], pl->invB, K, nz, pl->n, kpad);
@@ -684,7 +684,7 @@ static int fredholm_apply_impl(b2_fredholm_plan* pl, const void* x, void* y, voi
       else pack_x_small_kernel<false, MODE_H2><<<gs, PS_THREADS, 0, st>>>(xf, pl->BT[d], pl->invB, K, nz, pl->n, kpad);
     }
     B2_LAUNCH_CHECK();
-  } else if (parts & 1) {
+  } else {
     if (pl->mode == MODE_B3) {
       if (pl->cx) pack_x_kernel<true, MODE_B3><<<grid, PK_THREADS, 0, st>>>(xf, pl->BT[d], pl->invB, K, nz, pl->n, kpad);
       else pack_x_kernel<false, MODE_B3><<<grid, PK_THREADS, 0, st>>>(xf, pl->BT[d], pl->invB, K, nz, pl->n, kpad);
@@ -694,22 +694,10 @@ static int fredholm_apply_impl(b2_fredholm_plan* pl, const void* x, void* y, voi
     }
     B2_LAUNCH_CHECK();
   }
-  if (!(parts & 2)) return B2_OK;
   PeerOut po;
   po.n = npeers;
   for (int i = 0; i < 8; ++i) po.p[i] = i < npeers ? (float*)peers_host[i] : nullptr;
   if (pl->mode == MODE_B3)
     return launch_product<MODE_B3>(pl, d, (float*)y, po, st);
   return launch_product<MODE_H2>(pl, d, (float*)y, po, st);
-}
-
-extern "C" int b2_fredholm_apply(b2_fredholm_plan* pl, const void* x, void* y, void* const* peers_host, int npeers,
-                                 int adjoint, void* stream) {
-  return fredholm_apply_impl(pl, x, y, peers_host, npeers, adjoint, 3, stream);
-}
-
-// profiling aid: parts = 1 packs x only, 2 runs the product on the planes of the previous pack, 3 = both
-extern "C" int b2_fredholm_apply_parts(b2_fredholm_plan* pl, const void* x, void* y, int adjoint, int parts, void* stream) {
-  if (parts < 1 || parts > 3) return B2_ERR_ARG;
-  return fredholm_apply_impl(pl, x, y, nullptr, 0, adjoint, parts, stream);
 }

@@ -10,7 +10,6 @@
 //  * op = T/H: one lane per 16-byte column vector, warps stride over the rows of a
 //            row chunk, CTA-level smem fold, chunk partials folded in chunk order
 //            by the last CTA of each column tile (deterministic, no atomics on y).
-#include <cstdlib>
 #include "common.cuh"
 
 namespace {
@@ -246,15 +245,6 @@ gemv_n_split_kernel(const TA* __restrict__ A, size_t lda, size_t m, size_t n,
   }
 }
 
-inline bool gemv_split_enabled() {
-  static int on = -1;
-  if (on < 0) {
-    const char* e = getenv("B2_GEMV_SPLIT");
-    on = (e && e[0] == '0') ? 0 : 1;
-  }
-  return on == 1;
-}
-
 // -------------------------------------------------------------------------
 // op = T / H : y_j = sum_i op(A_ij) x_i
 // grid = (column tiles, row chunks); CTA = 8 warps; lane <-> 16-byte column vector
@@ -365,7 +355,7 @@ int launch_gemv(b2_ctx* ctx, const void* A, size_t lda, size_t m, size_t n, cons
   if (op == B2_OP_N) {
     if (m == 0) return B2_OK;
     unsigned grid = (unsigned)((m + GN_WARPS - 1) / GN_WARPS);
-    if (vec && b2_aligned16(x) && n * sizeof(TA) >= 32768 && gemv_split_enabled()) {
+    if (vec && b2_aligned16(x) && n * sizeof(TA) >= 32768) {
       constexpr int R = 4;
       gemv_n_split_kernel<TA, R><<<(unsigned)((m + R - 1) / R), GS_WARPS * 32, 0, st>>>((const TA*)A, lda, m, n, (const X*)x,
                                                                                         (X*)y);

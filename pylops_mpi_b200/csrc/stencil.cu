@@ -19,7 +19,6 @@
 // friendly; the 2R overlap rows are L2 hits, DRAM traffic stays ~algorithmic),
 // 64-row chunks (first design) reached 0.85 of the copy peak, 4-row chunks 1.04.
 // Algorithmic bytes: 2*sizeof(T) per element.
-#include <stdlib.h>
 #include "common.cuh"
 
 namespace {
@@ -159,14 +158,11 @@ __device__ __forceinline__ const double* special_taps(const StencilParams& p, lo
 // fast path: 16-byte column vectors, rolling window down a chunk of rows.
 // MASK bit (k+R) set <=> interior tap k is non-zero (compile-time skip).
 // -------------------------------------------------------------------------
-// tuning knobs (template parameters): ST_COLS threads along columns, ST_ROWS rows per chunk
-// (per thread), ST_U rows loaded per step.  Variant 0 is the default; B2_STENCIL_VARIANT selects
-// another one at run time (for tuning sweeps).
-template <typename T, int MASK, int ST_ROWS, int ST_U, int ST_COLS, bool PEER = false>
+constexpr int ST_ROWS = 4, ST_U = 4, ST_COLS = 128;   // rows per chunk, rows loaded per step, threads per CTA
+template <typename T, int MASK, bool PEER>
 __global__ void __launch_bounds__(ST_COLS)
 stencil_vec_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restrict__ lo,
-                   const T* __restrict__ hi, const __grid_constant__ StencilParams p,
-                   const HaloPeer hp = HaloPeer{}) {
+                   const T* __restrict__ hi, const __grid_constant__ StencilParams p, const HaloPeer hp) {
   constexpr int V = Vec16<T>::N;
   const long long ncv = p.ncols / V;
   // 1-D grid, column tile fastest: concurrently running CTAs cover whole rows
@@ -373,54 +369,26 @@ int interior_mask(const double t[NT]) {
   return m;
 }
 
-template <typename T, int ROWS, int U, int COLS>
-int launch_vec(const void* x, void* y, const void* lo, const void* hi, const StencilParams& p, int mask,
+// PEER: the halo rows arrive through hp's peer boxes (lo / hi unused, one problem); otherwise from lo / hi, with
+// p.nbatch problems along grid.y
+template <typename T, bool PEER>
+int launch_vec(const void* x, void* y, const void* lo, const void* hi, const StencilParams& p, const HaloPeer& hp,
                cudaStream_t st) {
   constexpr int V = Vec16<T>::N;
-  const long long nblk = ((p.ncols / V + COLS - 1) / COLS) * ((p.nloc + ROWS - 1) / ROWS);
+  const long long nblk = ((p.ncols / V + ST_COLS - 1) / ST_COLS) * ((p.nloc + ST_ROWS - 1) / ST_ROWS);
   if (nblk > 0x7fffffffLL) return B2_ERR_ARG;
-  const dim3 grid((unsigned)nblk, (unsigned)p.nbatch);
   if (p.nbatch > 65535) return B2_ERR_ARG;
-#define B2_ST_CASE(M)                                                                              \
-  case M:                                                                                          \
-    stencil_vec_kernel<T, M, ROWS, U, COLS><<<grid, COLS, 0, st>>>((const T*)x, (T*)y, (const T*)lo, \
-                                                                   (const T*)hi, p);               \
-    break;
-  switch (mask) {
-    B2_ST_CASE(0x0c)  // taps {0,+1}
-    B2_ST_CASE(0x06)  // taps {-1,0}
-    B2_ST_CASE(0x0a)  // taps {-1,+1}
-    B2_ST_CASE(0x1b)  // taps {-2,-1,+1,+2}
-    default:
-      stencil_vec_kernel<T, 0x1f, ROWS, U, COLS><<<grid, COLS, 0, st>>>((const T*)x, (T*)y, (const T*)lo,
-                                                                        (const T*)hi, p);
+  const dim3 grid((unsigned)nblk, PEER ? 1u : (unsigned)p.nbatch);
+#define B2_ST_LAUNCH(M) \
+  stencil_vec_kernel<T, M, PEER><<<grid, ST_COLS, 0, st>>>((const T*)x, (T*)y, (const T*)lo, (const T*)hi, p, hp)
+  switch (interior_mask(p.interior)) {
+    case 0x0c: B2_ST_LAUNCH(0x0c); break;   // taps {0,+1}
+    case 0x06: B2_ST_LAUNCH(0x06); break;   // taps {-1,0}
+    case 0x0a: B2_ST_LAUNCH(0x0a); break;   // taps {-1,+1}
+    case 0x1b: B2_ST_LAUNCH(0x1b); break;   // taps {-2,-1,+1,+2}
+    default: B2_ST_LAUNCH(0x1f);
   }
-#undef B2_ST_CASE
-  B2_LAUNCH_CHECK();
-  return B2_OK;
-}
-
-// peer-memory halo mode: the tuned (4, 4, 128) variant with the exchange fused in
-template <typename T>
-int launch_vec_peer(const void* x, void* y, const StencilParams& p, const HaloPeer& hp, int mask, cudaStream_t st) {
-  constexpr int V = Vec16<T>::N;
-  constexpr int ROWS = 4, U = 4, COLS = 128;
-  const long long nblk = ((p.ncols / V + COLS - 1) / COLS) * ((p.nloc + ROWS - 1) / ROWS);
-  if (nblk > 0x7fffffffLL) return B2_ERR_ARG;
-  const dim3 grid((unsigned)nblk, 1u);
-#define B2_ST_CASE(M)                                                                                       \
-  case M:                                                                                                   \
-    stencil_vec_kernel<T, M, ROWS, U, COLS, true><<<grid, COLS, 0, st>>>((const T*)x, (T*)y, nullptr, nullptr, p, hp); \
-    break;
-  switch (mask) {
-    B2_ST_CASE(0x0c)
-    B2_ST_CASE(0x06)
-    B2_ST_CASE(0x0a)
-    B2_ST_CASE(0x1b)
-    default:
-      stencil_vec_kernel<T, 0x1f, ROWS, U, COLS, true><<<grid, COLS, 0, st>>>((const T*)x, (T*)y, nullptr, nullptr, p, hp);
-  }
-#undef B2_ST_CASE
+#undef B2_ST_LAUNCH
   B2_LAUNCH_CHECK();
   return B2_OK;
 }
@@ -432,35 +400,12 @@ int launch_stencil(b2_ctx* ctx, const void* x, void* y, const void* lo, const vo
   const bool vec_ok = (p.ncols % V == 0) && b2_aligned16(x) && b2_aligned16(y) &&
                       (!lo || b2_aligned16(lo)) && (!hi || b2_aligned16(hi)) &&
                       (p.ncols / V >= 8);
-  const int mask = interior_mask(p.interior);
-  if (vec_ok) {
-    static int variant = -1;
-    if (variant < 0) {
-      const char* e = getenv("B2_STENCIL_VARIANT");
-      variant = e ? atoi(e) : 0;
-    }
-    switch (variant) {
-      case 1: return launch_vec<T, 8, 4, 128>(x, y, lo, hi, p, mask, st);
-      case 2: return launch_vec<T, 8, 2, 128>(x, y, lo, hi, p, mask, st);
-      case 3: return launch_vec<T, 4, 4, 128>(x, y, lo, hi, p, mask, st);
-      case 4: return launch_vec<T, 4, 2, 128>(x, y, lo, hi, p, mask, st);
-      case 5: return launch_vec<T, 8, 8, 128>(x, y, lo, hi, p, mask, st);
-      case 6: return launch_vec<T, 8, 4, 256>(x, y, lo, hi, p, mask, st);
-      case 7: return launch_vec<T, 8, 4, 64>(x, y, lo, hi, p, mask, st);
-      case 8: return launch_vec<T, 4, 4, 256>(x, y, lo, hi, p, mask, st);
-      case 9: return launch_vec<T, 8, 1, 128>(x, y, lo, hi, p, mask, st);
-      case 10: return launch_vec<T, 2, 2, 128>(x, y, lo, hi, p, mask, st);
-      case 11: return launch_vec<T, 8, 2, 256>(x, y, lo, hi, p, mask, st);
-      case 12: return launch_vec<T, 64, 4, 128>(x, y, lo, hi, p, mask, st);   // first design (r01 baseline)
-      default: return launch_vec<T, 4, 4, 128>(x, y, lo, hi, p, mask, st);    // tuned default
-    }
-  } else {
-    size_t total = (size_t)p.nloc * (size_t)p.ncols * (size_t)p.nbatch;
-    size_t need = (total + 255) / 256;
-    size_t cap = (size_t)ctx->sm_count * 8;
-    int grid = (int)(need < cap ? need : cap);
-    stencil_generic_kernel<T><<<grid, 256, 0, st>>>((const T*)x, (T*)y, (const T*)lo, (const T*)hi, p);
-  }
+  if (vec_ok) return launch_vec<T, false>(x, y, lo, hi, p, HaloPeer{}, st);
+  size_t total = (size_t)p.nloc * (size_t)p.ncols * (size_t)p.nbatch;
+  size_t need = (total + 255) / 256;
+  size_t cap = (size_t)ctx->sm_count * 8;
+  int grid = (int)(need < cap ? need : cap);
+  stencil_generic_kernel<T><<<grid, 256, 0, st>>>((const T*)x, (T*)y, (const T*)lo, (const T*)hi, p);
   B2_LAUNCH_CHECK();
   return B2_OK;
 }
@@ -617,9 +562,9 @@ extern "C" int b2_derivative_peer(b2_ctx* ctx, b2_halo* h, const void* x, void* 
   hp.tickets = h->tickets;
   hp.send_lo = h->box[0] ? need_hi : 0;    // rank-1 needs my first need_hi rows as ITS hi halo
   hp.send_hi = h->box[2] ? need_lo : 0;    // rank+1 needs my last need_lo rows as ITS lo halo
-  const int mask = interior_mask(p.interior);
   cudaStream_t st = (cudaStream_t)stream;
-  return dtype == B2_F32 ? launch_vec_peer<float>(x, y, p, hp, mask, st) : launch_vec_peer<double>(x, y, p, hp, mask, st);
+  return dtype == B2_F32 ? launch_vec<float, true>(x, y, nullptr, nullptr, p, hp, st)
+                         : launch_vec<double, true>(x, y, nullptr, nullptr, p, hp, st);
 }
 
 // ---- MPISecondDerivative per-rank apply (basicoperators/SecondDerivative.py:125-257) -----------------

@@ -12,7 +12,6 @@ Two execution modes, same numbers:
 """
 from __future__ import annotations
 
-import os
 import sys
 import time
 from typing import List, Optional, Sequence
@@ -52,7 +51,6 @@ _GRAPH_SAFE_TYPES = ("MPIBlockDiag", "MPIVStack", "MPIHStack", "MPIFirstDerivati
 
 
 _GRAPH_POOL = {}
-_CAPTURE_MODE = os.environ.get("B2_CGLS_CAPTURE_MODE", "thread_local")   # diagnostics: "global" / "relaxed"
 
 
 def _graph_pool():
@@ -472,7 +470,7 @@ class CGLS(Solver):
             if self._cc_ready:                      # the fused c.c partial belongs to the restored c again
                 _dots_device([self.c], self._dev, self._st)
 
-        use_graph = os.environ.get("B2_CGLS_GRAPH", "1") != "0" and _graph_safe(self.Op)
+        use_graph = _graph_safe(self.Op)
         state = {"graph": None, "use": use_graph, "warm": 0}
         self.graph_replays, self.graph_error = 0, (None if use_graph else "operator not on the graph-safe list")
         self._cc_ready = False                      # first body computes c.c itself
@@ -500,7 +498,7 @@ class CGLS(Solver):
                         # thread_local error mode: NCCL's helper threads keep polling CUDA while we capture
                         # (observed at 8 ranks: a "global"-mode capture was invalidated and left torch's RNG state
                         # stuck in capture mode)
-                        g.capture_begin(pool=pool, capture_error_mode=_CAPTURE_MODE)   # records only
+                        g.capture_begin(pool=pool, capture_error_mode="thread_local")   # records only
                         t_begin = time.perf_counter()
                         try:
                             self._body(x, hist, it_dev)

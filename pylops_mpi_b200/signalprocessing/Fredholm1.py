@@ -4,6 +4,7 @@ the slice axis; BROADCAST model in, BROADCAST data out via an NCCL Allgather(v)
 written straight into the output buffer."""
 from __future__ import annotations
 
+import ctypes as C
 import os
 
 import numpy as np
@@ -47,13 +48,20 @@ class MPIFredholm1(MPILinearOperator):
         self.saveGt = saveGt
         self.usematmul = usematmul
         # fused=True: product + all-gather in ONE kernel over NVLink peer memory (IPC-mapped output
-        # arenas); default: product kernels + chunked NCCL gather overlapped on a side stream
+        # arenas); fused=False: product kernel, then one NCCL Allgatherv in place
         # fused=None (default): on when CUDA IPC peer mapping works between the ranks (probed by comm.peer)
         if fused is None:
             fused = base_comm.Get_size() > 1 and base_comm.peer is not None
         self._fused = bool(fused) and base_comm.Get_size() > 1 and not self._scatter_data
         if self._fused:
-            self._setup_arenas(base_comm)
+            esz = torch.empty(0, dtype=self._tdtype).element_size()
+            self._arena = {}
+            for adjoint in (False, True):
+                nelem = nslstot * (self.ny if adjoint else self.nx) * self.nz
+                for b in range(2):
+                    self._arena[(adjoint, b)] = (*base_comm.symm_alloc(nelem * esz), nelem)
+            self._toggle = {False: 0, True: 0}
+            self._flag = torch.zeros(1, dtype=torch.float64, device="cuda")   # float64 -> peer-memory all-reduce
         # tensor-core plan (csrc/fredholm_tc.cu): float32 / complex64 products run on wgmma with fp16x2 / bf16x3 split
         # operands (float32-class accuracy); G and G^H planes are built once here.  B2_FREDHOLM_TC=0 keeps the SIMT
         # kernel, =1 forces the tensor-core path for every shape (tests), default: slices of >= 32768 products.
@@ -61,7 +69,6 @@ class MPIFredholm1(MPILinearOperator):
         self._plan = None
         if self._tdtype in (torch.float32, torch.complex64) and mode != "0" and \
                 (mode == "1" or self.nx * self.ny * self.nz >= 32768) and self.nsl > 0:
-            import ctypes as C
             h = C.c_void_p()
             _lib.check(_lib.lib.b2_fredholm_plan_create(_lib.ctx(), self.G.data_ptr(), self.nsl, self.nx, self.ny, self.nz,
                                                         _lib.code(self._tdtype), C.byref(h)), "b2_fredholm_plan_create")
@@ -76,35 +83,42 @@ class MPIFredholm1(MPILinearOperator):
                 pass
             self._plan = None
 
-    # ---- fused product + all-gather over peer memory ------------------------------------------------
-    def _setup_arenas(self, comm):
-        import ctypes as C
-        esz = torch.empty(0, dtype=self._tdtype).element_size()
-        self._arena = {}
-        nsltot = int(sum(self.nsls))
-        for adjoint in (False, True):
-            nelem = nsltot * (self.ny if adjoint else self.nx) * self.nz
-            for b in range(2):
-                ptr = C.c_void_p()
-                _lib.check(_lib.lib.b2_symm_alloc(max(nelem * esz, 16), C.byref(ptr)), "b2_symm_alloc")
-                h = (C.c_char * 64)()
-                _lib.check(_lib.lib.b2_ipc_get_handle(ptr, h), "b2_ipc_get_handle")
-                handles = comm.allgather(bytes(h.raw))
-                peers = []
-                for r, raw in enumerate(handles):
-                    if r == comm.Get_rank():
-                        peers.append(ptr.value)
-                    else:
-                        q = C.c_void_p()
-                        buf = (C.c_char * 64).from_buffer_copy(raw)
-                        _lib.check(_lib.lib.b2_ipc_open_handle(buf, C.byref(q)), "b2_ipc_open_handle")
-                        peers.append(q.value)
-                self._arena[(adjoint, b)] = (ptr.value, peers, nelem)
-        self._toggle = {False: 0, True: 0}
-        self._flag = torch.zeros(1, dtype=torch.float64, device="cuda")   # float64 -> peer-memory all-reduce
+    def _product(self, x_ptr: int, y_ptr: int, adjoint: bool, peers=()):
+        """this rank's slices: y = op(G) x on the tensor-core plan when one was built, the SIMT kernel otherwise.
+        ``peers``: y's position in the other ranks' IPC-mapped arenas; the epilogue stores every output element
+        there too (fused all-gather)"""
+        arr = (C.c_void_p * len(peers))(*peers) if peers else None
+        if self._plan is not None:
+            _lib.check(_lib.lib.b2_fredholm_apply(self._plan, x_ptr, y_ptr, arr, len(peers), int(adjoint),
+                                                  _lib.stream()), "b2_fredholm_apply")
+        elif peers:
+            _lib.check(_lib.lib.b2_batched_gemm_allgather(_lib.ctx(), self.G.data_ptr(), x_ptr, y_ptr, arr, len(peers),
+                                                          self.nsl, self.nx, self.ny, self.nz, int(adjoint),
+                                                          _lib.code(self._tdtype), _lib.stream()),
+                       "b2_batched_gemm_allgather")
+        else:
+            _lib.check(_lib.lib.b2_batched_gemm(_lib.ctx(), self.G.data_ptr(), x_ptr, y_ptr, self.nsl, self.nx, self.ny,
+                                                self.nz, int(adjoint), _lib.code(self._tdtype), _lib.stream()),
+                       "b2_batched_gemm")
 
+    def _product_gathered(self, xs: torch.Tensor, y: DistributedArray, adjoint: bool) -> DistributedArray:
+        """this rank's slices of op(G) x straight into their place in the BROADCAST ``y``, then ONE NCCL Allgatherv
+        in place on the current stream brings in the other ranks' slices"""
+        rank, pout = self.rank, (self.ny if adjoint else self.nx) * self.nz
+        yflat = y.local_array.view(-1)
+        mine = yflat[self.islstart[rank] * pout: self.islend[rank] * pout]
+        if self.nsl:
+            self._product(xs.data_ptr(), mine.data_ptr(), adjoint)
+        if y.size > 1:
+            comm = y.base_comm
+            counts = (C.c_size_t * comm.size)(*[int(n) * pout for n in self.nsls])
+            offs = (C.c_size_t * comm.size)(*[int(o) * pout for o in self.islstart])
+            _lib.check(_lib.lib.b2_allgatherv_at(comm.nccl, mine.data_ptr(), yflat.data_ptr(), counts, offs,
+                                                 _lib.code(self._tdtype), _lib.stream()), "b2_allgatherv_at")
+        return y
+
+    # ---- fused product + all-gather over peer memory ------------------------------------------------
     def _apply_fused(self, x: DistributedArray, adjoint: bool) -> DistributedArray:
-        import ctypes as C
         from ..Distributed import allreduce_
         rank, comm = self.rank, x.base_comm
         nin, nout = (self.nx, self.ny) if adjoint else (self.ny, self.nx)
@@ -114,17 +128,8 @@ class MPIFredholm1(MPILinearOperator):
         b = self._toggle[adjoint]
         self._toggle[adjoint] = 1 - b
         base, peers, nelem = self._arena[(adjoint, b)]
-        esz = xl.element_size()
-        off = int(self.islstart[rank]) * pout * esz
-        others = [peers[r] + off for r in range(comm.Get_size()) if r != rank]
-        arr = (C.c_void_p * len(others))(*others)
-        if self._plan is not None:
-            _lib.check(_lib.lib.b2_fredholm_apply(self._plan, xs.data_ptr(), base + off, arr, len(others), int(adjoint),
-                                                  _lib.stream()), "b2_fredholm_apply")
-        else:
-            _lib.check(_lib.lib.b2_batched_gemm_allgather(_lib.ctx(), self.G.data_ptr(), xs.data_ptr(), base + off, arr,
-                                                          len(others), self.nsl, self.nx, self.ny, self.nz, int(adjoint),
-                                                          _lib.code(self._tdtype), _lib.stream()), "b2_batched_gemm_allgather")
+        off = int(self.islstart[rank]) * pout * xl.element_size()
+        self._product(xs.data_ptr(), base + off, adjoint, [peers[r] + off for r in range(comm.Get_size()) if r != rank])
         # stream-ordered cross-rank completion: when this tiny Allreduce finishes every rank's product
         # kernel (and its peer stores) has finished
         allreduce_(comm, self._flag, "sum")
@@ -134,16 +139,6 @@ class MPIFredholm1(MPILinearOperator):
         _lib.check(_lib.lib.b2_lincomb(_lib.ctx(), y.local_array.data_ptr(), _lib.cpair(1.0), base, None, None, nelem,
                                        _lib.code(self._tdtype), 0, _lib.stream()), "b2_lincomb")
         return y
-
-    def _local_product(self, xs: torch.Tensor, yout: torch.Tensor, adjoint: bool):
-        """this rank's slices: yout = op(G) xs (tensor-core plan when built, SIMT kernel otherwise)"""
-        if self._plan is not None:
-            _lib.check(_lib.lib.b2_fredholm_apply(self._plan, xs.data_ptr(), yout.data_ptr(), None, 0, int(adjoint),
-                                                  _lib.stream()), "b2_fredholm_apply")
-        else:
-            _lib.check(_lib.lib.b2_batched_gemm(_lib.ctx(), self.G.data_ptr(), xs.data_ptr(), yout.data_ptr(), self.nsl,
-                                                self.nx, self.ny, self.nz, int(adjoint), _lib.code(self._tdtype),
-                                                _lib.stream()), "b2_batched_gemm")
 
     def _apply_scatter(self, x: DistributedArray, adjoint: bool) -> DistributedArray:
         rank = self.rank
@@ -157,28 +152,16 @@ class MPIFredholm1(MPILinearOperator):
             y = DistributedArray(global_shape=self.shape[0], base_comm=x.base_comm, partition=Partition.SCATTER,
                                  local_shapes=[(int(n) * self.nx * self.nz,) for n in self.nsls], dtype=self._tdtype)
             if self.nsl:
-                self._local_product(xs, y.local_array, False)
+                self._product(xs.data_ptr(), y.local_array.data_ptr(), False)
             return y
         if x.partition is not Partition.SCATTER:
             raise ValueError(f"x should have partition={Partition.SCATTER} Got {x.partition} instead...")
         xl = x.local_array if x.local_array.dtype == self._tdtype else x.local_array.to(self._tdtype)
         if xl.numel() != self.nsl * self.nx * self.nz:
             raise ValueError("scattered data does not match this rank's slices")
-        pout = self.ny * self.nz
         y = DistributedArray(global_shape=self.shape[1], base_comm=x.base_comm, partition=Partition.BROADCAST,
                              dtype=self._tdtype)
-        yflat = y.local_array.view(-1)
-        mine = yflat[self.islstart[rank] * pout: self.islend[rank] * pout]
-        if self.nsl:
-            self._local_product(xl.reshape(-1), mine, True)
-        if x.size > 1:
-            import ctypes as C
-            comm = x.base_comm
-            counts = (C.c_size_t * comm.size)(*[int(n) * pout for n in self.nsls])
-            offs = (C.c_size_t * comm.size)(*[int(o) * pout for o in self.islstart])
-            _lib.check(_lib.lib.b2_allgatherv_at(comm.nccl, mine.data_ptr(), yflat.data_ptr(), counts, offs,
-                                                 _lib.code(self._tdtype), _lib.stream()), "b2_allgatherv_at")
-        return y
+        return self._product_gathered(xl.reshape(-1), y, True)
 
     def _apply(self, x: DistributedArray, adjoint: bool) -> DistributedArray:
         if self._scatter_data:
@@ -192,85 +175,18 @@ class MPIFredholm1(MPILinearOperator):
             # single rank, tensor-core plan: one library call (the 18.6 us apply is otherwise host-bound)
             n = self.shape[1] if adjoint else self.shape[0]
             y = DistributedArray._internal((n,), [(n,)], x.base_comm, self._tdtype, partition=x.partition)
-            _lib.check(_lib.lib.b2_fredholm_apply(self._plan, x._cont().data_ptr(), y.local_array.data_ptr(), None, 0,
-                                                  int(adjoint), _lib.stream()), "b2_fredholm_apply")
+            self._product(x._cont().data_ptr(), y.local_array.data_ptr(), adjoint)
             return y
         rank = self.rank
-        nin, nout = (self.nx, self.ny) if adjoint else (self.ny, self.nx)
+        per = (self.nx if adjoint else self.ny) * self.nz
+        xl = x.local_array if x.local_array.dtype == self._tdtype else x.local_array.to(self._tdtype)
+        xs = xl.reshape(-1)[self.islstart[rank] * per: self.islend[rank] * per]
         y = DistributedArray(global_shape=self.shape[1] if adjoint else self.shape[0],
                              base_comm=x.base_comm, partition=x.partition, dtype=self._tdtype)
-        xl = x.local_array
-        if xl.dtype != self._tdtype:
-            xl = xl.to(self._tdtype)
-        per = nin * self.nz
-        xs = xl.reshape(-1)[self.islstart[rank] * per: self.islend[rank] * per]
-        pout = nout * self.nz
-        yflat = y.local_array.view(-1)
-        ctx = _lib.ctx()
-        code = _lib.code(self._tdtype)
+        return self._product_gathered(xs, y, adjoint)
 
-        def product(s0, s1):
-            """slices [s0, s1) of this rank, written straight into their place in the gathered output"""
-            if s1 <= s0:
-                return
-            if self._plan is not None:      # whole-rank product on the tensor cores (nchunk == 1)
-                assert s0 == 0 and s1 == self.nsl
-                yout = yflat[self.islstart[rank] * pout:self.islend[rank] * pout]
-                _lib.check(_lib.lib.b2_fredholm_apply(self._plan, xs.data_ptr(), yout.data_ptr(), None, 0, int(adjoint),
-                                                      _lib.stream()), "b2_fredholm_apply")
-                return
-            G = self.G[s0:s1]
-            xin = xs[s0 * per:s1 * per]
-            yout = yflat[(self.islstart[rank] + s0) * pout:(self.islstart[rank] + s1) * pout]
-            _lib.check(_lib.lib.b2_batched_gemm(ctx, G.data_ptr(), xin.data_ptr(), yout.data_ptr(), s1 - s0,
-                                                self.nx, self.ny, self.nz, int(adjoint), code, _lib.stream()),
-                       "b2_batched_gemm")
+    def _matvec(self, x: DistributedArray) -> DistributedArray:
+        return self._apply(x, False)
 
-        if x.size == 1:
-            product(0, self.nsl)
-            return y
-        # chunked: gather chunk c over NVLink (side stream) while chunk c+1 is being computed
-        import ctypes as C
-        comm = x.base_comm
-        nchunk = 1   # 4 chunked gathers were slower than one (NCCL launch latency)
-        bounds = [[(c * n) // nchunk for c in range(nchunk + 1)] for n in self.nsls]
-        main = torch.cuda.current_stream()
-        side = _side_stream(xl.device)
-        comm.nccl
-        for c in range(nchunk):
-            product(bounds[rank][c], bounds[rank][c + 1])
-            ev = torch.cuda.Event()
-            ev.record(main)
-            counts = (C.c_size_t * comm.size)(*[(bounds[r][c + 1] - bounds[r][c]) * pout for r in range(comm.size)])
-            offs = (C.c_size_t * comm.size)(*[(int(self.islstart[r]) + bounds[r][c]) * pout for r in range(comm.size)])
-            mine = yflat[(int(self.islstart[rank]) + bounds[rank][c]) * pout:]
-            with torch.cuda.stream(side):
-                side.wait_event(ev)
-                _lib.check(_lib.lib.b2_allgatherv_at(comm.nccl, mine.data_ptr(), yflat.data_ptr(), counts, offs, code,
-                                                     _lib.stream()), "b2_allgatherv_at")
-        done = torch.cuda.Event()
-        done.record(side)
-        main.wait_event(done)
-        return y
-
-
-_SIDE = {}
-
-
-def _side_stream(device):
-    st = _SIDE.get(device)
-    if st is None:
-        st = _SIDE[device] = torch.cuda.Stream(device=device)
-    return st
-
-
-def _fr_matvec(self, x: DistributedArray) -> DistributedArray:
-    return self._apply(x, False)
-
-
-def _fr_rmatvec(self, x: DistributedArray) -> DistributedArray:
-    return self._apply(x, True)
-
-
-MPIFredholm1._matvec = _fr_matvec
-MPIFredholm1._rmatvec = _fr_rmatvec
+    def _rmatvec(self, x: DistributedArray) -> DistributedArray:
+        return self._apply(x, True)
