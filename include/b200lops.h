@@ -146,6 +146,12 @@ int b2_second_derivative_halo(int kind, int edge, int adjoint, int* need_lo, int
 int b2_derivative_axis(b2_ctx* ctx, const void* x, void* y, size_t n_outer, size_t n_axis, size_t n_inner,
                        int deriv, int kind, int order, int edge, double sampling, int adjoint, int dtype,
                        void* stream);
+/* rank-local 1-D convolution along the MIDDLE axis of a C-ordered [n_outer][n_axis][n_inner] block with nh real
+ * taps h (device pointer, same dtype as x); forward y[i] = sum_k h[k] x[i+offset-k], adjoint = exact transpose.
+ * pylops.signalprocessing.Convolve1D inside MPIBlockDiag (tutorials/reflectivity.py:74-76).  dtype F32 / F64
+ * (complex data: the real dtype and 2 * n_inner); 0 <= offset < nh, x != y; any nh is exact, nh > n_axis included */
+int b2_convolve_axis(b2_ctx* ctx, const void* x, void* y, size_t n_outer, size_t n_axis, size_t n_inner,
+                     const void* h, int nh, int offset, int adjoint, int dtype, void* stream);
 /* Peer-memory halo exchange fused INTO the stencil kernel (replaces the add_ghost_cells Send/Recv pairs of
  * DistributedArray.py:876-953 as used by FirstDerivative.py:221-247, 276-319 and SecondDerivative.py): every rank
  * owns a box of b2_halo_bytes(cap) bytes in IPC-mapped memory (b2_symm_alloc + b2_ipc_*); boxes_host[r] is rank r's

@@ -215,6 +215,80 @@ class SecondDerivative(_AxisDerivative):
         super().__init__(dims, axis=axis, sampling=sampling, kind=kind, edge=edge, order=3, dtype=dtype)
 
 
+class Convolve1D(LocalOperator):
+    """Rank-local 1-D convolution along ``axis`` of a C-ordered ``dims`` block with a stationary real filter ``h``:
+    the role of pylops.signalprocessing.Convolve1D inside MPIBlockDiag (tutorials/reflectivity.py:74-76).  For each
+    line ``x`` of length ``n`` along ``axis``::
+
+        y[i] = sum_k h[k] x[i + offset - k]  ==  np.convolve(x, h, "full")[offset:offset + n]
+
+    and the adjoint is the exact transpose (the same kernel with ``h`` reversed and offset ``nh - 1 - offset``).
+    One b2_convolve_axis launch per apply (csrc/convolve.cu).  ``method="fft"`` is accepted and computed by the
+    direct kernel: it is the same linear map, equal within rounding."""
+
+    def __init__(self, dims, h, offset: int = 0, axis: int = -1, method=None, dtype="float64"):
+        if method not in (None, "direct", "fft"):
+            raise ValueError("method must be None, 'direct' or 'fft'")
+        h = h.detach().cpu().numpy() if isinstance(h, torch.Tensor) else np.asarray(h)
+        if np.iscomplexobj(h):
+            raise NotImplementedError("complex filters are not supported")
+        if h.ndim != 1:
+            raise NotImplementedError("only stationary (1-D) filters are supported")
+        self.nh = int(h.size)
+        self.offset = int(offset)
+        if self.nh < 1 or not 0 <= self.offset <= self.nh - 1:
+            raise ValueError(f"offset must be in [0, nh - 1] = [0, {self.nh - 1}], got {offset}")
+        self.dims = tuple(int(d) for d in (dims if np.ndim(dims) else (dims,)))
+        self.axis = axis % len(self.dims)
+        self.method = method
+        n = int(np.prod(self.dims))
+        self.shape = (n, n)
+        self._tdtype = _lib.torch_dtype(dtype)
+        self.dtype = _lib.numpy_dtype(self._tdtype)
+        _lib.ctx()
+        # taps in both real precisions, uploaded once
+        self._h = {t: torch.as_tensor(h.astype(_lib.numpy_dtype(t))).to("cuda") for t in (torch.float32, torch.float64)}
+
+    def _apply(self, x: torch.Tensor, adjoint: int, out=None) -> torch.Tensor:
+        x = x.reshape(-1)
+        tdt = self._tdtype
+        if x.dtype.is_complex and not tdt.is_complex:
+            tdt = _CPLX_OF[torch.promote_types(tdt, _REAL_OF[x.dtype])]     # real taps on complex data
+        if x.dtype != tdt:
+            x = x.to(tdt)
+        if not x.is_contiguous():
+            x = x.contiguous()
+        if x.numel() != self.shape[1]:
+            raise ValueError(f"dimension mismatch: operator {self.shape}, vector {x.numel()}")
+        direct = (out is not None and out.dtype == tdt and out.is_contiguous() and out.numel() == x.numel()
+                  and out.data_ptr() != x.data_ptr())
+        y = out if direct else torch.empty_like(x)
+        n_outer = int(np.prod(self.dims[:self.axis])) if self.axis else 1
+        n_axis = self.dims[self.axis]
+        n_inner = int(np.prod(self.dims[self.axis + 1:])) if self.axis + 1 < len(self.dims) else 1
+        real = _REAL_OF.get(tdt, tdt)
+        if tdt.is_complex:
+            n_inner *= 2                                  # (re, im) pairs: the same real map on both parts
+        _lib.check(_lib.lib.b2_convolve_axis(_lib.ctx(), x.data_ptr(), y.data_ptr(), n_outer, n_axis, n_inner,
+                                             self._h[real].data_ptr(), self.nh, self.offset, adjoint,
+                                             _lib.code(real), _lib.stream()), "b2_convolve_axis")
+        if out is not None and not direct:
+            return _store(out, y)
+        return y
+
+    def _matvec(self, x, out=None):
+        return self._apply(x, 0, out)
+
+    def _rmatvec(self, x, out=None):
+        return self._apply(x, 1, out)
+
+    def matvec(self, x, out=None):
+        return self._apply(x, 0, out)
+
+    def rmatvec(self, x, out=None):
+        return self._apply(x, 1, out)
+
+
 class FFT(LocalOperator):
     """Rank-local real FFT along ``axis`` of a ``dims`` block -- the role of third-party
     ``pylops.signalprocessing.FFT(dims, axis, real=True, ifftshift_before=..., norm="ortho")`` inside
