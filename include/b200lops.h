@@ -152,6 +152,13 @@ int b2_derivative_axis(b2_ctx* ctx, const void* x, void* y, size_t n_outer, size
  * (complex data: the real dtype and 2 * n_inner); 0 <= offset < nh, x != y; any nh is exact, nh > n_axis included */
 int b2_convolve_axis(b2_ctx* ctx, const void* x, void* y, size_t n_outer, size_t n_axis, size_t n_inner,
                      const void* h, int nh, int offset, int adjoint, int dtype, void* stream);
+/* rank-local post-stack modelling along the MIDDLE axis of the same block: pylops.avo.poststack.
+ * PoststackLinearModelling, y = C D x with D the first derivative along the axis (FirstDerivative, edge=False,
+ * sampling=1, kind B2_FD_CENTERED or B2_FD_FORWARD) and C the convolution of b2_convolve_axis; adjoint x = D^T C^T y.
+ * One launch; equals b2_derivative_axis then b2_convolve_axis (adjoint: the reverse) bit for bit.  Arguments and
+ * error codes as b2_convolve_axis, plus B2_ERR_ARG for any other kind; y is untouched on every error */
+int b2_poststack_axis(b2_ctx* ctx, const void* x, void* y, size_t n_outer, size_t n_axis, size_t n_inner,
+                      const void* h, int nh, int offset, int kind, int adjoint, int dtype, void* stream);
 /* Peer-memory halo exchange fused INTO the stencil kernel (replaces the add_ghost_cells Send/Recv pairs of
  * DistributedArray.py:876-953 as used by FirstDerivative.py:221-247, 276-319 and SecondDerivative.py): every rank
  * owns a box of b2_halo_bytes(cap) bytes in IPC-mapped memory (b2_symm_alloc + b2_ipc_*); boxes_host[r] is rank r's

@@ -10,6 +10,16 @@
 // Every thread produces R consecutive outputs from a rolling register window: each 16-byte shared-memory read
 // feeds R*R (innermost) or RT*RT*V (middle axis) FMAs.  Tap chunks and taps within a chunk are summed in a fixed
 // order, so repeated applies give identical bits.
+//
+// The same kernel bodies also run pylops.avo.poststack.PoststackLinearModelling, C D with D the first derivative
+// along the axis (FirstDerivative, edge=False, sampling=1), through a compile-time derivative stage DS:
+//   DS_FWD  y = C D x: the loader stages x with one extra sample on each side and turns it into d = D x in shared
+//           memory; the correlation then runs unchanged on d.
+//   DS_ADJ  x = D^T C^T y: the correlation computes e = C^T y on the tile plus one neighbour on each side, and the
+//           epilogue applies D^T to e from shared memory.
+// d and D^T e use the stencil kernel's arithmetic (stencil.cu: non-zero taps in ascending offset order, each an fma
+// into an accumulator that starts at 0), and e the same tap chunks as b2_convolve_axis, so the fused operator
+// equals the two-launch chain b2_derivative_axis + b2_convolve_axis bit for bit.
 #include "common.cuh"
 
 namespace {
@@ -18,11 +28,40 @@ constexpr int CV_THREADS = 256;
 constexpr int CV_KC_LINE = 128;              // taps per chunk, innermost axis
 constexpr int CV_KC_MID = 64;                // taps per chunk, middle axis
 constexpr size_t CV_SMEM_BUDGET = 32 * 1024; // bytes of staged windows per CTA (packed short lines)
+constexpr int DS_NONE = 0, DS_FWD = 1, DS_ADJ = 2;   // derivative stage: none, D before C, D^T after C^T
 
 // V consecutive elements, aligned to their size so that shared-memory reads of a whole vector compile to one
 // LDS.64 / LDS.128 (Vec16 is only element-aligned: the compiler would split it into conflicting scalar reads)
 template <typename T, int V>
 struct alignas(V * sizeof(T)) VecN { T v[V]; };
+
+// (D x)[j] from x[j-1], x[j], x[j+1] on a line of n samples: 0.5 (x[j+1] - x[j-1]) on [1, n-2] (centered) or
+// x[j+1] - x[j] on [0, n-2] (forward), zero elsewhere
+template <typename T>
+__device__ __forceinline__ T fd_fwd(T xm, T x0, T xp, long long j, long long n, int kind) {
+  T acc = T(0);
+  if (kind == B2_FD_CENTERED) {
+    if (j >= 1 && j <= n - 2) { acc = fma(T(-0.5), xm, acc); acc = fma(T(0.5), xp, acc); }
+  } else if (j >= 0 && j <= n - 2) {
+    acc = fma(T(-1), x0, acc);
+    acc = fma(T(1), xp, acc);
+  }
+  return acc;
+}
+
+// (D^T e)[i] from e[i-1], e[i], e[i+1]: row i of the transpose, whose taps come from the forward rows i-1, i, i+1
+template <typename T>
+__device__ __forceinline__ T fd_adj(T em, T e0, T ep, long long i, long long n, int kind) {
+  T acc = T(0);
+  if (kind == B2_FD_CENTERED) {
+    if (i - 1 >= 1 && i - 1 <= n - 2) acc = fma(T(0.5), em, acc);
+    if (i + 1 >= 1 && i + 1 <= n - 2) acc = fma(T(-0.5), ep, acc);
+  } else {
+    if (i >= 1 && i - 1 <= n - 2) acc = fma(T(1), em, acc);
+    if (i <= n - 2) acc = fma(T(-1), e0, acc);
+  }
+  return acc;
+}
 
 // ---- innermost axis (n_inner == 1) ----------------------------------------------------------------------------
 // A CTA covers L lines x S outputs (S = R * ceil(n / R) capped at the tile, L = tile / S when lines are short).
@@ -40,13 +79,20 @@ __device__ __forceinline__ T tap(const T* __restrict__ h, int k, int nh, int adj
   return k < nh ? __ldg(h + (adjoint ? nh - 1 - k : k)) : T(0);
 }
 
-template <typename T>
-__global__ void __launch_bounds__(CV_THREADS)
-conv_line_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restrict__ h, const LineParams p) {
+// DS_FWD: the window of x, one sample wider on each side, is staged in a second buffer after the L windows and
+// turned into d.  DS_ADJ: a tile's outputs only need e on [i0 - 1, i0 + S]; when a line spans several tiles
+// (then L == 1) thread 0 computes e[i0 - 1] and the last thread e[i0 + S], with the same tap order as the others,
+// so the 16-byte tile geometry and stores of the plain convolution are kept.
+template <typename T, int DS>
+__device__ __forceinline__ void conv_line(const T* __restrict__ x, T* __restrict__ y, const T* __restrict__ h,
+                                          const LineParams p, const int kind) {
   constexpr int R = Vec16<T>::N;
+  constexpr int XH = DS == DS_FWD ? 1 : 0;  // extra staged samples on each side of the window
   extern __shared__ __align__(16) unsigned char cv_smem[];
   T* g = reinterpret_cast<T*>(cv_smem);     // kc reversed taps (kc is a multiple of R: w stays 16-byte aligned)
   T* w = g + p.kc;                          // L windows of W elements
+  T* xs = DS == DS_FWD ? w + p.L * p.W : w; // DS_FWD: L windows of x of W + 2 elements
+  const int Ws = p.W + 2 * XH;
   const long long grp = (long long)blockIdx.x / p.tiles;
   const long long i0 = ((long long)blockIdx.x - grp * p.tiles) * p.S;
   const long long line0 = grp * p.L;
@@ -57,16 +103,18 @@ conv_line_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restrict
   T acc[R];
 #pragma unroll
   for (int r = 0; r < R; ++r) acc[r] = T(0);
+  T hlo = T(0), hhi = T(0);                 // DS_ADJ: e[i0 - 1] (thread 0), e[i0 + S] (last thread)
 
   for (int k0 = 0; k0 < p.nh; k0 += p.kc) {
     __syncthreads();                                   // the previous chunk's readers are done
     for (int q = threadIdx.x; q < p.kc; q += CV_THREADS) g[q] = tap(h, k0 + p.kc - 1 - q, p.nh, p.adjoint);
     const long long b = i0 + p.off - k0 - p.kc + 1;    // line index of w[0]
+    const long long bs = b - XH;                       // line index of xs[0]
     if (p.vec) {
       // one line per CTA, 16-byte aligned line: aligned vector loads of the R-blocks covering the window
       const T* xl = x + line0 * p.n;
-      const long long a = b >= 0 ? b / R * R : -((-b + R - 1) / R) * R;
-      const int nv = (int)((b + p.W - a + R - 1) / R);
+      const long long a = bs >= 0 ? bs / R * R : -((-bs + R - 1) / R) * R;
+      const int nv = (int)((bs + Ws - a + R - 1) / R);
       for (int v = threadIdx.x; v < nv; v += CV_THREADS) {
         const long long j0 = a + (long long)v * R;
         Vec16<T> o;
@@ -76,16 +124,25 @@ conv_line_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restrict
           for (int e = 0; e < R; ++e) o.v[e] = (j0 + e >= 0 && j0 + e < p.n) ? __ldg(xl + j0 + e) : T(0);
 #pragma unroll
         for (int e = 0; e < R; ++e) {
-          const long long m = j0 + e - b;
-          if (m >= 0 && m < p.W) w[m] = o.v[e];
+          const long long m = j0 + e - bs;
+          if (m >= 0 && m < Ws) xs[m] = o.v[e];
         }
       }
     } else {
+      const int tot = nl * Ws;
+      for (int e = threadIdx.x; e < tot; e += CV_THREADS) {
+        const int ll = e / Ws, m = e - ll * Ws;
+        const long long j = bs + m;
+        xs[e] = (j >= 0 && j < p.n) ? __ldg(x + (line0 + ll) * p.n + j) : T(0);
+      }
+    }
+    if constexpr (DS == DS_FWD) {
+      __syncthreads();
       const int tot = nl * p.W;
       for (int e = threadIdx.x; e < tot; e += CV_THREADS) {
         const int ll = e / p.W, m = e - ll * p.W;
-        const long long j = b + m;
-        w[e] = (j >= 0 && j < p.n) ? __ldg(x + (line0 + ll) * p.n + j) : T(0);
+        const T* s = xs + ll * Ws + m;                 // x[b + m - 1], x[b + m], x[b + m + 1]
+        w[e] = fd_fwd(s[0], s[1], s[2], b + m, p.n, kind);
       }
     }
     __syncthreads();
@@ -104,6 +161,28 @@ conv_line_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restrict
         lo = hi;
       }
     }
+    if constexpr (DS == DS_ADJ) {
+      if (p.tiles > 1 && threadIdx.x == 0) {           // e[i0 - 1] = sum_q g[q] w[q - 1], w[-1] = x[b - 1]
+        const T* xl = x + line0 * p.n;
+        hlo = fma(g[0], (b - 1 >= 0 && b - 1 < p.n) ? __ldg(xl + b - 1) : T(0), hlo);
+        for (int q = 1; q < p.kc; ++q) hlo = fma(g[q], w[q - 1], hlo);
+      } else if (p.tiles > 1 && threadIdx.x == CV_THREADS - 1) {   // e[i0 + S] = sum_q g[q] w[S + q]
+        for (int q = 0; q < p.kc; ++q) hhi = fma(g[q], w[p.S + q], hhi);
+      }
+    }
+  }
+  if constexpr (DS == DS_ADJ) {
+    __syncthreads();                                   // the window is free: it now holds e
+    T* e = w + l * p.W + 1;                            // e[t] = e[i0 + t] of this thread's line, t in [-1, S]
+    if (active)
+#pragma unroll
+      for (int r = 0; r < R; ++r) e[li + r] = acc[r];
+    if (p.tiles > 1 && threadIdx.x == 0) w[0] = hlo;
+    if (p.tiles > 1 && threadIdx.x == CV_THREADS - 1) w[p.S + 1] = hhi;
+    __syncthreads();
+    if (active)
+#pragma unroll
+      for (int r = 0; r < R; ++r) acc[r] = fd_adj(e[li + r - 1], e[li + r], e[li + r + 1], i0 + li + r, p.n, kind);
   }
   if (!active) return;
   const long long i = i0 + li;
@@ -118,6 +197,19 @@ conv_line_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restrict
     for (int r = 0; r < R; ++r)
       if (i + r < p.n) __stcs(yp + r, acc[r]);
   }
+}
+
+template <typename T>
+__global__ void __launch_bounds__(CV_THREADS)
+conv_line_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restrict__ h, const LineParams p) {
+  conv_line<T, DS_NONE>(x, y, h, p, 0);
+}
+
+template <typename T, int DS>
+__global__ void __launch_bounds__(CV_THREADS)
+poststack_line_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restrict__ h, const LineParams p,
+                      const int kind) {
+  conv_line<T, DS>(x, y, h, p, kind);
 }
 
 // ---- middle axis (n_inner > 1) --------------------------------------------------------------------------------
@@ -140,15 +232,18 @@ __device__ __forceinline__ VecN<T, V> ld_vec(const T* p) {
   return o;
 }
 
-template <typename T, int V>
-__global__ void __launch_bounds__(MID_LANES * MID_GROUPS)
-conv_mid_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restrict__ h, const MidParams p) {
+template <typename T, int V, int DS>
+__device__ __forceinline__ void conv_mid(const T* __restrict__ x, T* __restrict__ y, const T* __restrict__ h,
+                                         const MidParams p, const int kind) {
   constexpr int COLS = MID_LANES * V;
+  constexpr int XH = DS == DS_FWD ? 1 : 0;  // extra staged rows on each side of the window
+  constexpr int EH = DS == DS_ADJ ? 1 : 0;  // e rows computed on each side of the stored rows
+  constexpr int RO = MID_RB - 2 * EH;       // rows stored per tile
   extern __shared__ __align__(16) unsigned char cv_smem[];
   T* g = reinterpret_cast<T*>(cv_smem);     // kc taps (kc is a multiple of MID_RT)
   VecN<T, V>* w = reinterpret_cast<VecN<T, V>*>(g + p.kc);   // (RB + kc) rows x MID_LANES vectors
   const long long ct = (long long)blockIdx.x % p.ctiles;
-  const long long r0 = ((long long)blockIdx.x / p.ctiles) * MID_RB;
+  const long long r0 = ((long long)blockIdx.x / p.ctiles) * RO - EH;   // first row computed
   const size_t plane = (size_t)p.n * (size_t)p.ni;
   x += (size_t)blockIdx.y * plane;
   y += (size_t)blockIdx.y * plane;
@@ -162,18 +257,30 @@ conv_mid_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restrict_
     for (int e = 0; e < V; ++e) acc[r][e] = T(0);
 
   const int rows = MID_RB + p.kc;
+  VecN<T, V>* xs = DS == DS_FWD ? w + rows * MID_LANES : w;   // DS_FWD: rows + 2 rows of x
   for (int k0 = 0; k0 < p.nh; k0 += p.kc) {
     __syncthreads();
     for (int q = tid; q < p.kc; q += MID_LANES * MID_GROUPS) g[q] = tap(h, k0 + p.kc - 1 - q, p.nh, p.adjoint);
     const long long b = r0 + p.off - k0 - p.kc + 1;     // axis index of staged row 0
-    for (int m = grp; m < rows; m += MID_GROUPS) {
-      const long long j = b + m;
+    for (int m = grp; m < rows + 2 * XH; m += MID_GROUPS) {
+      const long long j = b - XH + m;
       VecN<T, V> v;
       if (col_ok && j >= 0 && j < p.n) v = ld_vec<T, V>(x + (size_t)j * p.ni + c);
       else
 #pragma unroll
         for (int e = 0; e < V; ++e) v.v[e] = T(0);
-      w[m * MID_LANES + lane] = v;
+      xs[m * MID_LANES + lane] = v;
+    }
+    if constexpr (DS == DS_FWD) {
+      __syncthreads();
+      for (int m = grp; m < rows; m += MID_GROUPS) {
+        const VecN<T, V>* s = xs + m * MID_LANES + lane;   // rows b + m - 1, b + m, b + m + 1
+        const VecN<T, V> a = s[0], o = s[MID_LANES], z = s[2 * MID_LANES];
+        VecN<T, V> d;
+#pragma unroll
+        for (int e = 0; e < V; ++e) d.v[e] = fd_fwd(a.v[e], o.v[e], z.v[e], b + m, p.n, kind);
+        w[m * MID_LANES + lane] = d;
+      }
     }
     __syncthreads();
     const VecN<T, V>* wl = w + (grp * MID_RT) * MID_LANES + lane;
@@ -197,11 +304,28 @@ conv_mid_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restrict_
       for (int r = 0; r < MID_RT; ++r) lo[r] = hi[r];
     }
   }
+  if constexpr (DS == DS_ADJ) {
+    __syncthreads();                                    // the window is free: row t of it now holds e[r0 + t]
+#pragma unroll
+    for (int r = 0; r < MID_RT; ++r)
+#pragma unroll
+      for (int e = 0; e < V; ++e) w[(grp * MID_RT + r) * MID_LANES + lane].v[e] = acc[r][e];
+    __syncthreads();
+#pragma unroll
+    for (int r = 0; r < MID_RT; ++r) {
+      const int t = grp * MID_RT + r;
+      if (t == 0 || t == MID_RB - 1) continue;
+      const VecN<T, V> a = w[(t - 1) * MID_LANES + lane], o = w[t * MID_LANES + lane], z = w[(t + 1) * MID_LANES + lane];
+#pragma unroll
+      for (int e = 0; e < V; ++e) acc[r][e] = fd_adj(a.v[e], o.v[e], z.v[e], r0 + t, p.n, kind);
+    }
+  }
   if (!col_ok) return;
 #pragma unroll
   for (int r = 0; r < MID_RT; ++r) {
     const long long i = r0 + grp * MID_RT + r;
     if (i >= p.n) break;
+    if (DS == DS_ADJ && (grp * MID_RT + r == 0 || grp * MID_RT + r == MID_RB - 1)) continue;
     T* yp = y + (size_t)i * p.ni + c;
     if constexpr (V * sizeof(T) == 16) {
       store_vec(yp, *reinterpret_cast<const Vec16<T>*>(&acc[r][0]));
@@ -212,17 +336,31 @@ conv_mid_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restrict_
   }
 }
 
+template <typename T, int V>
+__global__ void __launch_bounds__(MID_LANES * MID_GROUPS)
+conv_mid_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restrict__ h, const MidParams p) {
+  conv_mid<T, V, DS_NONE>(x, y, h, p, 0);
+}
+
+template <typename T, int V, int DS>
+__global__ void __launch_bounds__(MID_LANES * MID_GROUPS)
+poststack_mid_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restrict__ h, const MidParams p,
+                     const int kind) {
+  conv_mid<T, V, DS>(x, y, h, p, kind);
+}
+
 inline int round_up(int v, int m) { return (v + m - 1) / m * m; }
 
-template <typename T>
-int launch_line(const T* x, T* y, const T* h, size_t n_lines, size_t n, int nh, int off, int adjoint,
+template <typename T, int DS>
+int launch_line(const T* x, T* y, const T* h, size_t n_lines, size_t n, int nh, int off, int adjoint, int kind,
                 cudaStream_t st) {
   constexpr int R = Vec16<T>::N, TILE = CV_THREADS * R;
   LineParams p;
   p.kc = round_up(nh < CV_KC_LINE ? nh : CV_KC_LINE, R);
   p.S = (int)(n < (size_t)TILE ? round_up((int)n, R) : TILE);
   p.W = p.S + p.kc;
-  const int fit = (int)((CV_SMEM_BUDGET / sizeof(T) - p.kc) / p.W);
+  const int per_line = DS == DS_FWD ? 2 * p.W + 2 : p.W;      // DS_FWD also stages x, W + 2 per line
+  const int fit = (int)((CV_SMEM_BUDGET / sizeof(T) - p.kc) / per_line);
   p.L = TILE / p.S < fit ? TILE / p.S : fit;
   if (p.L < 1) p.L = 1;
   p.n = (long long)n;
@@ -231,23 +369,26 @@ int launch_line(const T* x, T* y, const T* h, size_t n_lines, size_t n, int nh, 
   p.off = off;
   p.adjoint = adjoint;
   p.vec = p.L == 1 && n % R == 0 && b2_aligned16(x);
-  const size_t smem = ((size_t)p.kc + (size_t)p.L * p.W) * sizeof(T);
+  const size_t smem = ((size_t)p.kc + (size_t)p.L * per_line) * sizeof(T);
   const size_t max_groups = (size_t)(0x7fffffffLL / p.tiles);
   const size_t lines_per_launch = (max_groups / p.L) * p.L;
   for (size_t done = 0; done < n_lines; done += lines_per_launch) {
     const size_t cnt = n_lines - done < lines_per_launch ? n_lines - done : lines_per_launch;
     p.nlines = (long long)cnt;
     const size_t blocks = (cnt + p.L - 1) / p.L * (size_t)p.tiles;
-    conv_line_kernel<T><<<(unsigned)blocks, CV_THREADS, smem, st>>>(x + done * n, y + done * n, h, p);
+    if constexpr (DS == DS_NONE)
+      conv_line_kernel<T><<<(unsigned)blocks, CV_THREADS, smem, st>>>(x + done * n, y + done * n, h, p);
+    else
+      poststack_line_kernel<T, DS><<<(unsigned)blocks, CV_THREADS, smem, st>>>(x + done * n, y + done * n, h, p, kind);
     B2_LAUNCH_CHECK();
   }
   return B2_OK;
 }
 
-template <typename T, int V>
+template <typename T, int V, int DS>
 int launch_mid_v(const T* x, T* y, const T* h, size_t n_outer, size_t n, size_t ni, int nh, int off, int adjoint,
-                 cudaStream_t st) {
-  constexpr int COLS = MID_LANES * V;
+                 int kind, cudaStream_t st) {
+  constexpr int COLS = MID_LANES * V, RO = DS == DS_ADJ ? MID_RB - 2 : MID_RB;   // rows stored per tile
   MidParams p;
   p.kc = round_up(nh < CV_KC_MID ? nh : CV_KC_MID, MID_RT);
   p.n = (long long)n;
@@ -256,31 +397,52 @@ int launch_mid_v(const T* x, T* y, const T* h, size_t n_outer, size_t n, size_t 
   p.nh = nh;
   p.off = off;
   p.adjoint = adjoint;
-  const long long nblk = p.ctiles * (long long)((n + MID_RB - 1) / MID_RB);
+  const long long nblk = p.ctiles * (long long)((n + RO - 1) / RO);
   if (nblk > 0x7fffffffLL) return B2_ERR_ARG;
-  const size_t smem = (size_t)p.kc * sizeof(T) + (size_t)(MID_RB + p.kc) * MID_LANES * V * sizeof(T);
+  const size_t rows = (size_t)(MID_RB + p.kc) + (DS == DS_FWD ? MID_RB + p.kc + 2 : 0);   // DS_FWD: + rows of x
+  const size_t smem = (size_t)p.kc * sizeof(T) + rows * MID_LANES * V * sizeof(T);
+  if constexpr (DS != DS_NONE) {
+    // DS_FWD with kc > 20 taps needs more than the default 48 KB (set once, before the first such launch)
+    static size_t smem_opt_in = 48 * 1024;
+    if (smem > smem_opt_in) {
+      const cudaError_t e = cudaFuncSetAttribute(poststack_mid_kernel<T, V, DS>,
+                                                 cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+      if (e != cudaSuccess) return (int)e;
+      smem_opt_in = smem;
+    }
+  }
   const dim3 block(MID_LANES, MID_GROUPS);
   for (size_t done = 0; done < n_outer; done += 65535) {
     const unsigned cnt = (unsigned)(n_outer - done < 65535 ? n_outer - done : 65535);
     const size_t o = done * n * ni;
-    conv_mid_kernel<T, V><<<dim3((unsigned)nblk, cnt), block, smem, st>>>(x + o, y + o, h, p);
+    if constexpr (DS == DS_NONE)
+      conv_mid_kernel<T, V><<<dim3((unsigned)nblk, cnt), block, smem, st>>>(x + o, y + o, h, p);
+    else
+      poststack_mid_kernel<T, V, DS><<<dim3((unsigned)nblk, cnt), block, smem, st>>>(x + o, y + o, h, p, kind);
     B2_LAUNCH_CHECK();
   }
   return B2_OK;
 }
 
-template <typename T>
+template <typename T, int DS>
 int launch_conv(const void* xv, void* yv, const void* hv, size_t n_outer, size_t n, size_t ni, int nh, int off,
-                int adjoint, cudaStream_t st) {
+                int adjoint, int kind, cudaStream_t st) {
   const T* x = static_cast<const T*>(xv);
   T* y = static_cast<T*>(yv);
   const T* h = static_cast<const T*>(hv);
   if (adjoint) off = nh - 1 - off;     // exact transpose: reversed taps (read in the kernel), mirrored offset
-  if (ni == 1) return launch_line<T>(x, y, h, n_outer, n, nh, off, adjoint, st);
+  if (ni == 1) return launch_line<T, DS>(x, y, h, n_outer, n, nh, off, adjoint, kind, st);
   constexpr int V = Vec16<T>::N;
   if (ni % V == 0 && b2_aligned16(x) && b2_aligned16(y))
-    return launch_mid_v<T, V>(x, y, h, n_outer, n, ni, nh, off, adjoint, st);
-  return launch_mid_v<T, 1>(x, y, h, n_outer, n, ni, nh, off, adjoint, st);
+    return launch_mid_v<T, V, DS>(x, y, h, n_outer, n, ni, nh, off, adjoint, kind, st);
+  return launch_mid_v<T, 1, DS>(x, y, h, n_outer, n, ni, nh, off, adjoint, kind, st);
+}
+
+template <typename T>
+int launch_poststack(const void* x, void* y, const void* h, size_t n_outer, size_t n, size_t ni, int nh, int off,
+                     int kind, int adjoint, cudaStream_t st) {
+  return adjoint ? launch_conv<T, DS_ADJ>(x, y, h, n_outer, n, ni, nh, off, 1, kind, st)
+                 : launch_conv<T, DS_FWD>(x, y, h, n_outer, n, ni, nh, off, 0, kind, st);
 }
 
 }  // namespace
@@ -292,6 +454,19 @@ extern "C" int b2_convolve_axis(b2_ctx* ctx, const void* x, void* y, size_t n_ou
   if (n_outer == 0 || n_axis == 0 || n_inner == 0) return B2_OK;
   if (!x || !y || x == y) return B2_ERR_ARG;
   cudaStream_t st = (cudaStream_t)stream;
-  return dtype == B2_F32 ? launch_conv<float>(x, y, h, n_outer, n_axis, n_inner, nh, offset, adjoint, st)
-                         : launch_conv<double>(x, y, h, n_outer, n_axis, n_inner, nh, offset, adjoint, st);
+  return dtype == B2_F32
+             ? launch_conv<float, DS_NONE>(x, y, h, n_outer, n_axis, n_inner, nh, offset, adjoint, 0, st)
+             : launch_conv<double, DS_NONE>(x, y, h, n_outer, n_axis, n_inner, nh, offset, adjoint, 0, st);
+}
+
+extern "C" int b2_poststack_axis(b2_ctx* ctx, const void* x, void* y, size_t n_outer, size_t n_axis, size_t n_inner,
+                                 const void* h, int nh, int offset, int kind, int adjoint, int dtype, void* stream) {
+  if (!ctx || nh < 1 || offset < 0 || offset > nh - 1 || !h) return B2_ERR_ARG;
+  if (kind != B2_FD_CENTERED && kind != B2_FD_FORWARD) return B2_ERR_ARG;
+  if (dtype != B2_F32 && dtype != B2_F64) return B2_ERR_DTYPE;
+  if (n_outer == 0 || n_axis == 0 || n_inner == 0) return B2_OK;
+  if (!x || !y || x == y) return B2_ERR_ARG;
+  cudaStream_t st = (cudaStream_t)stream;
+  return dtype == B2_F32 ? launch_poststack<float>(x, y, h, n_outer, n_axis, n_inner, nh, offset, kind, adjoint, st)
+                         : launch_poststack<double>(x, y, h, n_outer, n_axis, n_inner, nh, offset, kind, adjoint, st);
 }

@@ -59,7 +59,9 @@ def _store(out: torch.Tensor, y: torch.Tensor) -> torch.Tensor:
 
 
 class LocalOperator:
-    """minimal rank-local linear operator interface"""
+    """minimal rank-local linear operator interface.  ``A.H`` is the adjoint; ``A @ B`` and ``A * B`` between local
+    operators are the product (applied right to left), in which ``T.H @ X @ T`` with ``T`` a :class:`Transpose` and
+    ``X`` an axis operator on ``T``'s output dims is folded into ``X`` along the matching axis of ``T``'s input"""
     shape = (0, 0)
     dtype = np.float64
 
@@ -75,6 +77,88 @@ class LocalOperator:
 
     def _rmatvec(self, x):
         raise NotImplementedError
+
+    @property
+    def H(self) -> "LocalOperator":
+        return _LocalAdjoint(self)
+
+    def __matmul__(self, other):
+        if not isinstance(other, LocalOperator):
+            return NotImplemented
+        return _product(self, other)
+
+    __mul__ = __matmul__
+
+
+class _LocalAdjoint(LocalOperator):
+    """``A.H`` of a rank-local operator: its matvec is ``A.rmatvec`` and the reverse"""
+
+    def __init__(self, op: LocalOperator):
+        self.op = op
+        self.shape = (op.shape[1], op.shape[0])
+        self.dtype = op.dtype
+
+    @property
+    def H(self) -> LocalOperator:
+        return self.op
+
+    def _matvec(self, x):
+        return self.op.rmatvec(x)
+
+    def _rmatvec(self, x):
+        return self.op.matvec(x)
+
+
+class _LocalProduct(LocalOperator):
+    """``ops[0] @ ops[1] @ ... @ ops[-1]`` applied right to left, one operator at a time (eager)"""
+
+    def __init__(self, ops):
+        for a, b in zip(ops[:-1], ops[1:]):
+            if a.shape[1] != b.shape[0]:
+                raise ValueError(f"dimension mismatch in product: {a.shape} @ {b.shape}")
+        self.ops = list(ops)
+        self.shape = (ops[0].shape[0], ops[-1].shape[1])
+        self.dtype = np.result_type(*[op.dtype for op in ops])
+
+    @property
+    def H(self) -> LocalOperator:
+        return _product(*[op.H for op in reversed(self.ops)])
+
+    def _matvec(self, x):
+        for op in reversed(self.ops):
+            x = op.matvec(x)
+        return x
+
+    def _rmatvec(self, x):
+        for op in self.ops:
+            x = op.rmatvec(x)
+        return x
+
+
+def _fold(t_inv, op, t) -> "LocalOperator | None":
+    """``T.H @ X @ T`` as one operator: ``X`` along axis ``T.axes[X.axis]`` of ``T.dims`` (no transposes), when
+    ``t`` is a Transpose, ``t_inv`` its inverse and ``op`` an axis operator on ``t``'s output dims; else None"""
+    if not (isinstance(t, Transpose) and isinstance(t_inv, Transpose) and isinstance(op, _AXIS_OPERATORS)):
+        return None
+    if t_inv.dims != t.dimsd or t_inv.axes != tuple(int(a) for a in np.argsort(t.axes)) or op.dims != t.dimsd:
+        return None
+    return op._along(t.dims, t.axes[op.axis])
+
+
+def _product(*ops) -> LocalOperator:
+    """product of rank-local operators, flattened, with every ``T.H @ X @ T`` folded"""
+    flat = []
+    for op in ops:
+        flat.extend(op.ops if isinstance(op, _LocalProduct) else [op])
+    i = 0
+    while i + 2 < len(flat):
+        f = _fold(*flat[i:i + 3])
+        if f is None:
+            i += 1
+        else:
+            flat[i:i + 3] = [f]
+            i = max(i - 2, 0)
+    return flat[0] if len(flat) == 1 else _LocalProduct(flat)
 
 
 class MatrixMult(LocalOperator):
@@ -161,6 +245,10 @@ class _AxisDerivative(LocalOperator):
         self._tdtype = _lib.torch_dtype(dtype)
         self.dtype = _lib.numpy_dtype(self._tdtype)
         _lib.ctx()
+
+    def _along(self, dims, axis):
+        """the same operator on a ``dims`` block along ``axis`` (``prod(dims)`` unchanged)"""
+        return _along(self, dims, axis)
 
     def _apply(self, x: torch.Tensor, adjoint: int, out=None) -> torch.Tensor:
         x = x.reshape(-1)
@@ -249,6 +337,15 @@ class Convolve1D(LocalOperator):
         # taps in both real precisions, uploaded once
         self._h = {t: torch.as_tensor(h.astype(_lib.numpy_dtype(t))).to("cuda") for t in (torch.float32, torch.float64)}
 
+    def _along(self, dims, axis):
+        """the same operator on a ``dims`` block along ``axis`` (``prod(dims)`` unchanged)"""
+        return _along(self, dims, axis)
+
+    def _launch(self, x, y, n_outer, n_axis, n_inner, real, adjoint):
+        _lib.check(_lib.lib.b2_convolve_axis(_lib.ctx(), x.data_ptr(), y.data_ptr(), n_outer, n_axis, n_inner,
+                                             self._h[real].data_ptr(), self.nh, self.offset, adjoint,
+                                             _lib.code(real), _lib.stream()), "b2_convolve_axis")
+
     def _apply(self, x: torch.Tensor, adjoint: int, out=None) -> torch.Tensor:
         x = x.reshape(-1)
         tdt = self._tdtype
@@ -269,9 +366,7 @@ class Convolve1D(LocalOperator):
         real = _REAL_OF.get(tdt, tdt)
         if tdt.is_complex:
             n_inner *= 2                                  # (re, im) pairs: the same real map on both parts
-        _lib.check(_lib.lib.b2_convolve_axis(_lib.ctx(), x.data_ptr(), y.data_ptr(), n_outer, n_axis, n_inner,
-                                             self._h[real].data_ptr(), self.nh, self.offset, adjoint,
-                                             _lib.code(real), _lib.stream()), "b2_convolve_axis")
+        self._launch(x, y, n_outer, n_axis, n_inner, real, adjoint)
         if out is not None and not direct:
             return _store(out, y)
         return y
@@ -287,6 +382,78 @@ class Convolve1D(LocalOperator):
 
     def rmatvec(self, x, out=None):
         return self._apply(x, 1, out)
+
+
+class PoststackLinearModelling(Convolve1D):
+    """Rank-local post-stack seismic modelling, pylops.avo.poststack.PoststackLinearModelling (pylops 2.x) for a
+    stationary real wavelet, as tutorials/poststack.py uses it inside MPIBlockDiag::
+
+        PoststackLinearModelling(wav, nt0, spatdims) == Convolve1D(dims, wav, offset=len(wav) // 2, axis=0)
+                                                        * FirstDerivative(dims, axis=0, sampling=1.0, kind=kind)
+
+    on ``dims = (nt0,) + spatdims``; the adjoint is ``D^T C^T``.  The operator dtype is ``wav.dtype``; data are
+    promoted and ``out=`` is handled as in :class:`Convolve1D`.  Each apply is ONE b2_poststack_axis launch
+    (csrc/convolve.cu: the derivative is fused into the convolution kernel), equal bit for bit to the two-launch
+    chain.  ``explicit`` / ``sparse`` matrices, non-stationary (2-D) and complex wavelets are not provided."""
+
+    def __init__(self, wav, nt0: int, spatdims=None, explicit: bool = False, sparse: bool = False,
+                 kind: str = "centered"):
+        if explicit or sparse:
+            raise NotImplementedError("explicit / sparse matrices are not provided: use the matrix-free operator")
+        if kind not in ("forward", "centered"):
+            raise NotImplementedError(f"{kind} not an available derivative kind...")
+        wav = wav.detach().cpu().numpy() if isinstance(wav, torch.Tensor) else np.asarray(wav)
+        if spatdims is None:
+            dims = (int(nt0),)
+        elif np.ndim(spatdims) == 0:
+            dims = (int(nt0), int(spatdims))
+        else:
+            dims = (int(nt0),) + tuple(int(d) for d in spatdims)
+        super().__init__(dims, wav, offset=len(wav) // 2, axis=0, dtype=np.result_type(wav.dtype, np.float32))
+        self.kind = kind
+        self._kind = _lib.FD_CENTERED if kind == "centered" else _lib.FD_FORWARD
+
+    def _launch(self, x, y, n_outer, n_axis, n_inner, real, adjoint):
+        _lib.check(_lib.lib.b2_poststack_axis(_lib.ctx(), x.data_ptr(), y.data_ptr(), n_outer, n_axis, n_inner,
+                                              self._h[real].data_ptr(), self.nh, self.offset, self._kind, adjoint,
+                                              _lib.code(real), _lib.stream()), "b2_poststack_axis")
+
+
+class Transpose(LocalOperator):
+    """pylops.basicoperators.Transpose: ``y = x.reshape(dims).transpose(axes).ravel()``; the adjoint applies the
+    inverse permutation.  A strided copy through torch (plumbing, not a hot path: inside ``T.H @ X @ T`` it is
+    folded away, see :class:`LocalOperator`).  ``T.H`` is the inverse Transpose."""
+
+    def __init__(self, dims, axes, dtype="float64"):
+        self.dims = tuple(int(d) for d in (dims if np.ndim(dims) else (dims,)))
+        self.axes = tuple(int(a) for a in (axes if np.ndim(axes) else (axes,)))
+        if sorted(self.axes) != list(range(len(self.dims))):
+            raise ValueError(f"axes {axes} is not a permutation of the {len(self.dims)} axes of dims {self.dims}")
+        self.dimsd = tuple(self.dims[a] for a in self.axes)
+        n = int(np.prod(self.dims))
+        self.shape = (n, n)
+        self.dtype = np.dtype(dtype)
+
+    @property
+    def H(self) -> "Transpose":
+        return Transpose(self.dimsd, tuple(int(a) for a in np.argsort(self.axes)), dtype=self.dtype)
+
+    def _matvec(self, x):
+        return x.reshape(self.dims).permute(self.axes).contiguous().reshape(-1)
+
+    def _rmatvec(self, x):
+        return x.reshape(self.dimsd).permute(tuple(int(a) for a in np.argsort(self.axes))).contiguous().reshape(-1)
+
+
+def _along(op, dims, axis):
+    import copy
+    new = copy.copy(op)
+    new.dims = tuple(int(d) for d in dims)
+    new.axis = int(axis) % len(new.dims)
+    return new
+
+
+_AXIS_OPERATORS = (_AxisDerivative, Convolve1D)      # PoststackLinearModelling is a Convolve1D
 
 
 class FFT(LocalOperator):

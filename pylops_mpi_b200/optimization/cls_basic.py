@@ -47,7 +47,8 @@ class Solver:
 _GRAPH_SAFE_TYPES = ("MPIBlockDiag", "MPIVStack", "MPIHStack", "MPIFirstDerivative", "MPISecondDerivative",
                      "_MPISummaMatrixMult", "_MPIBlockMatrixMult", "_AdjointLinearOperator", "_TransposedLinearOperator",
                      "_ProductLinearOperator", "_ScaledLinearOperator", "_SumLinearOperator", "_ConjLinearOperator",
-                     "MatrixMult", "FirstDerivative", "SecondDerivative", "Convolve1D")
+                     "MatrixMult", "FirstDerivative", "SecondDerivative", "Convolve1D",
+                     "PoststackLinearModelling")
 
 
 _GRAPH_POOL = {}
