@@ -159,6 +159,18 @@ int b2_convolve_axis(b2_ctx* ctx, const void* x, void* y, size_t n_outer, size_t
  * error codes as b2_convolve_axis, plus B2_ERR_ARG for any other kind; y is untouched on every error */
 int b2_poststack_axis(b2_ctx* ctx, const void* x, void* y, size_t n_outer, size_t n_axis, size_t n_inner,
                       const void* h, int nh, int offset, int kind, int adjoint, int dtype, void* stream);
+/* rank-local Kirchhoff demigration, spreading / stacking stage: pylops.waveeqprocessing.Kirchhoff (mode="analytic",
+ * 2-D, dynamic=False) before its wavelet convolution (run that as b2_convolve_axis on the [ns*nr][nt] traces).
+ * Tables are float64 device arrays in the kernel's layout: trav_srcs [ns][ni], trav_recs [nr][ni] (a trace reads
+ * contiguous image points).  Forward: x is the image [ni], y the traces [ns*nr][nt] (trace isrc*nr + irec), every
+ * sample written; adjoint: the reverse.  Per pair q = (trav_srcs + trav_recs) / dt in float64 (one add, one IEEE
+ * divide), it = trunc(q), d = q - it, used iff 0 <= it < nt - 1: forward y[it] += x (1-d), y[it+1] += x d; adjoint
+ * y += x[it] (1-d) + x[it+1] d, in (isrc, irec) order: float64 adjoints equal pylops' loop bit for bit.  Deterministic
+ * (no floating-point atomics), no allocation.  dtype F32 / F64 (index math always float64).  B2_ERR_ARG: a null
+ * pointer, x == y, a zero size, dt not finite and positive; B2_ERR_DTYPE: another dtype; y is untouched on every
+ * error */
+int b2_kirchhoff(b2_ctx* ctx, const void* x, void* y, const double* trav_srcs, const double* trav_recs, size_t ni,
+                 size_t ns, size_t nr, size_t nt, double dt, int adjoint, int dtype, void* stream);
 /* Peer-memory halo exchange fused INTO the stencil kernel (replaces the add_ghost_cells Send/Recv pairs of
  * DistributedArray.py:876-953 as used by FirstDerivative.py:221-247, 276-319 and SecondDerivative.py): every rank
  * owns a box of b2_halo_bytes(cap) bytes in IPC-mapped memory (b2_symm_alloc + b2_ipc_*); boxes_host[r] is rank r's

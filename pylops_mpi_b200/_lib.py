@@ -88,6 +88,7 @@ def _load():
         "b2_derivative_axis": ([vp, vp, vp, sz, sz, sz, i, i, i, i, d, i, i, vp], i),
         "b2_convolve_axis": ([vp, vp, vp, sz, sz, sz, vp, i, i, i, i, vp], i),
         "b2_poststack_axis": ([vp, vp, vp, sz, sz, sz, vp, i, i, i, i, i, vp], i),
+        "b2_kirchhoff": ([vp, vp, vp, vp, vp, sz, sz, sz, sz, d, i, i, vp], i),
         "b2_halo_bytes": ([sz], sz),
         "b2_halo_create": ([i, i, C.POINTER(vp), sz, C.POINTER(vp)], i),
         "b2_halo_destroy": ([vp], i),

@@ -456,6 +456,138 @@ def _along(op, dims, axis):
 _AXIS_OPERATORS = (_AxisDerivative, Convolve1D)      # PoststackLinearModelling is a Convolve1D
 
 
+def _traveltime_tables(z, x, srcs, recs, vel):
+    """analytic (constant-velocity) traveltime tables of pylops.waveeqprocessing.Kirchhoff, in float64, computed with
+    pylops' NumPy expressions: ``trav_srcs[ii, isrc] = sqrt((X - sx)**2 + (Z - sz)**2) / vel`` on the raveled
+    ``meshgrid(x, z, indexing="ij")`` grid (``ii = ix * nz + iz``), and the same for the receivers"""
+    X, Z = np.meshgrid(x, z, indexing="ij")
+    X, Z = X.ravel(), Z.ravel()
+    srcs, recs = np.asarray(srcs), np.asarray(recs)
+    trav_srcs = np.sqrt((X[:, None] - srcs[0][None]) ** 2 + (Z[:, None] - srcs[1][None]) ** 2) / vel
+    trav_recs = np.sqrt((X[:, None] - recs[0][None]) ** 2 + (Z[:, None] - recs[1][None]) ** 2) / vel
+    return trav_srcs.astype(np.float64), trav_recs.astype(np.float64)
+
+
+class Kirchhoff(LocalOperator):
+    """Rank-local Kirchhoff demigration, pylops.waveeqprocessing.Kirchhoff (pylops 2.x) with ``mode="analytic"`` in
+    2-D: the ``Demop`` of tutorials/lsm.py inside MPIVStack.  The model is the image ``(nx, nz)``, the data the traces
+    ``(ns, nr, nt)``.  For every (image point, trace) pair the traveltime ``trav`` indexes the trace at
+    ``it = int(trav / dt)`` with weights ``1 - d`` and ``d`` on samples ``it`` and ``it + 1`` (``d = trav / dt - it``,
+    pairs with ``it >= nt - 1`` are dropped); the traces are then convolved with ``wav`` (``Convolve1D`` with
+    ``offset=wavcenter`` along time).
+
+    The float64 traveltime tables are computed on the host at construction, with pylops' expressions, and uploaded
+    once; a workspace of ``ns * nr * nt`` samples holds the traces between the two stages.  Forward: b2_kirchhoff
+    (spreading) into the workspace, then b2_convolve_axis into the output; adjoint: the reverse (csrc/kirchhoff.cu,
+    csrc/convolve.cu).  Only the analytic, 2-D, static (``dynamic=False``) operator without wavelet filtering,
+    apertures, or user tables is provided; ``engine`` is accepted and ignored."""
+
+    def __init__(self, z, x, t, srcs, recs, vel, wav, wavcenter, y=None, mode="eikonal", wavfilter=False,
+                 dynamic=False, trav=None, amp=None, aperture=None, angleaperture=90, snell=None, engine="numpy",
+                 dtype="float64", name="K"):
+        for opt, val, default in (("y", y, None), ("wavfilter", wavfilter, False), ("dynamic", dynamic, False),
+                                  ("trav", trav, None), ("amp", amp, None), ("aperture", aperture, None),
+                                  ("angleaperture", angleaperture, 90), ("snell", snell, None)):
+            if not (val is default or (default is not None and np.ndim(val) == 0 and val == default)):
+                raise NotImplementedError(f"Kirchhoff: {opt}={val!r} is not supported (only its default {default!r})")
+        if mode != "analytic":
+            raise NotImplementedError(f"Kirchhoff: mode={mode!r} is not supported (only mode='analytic')")
+        if np.ndim(vel) != 0:
+            raise ValueError("vel must be scalar for mode=analytical")
+        z, x, t = (np.asarray(a) for a in (z, x, t))
+        srcs, recs = np.asarray(srcs), np.asarray(recs)
+        if srcs.ndim != 2 or recs.ndim != 2 or srcs.shape[0] != 2 or recs.shape[0] != 2:
+            raise NotImplementedError("Kirchhoff: only 2-D geometries (srcs, recs of shape (2, n)) are supported")
+        wav = wav.detach().cpu().numpy() if isinstance(wav, torch.Tensor) else np.asarray(wav)
+        if np.iscomplexobj(wav) or wav.ndim != 1:
+            raise NotImplementedError("Kirchhoff: only a real 1-D wavelet is supported")
+        self.nx, self.nz, self.nt = x.size, z.size, t.size
+        self.ns, self.nr = srcs.shape[1], recs.shape[1]
+        self.ni = self.nx * self.nz
+        self.dt = float(t[1] - t[0])
+        self.dims, self.dimsd = (self.nx, self.nz), (self.ns, self.nr, self.nt)
+        self.shape = (self.ns * self.nr * self.nt, self.ni)
+        self.engine = engine
+        self._tdtype = _lib.torch_dtype(dtype)
+        self.dtype = _lib.numpy_dtype(self._tdtype)
+        if self._tdtype not in (torch.float32, torch.float64):
+            raise NotImplementedError(f"Kirchhoff: dtype {dtype} is not supported (float32 or float64)")
+        trav_srcs, trav_recs = _traveltime_tables(z, x, srcs, recs, vel)
+        _lib.ctx()
+        # kernel layout: (ns, ni) and (nr, ni), a trace reads contiguous image points
+        self._ts = torch.as_tensor(np.ascontiguousarray(trav_srcs.T)).to("cuda")
+        self._tr = torch.as_tensor(np.ascontiguousarray(trav_recs.T)).to("cuda")
+        self.cop = Convolve1D((self.ns * self.nr, self.nt), wav, offset=int(wavcenter), axis=1, dtype=self.dtype)
+        self._ws = {self._tdtype: torch.empty(self.shape[0], dtype=self._tdtype, device="cuda")}
+
+    def _workspace(self, real):
+        ws = self._ws.get(real)
+        if ws is None:                          # data of the other precision: one more workspace, kept
+            ws = self._ws[real] = torch.empty(self.shape[0], dtype=real, device="cuda")
+        return ws
+
+    def _kirch(self, x, y, real, adjoint):
+        _lib.check(_lib.lib.b2_kirchhoff(_lib.ctx(), x.data_ptr(), y.data_ptr(), self._ts.data_ptr(),
+                                         self._tr.data_ptr(), self.ni, self.ns, self.nr, self.nt, self.dt,
+                                         int(adjoint), _lib.code(real), _lib.stream()), "b2_kirchhoff")
+
+    def _apply(self, x: torch.Tensor, adjoint: int, out=None) -> torch.Tensor:
+        x = x.reshape(-1)
+        nin, nout = (self.shape[0], self.shape[1]) if adjoint else (self.shape[1], self.shape[0])
+        if x.numel() != nin:
+            raise ValueError(f"dimension mismatch: operator {self.shape}, vector {x.numel()}")
+        if out is not None and out.numel() != nout:
+            raise ValueError(f"dimension mismatch: operator {self.shape}, out {out.numel()}")
+        if x.dtype.is_complex:
+            # real operator, complex data: the same real map on the real and imaginary parts
+            y = torch.complex(self._apply(x.real.contiguous(), adjoint), self._apply(x.imag.contiguous(), adjoint))
+            return y if out is None else _store(out, y)
+        real = torch.promote_types(self._tdtype, x.dtype) if x.dtype in (torch.float32, torch.float64) else self._tdtype
+        if x.dtype != real:
+            x = x.to(real)
+        if not x.is_contiguous():
+            x = x.contiguous()
+        direct = (out is not None and out.dtype == real and out.is_contiguous() and out.data_ptr() != x.data_ptr())
+        y = out if direct else torch.empty(nout, dtype=real, device=x.device)
+        ws = self._workspace(real)
+        if adjoint:
+            self.cop._launch(x, ws, self.ns * self.nr, self.nt, 1, real, 1)
+            self._kirch(ws, y, real, True)
+        else:
+            self._kirch(x, ws, real, False)
+            self.cop._launch(ws, y, self.ns * self.nr, self.nt, 1, real, 0)
+        if out is not None and not direct:
+            return _store(out, y)
+        return y
+
+    def _matvec(self, x, out=None):
+        return self._apply(x, 0, out)
+
+    def _rmatvec(self, x, out=None):
+        return self._apply(x, 1, out)
+
+    def matvec(self, x, out=None):
+        return self._apply(x, 0, out)
+
+    def rmatvec(self, x, out=None):
+        return self._apply(x, 1, out)
+
+
+class LSM:
+    """pylops.waveeqprocessing.LSM (pylops 2.x) for ``kind="kirchhoff"``: builds the demigration operator ``Demop``, a
+    :class:`Kirchhoff` with ``kwargs_mod`` passed through -- the only part tutorials/lsm.py uses (each rank's
+    ``lsm.Demop`` goes into MPIVStack).  ``solve`` is not provided: run ``cgls`` on the stacked operator."""
+
+    def __init__(self, z, x, t, srcs, recs, vel, wav, wavcenter, y=None, kind="kirchhoff", dottest=False,
+                 **kwargs_mod):
+        if kind != "kirchhoff":
+            raise NotImplementedError(f"LSM: kind={kind!r} is not supported (only 'kirchhoff')")
+        if dottest:
+            raise NotImplementedError("LSM: dottest=True is not supported (run utils.dottest on Demop)")
+        self.y, self.x, self.z, self.t = y, x, z, t
+        self.Demop = Kirchhoff(z, x, t, srcs, recs, vel, wav, wavcenter, y=y, **kwargs_mod)
+
+
 class FFT(LocalOperator):
     """Rank-local real FFT along ``axis`` of a ``dims`` block -- the role of third-party
     ``pylops.signalprocessing.FFT(dims, axis, real=True, ifftshift_before=..., norm="ortho")`` inside

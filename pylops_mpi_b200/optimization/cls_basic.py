@@ -48,7 +48,7 @@ _GRAPH_SAFE_TYPES = ("MPIBlockDiag", "MPIVStack", "MPIHStack", "MPIFirstDerivati
                      "_MPISummaMatrixMult", "_MPIBlockMatrixMult", "_AdjointLinearOperator", "_TransposedLinearOperator",
                      "_ProductLinearOperator", "_ScaledLinearOperator", "_SumLinearOperator", "_ConjLinearOperator",
                      "MatrixMult", "FirstDerivative", "SecondDerivative", "Convolve1D",
-                     "PoststackLinearModelling")
+                     "PoststackLinearModelling", "Kirchhoff")
 
 
 _GRAPH_POOL = {}
