@@ -6,28 +6,14 @@ from typing import Sequence
 
 from ..comm import COMM_WORLD
 from ..LinearOperator import MPILinearOperator
+from ..local import _LocalAdjoint
 from .VStack import MPIVStack
-
-
-class _AdjLocal:
-    """H of a rank-local operator"""
-
-    def __init__(self, op):
-        self.op = op
-        self.shape = (op.shape[1], op.shape[0])
-        self.dtype = op.dtype
-
-    def matvec(self, x, out=None):
-        return self.op.rmatvec(x, out=out) if out is not None else self.op.rmatvec(x)
-
-    def rmatvec(self, x, out=None):
-        return self.op.matvec(x, out=out) if out is not None else self.op.matvec(x)
 
 
 class MPIHStack(MPILinearOperator):
     def __init__(self, ops: Sequence, base_comm=COMM_WORLD, dtype=None):
         self.ops = ops
-        hops = [_AdjLocal(op) for op in ops]
+        hops = [_LocalAdjoint(op) for op in ops]
         self.HStack = MPIVStack(ops=hops, base_comm=base_comm, dtype=dtype).H
         super().__init__(shape=self.HStack.shape, dtype=self.HStack.dtype, base_comm=base_comm)
 

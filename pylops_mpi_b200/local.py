@@ -8,6 +8,9 @@ reference test / BASELINE config uses, applied by the b2_gemv kernels.
 """
 from __future__ import annotations
 
+import copy
+import math
+
 import numpy as np
 import torch
 
@@ -16,31 +19,16 @@ from . import _lib
 __all__ = ["MatrixMult", "LocalOperator", "apply_into"]
 
 _REAL_OF = {torch.complex64: torch.float32, torch.complex128: torch.float64}
-_CPLX_OF = {torch.float32: torch.complex64, torch.float64: torch.complex128, torch.bfloat16: torch.complex64}
-_OUT_OK = {}
-
-
-def _accepts_out(fn) -> bool:
-    """does this bound method take an ``out=`` keyword?  (signature inspection, cached per function: catching
-    TypeError around the call would mask genuine TypeErrors raised inside the operator and re-run it)"""
-    import inspect
-    key = getattr(fn, "__func__", fn)
-    ok = _OUT_OK.get(key)
-    if ok is None:
-        try:
-            params = inspect.signature(fn).parameters
-            ok = "out" in params or any(p.kind is inspect.Parameter.VAR_KEYWORD for p in params.values())
-        except (TypeError, ValueError):
-            ok = False
-        _OUT_OK[key] = ok
-    return ok
+_CPLX_OF = {torch.float32: torch.complex64, torch.float64: torch.complex128}
 
 
 def apply_into(oper, x: torch.Tensor, out: torch.Tensor, adjoint: bool) -> None:
-    """``out[...] = oper(x)`` / ``oper^H(x)`` for a rank-local operator, writing in place when the operator
-    supports ``out=`` (the b200 local operators), else through a temporary (cast to ``out``'s dtype)."""
+    """``out[...] = oper(x)`` / ``oper^H(x)`` for a rank-local operator: a kernel operator of this package (or the
+    ``.H`` of one) writes into ``out`` itself, any other operator through a temporary (cast to ``out``'s dtype)."""
+    while isinstance(oper, _LocalAdjoint):
+        oper, adjoint = oper.op, not adjoint
     fn = oper.rmatvec if adjoint else oper.matvec
-    if _accepts_out(fn):
+    if isinstance(oper, _KernelOperator):
         fn(x, out=out)
     else:
         _store(out, fn(x))
@@ -138,7 +126,7 @@ class _LocalProduct(LocalOperator):
 def _fold(t_inv, op, t) -> "LocalOperator | None":
     """``T.H @ X @ T`` as one operator: ``X`` along axis ``T.axes[X.axis]`` of ``T.dims`` (no transposes), when
     ``t`` is a Transpose, ``t_inv`` its inverse and ``op`` an axis operator on ``t``'s output dims; else None"""
-    if not (isinstance(t, Transpose) and isinstance(t_inv, Transpose) and isinstance(op, _AXIS_OPERATORS)):
+    if not (isinstance(t, Transpose) and isinstance(t_inv, Transpose) and isinstance(op, _AxisOperator)):
         return None
     if t_inv.dims != t.dimsd or t_inv.axes != tuple(int(a) for a in np.argsort(t.axes)) or op.dims != t.dimsd:
         return None
@@ -161,7 +149,90 @@ def _product(*ops) -> LocalOperator:
     return flat[0] if len(flat) == 1 else _LocalProduct(flat)
 
 
-class MatrixMult(LocalOperator):
+class _KernelOperator(LocalOperator):
+    """A rank-local operator applied by this package's kernels.  Each apply is a fixed sequence of launches with no
+    per-call host state (so ``CGLS.run`` may replay it in a CUDA graph), and ``matvec`` / ``rmatvec`` take ``out=``:
+    ``x`` or ``out`` of the wrong length raises ``ValueError``; the result is written into ``out`` directly when it
+    is contiguous, has the compute dtype and is not ``x``, else through a temporary with NumPy's assignment casting.
+    A subclass provides ``_launch`` and, when its dtype rule is not "compute in the operator's dtype",
+    ``_compute_dtype``."""
+
+    def _compute_dtype(self, xdt: torch.dtype) -> torch.dtype:
+        """the dtype data of dtype ``xdt`` are applied in; a real dtype for complex data means that the real and
+        imaginary parts are applied one after the other"""
+        return self._tdtype
+
+    def _launch(self, x: torch.Tensor, y: torch.Tensor, dt: torch.dtype, adjoint: int) -> None:
+        """``y = A x`` (adjoint 0) or ``y = A^H x`` (adjoint 1) on contiguous ``x``, ``y`` of the compute dtype ``dt``"""
+        raise NotImplementedError
+
+    def _apply(self, x: torch.Tensor, adjoint: int, out=None) -> torch.Tensor:
+        x = x.reshape(-1)
+        nout, nin = self.shape[::-1] if adjoint else self.shape
+        if x.numel() != nin:
+            raise ValueError(f"dimension mismatch: operator {self.shape}, vector {x.numel()}")
+        if out is not None and out.numel() != nout:
+            raise ValueError(f"dimension mismatch: operator {self.shape}, out {out.numel()}")
+        dt = self._compute_dtype(x.dtype)
+        if x.dtype.is_complex and not dt.is_complex:
+            # real operator, complex data: result_type(op, x) is complex (the reference's NumPy promotion) --
+            # apply to the real and imaginary parts instead of dropping the imaginary one
+            rdt = torch.promote_types(dt, _REAL_OF[x.dtype])
+            y = torch.complex(self._apply(x.real.contiguous(), adjoint).to(rdt),
+                              self._apply(x.imag.contiguous(), adjoint).to(rdt))
+            return y if out is None else _store(out, y)
+        if x.dtype != dt:
+            x = x.to(dt)
+        if not x.is_contiguous():
+            x = x.contiguous()
+        direct = out is not None and out.dtype == dt and out.is_contiguous() and out.data_ptr() != x.data_ptr()
+        y = out if direct else torch.empty(nout, dtype=dt, device=x.device)
+        self._launch(x, y, dt, adjoint)
+        if out is not None and not direct:       # caller's buffer has another dtype (e.g. mixed-dtype BlockDiag)
+            return _store(out, y)
+        return y
+
+    def matvec(self, x, out=None):
+        return self._apply(x, 0, out)
+
+    def rmatvec(self, x, out=None):
+        return self._apply(x, 1, out)
+
+    _matvec, _rmatvec = matvec, rmatvec
+
+
+class _AxisOperator(_KernelOperator):
+    """A square operator applied line by line along ``axis`` of a C-ordered ``dims`` block, with real taps: complex
+    data are applied in one launch, their (re, im) pairs as the innermost dimension"""
+
+    def __init__(self, dims, axis: int, dtype):
+        self.dims = tuple(int(d) for d in (dims if np.ndim(dims) else (dims,)))
+        self.axis = axis % len(self.dims)
+        n = int(np.prod(self.dims))
+        self.shape = (n, n)
+        self._tdtype = _lib.torch_dtype(dtype)
+        self.dtype = _lib.numpy_dtype(self._tdtype)
+        _lib.ctx()
+
+    def _along(self, dims, axis):
+        """the same operator on a ``dims`` block along ``axis`` (``prod(dims)`` unchanged)"""
+        new = copy.copy(self)
+        new.dims = tuple(int(d) for d in dims)
+        new.axis = int(axis) % len(new.dims)
+        return new
+
+    def _compute_dtype(self, xdt):
+        if xdt.is_complex and not self._tdtype.is_complex:
+            return _CPLX_OF[torch.promote_types(self._tdtype, _REAL_OF[xdt])]
+        return self._tdtype
+
+    def _lines(self, dt):
+        """``(n_outer, n_axis, n_inner, real dtype)`` of a launch on data of dtype ``dt``"""
+        n_inner = math.prod(self.dims[self.axis + 1:]) * (2 if dt.is_complex else 1)
+        return math.prod(self.dims[:self.axis]), self.dims[self.axis], n_inner, _REAL_OF.get(dt, dt)
+
+
+class MatrixMult(_KernelOperator):
     """Dense block ``y = A x`` / ``y = A^H x`` (pylops.MatrixMult for a single
     right-hand side).  ``A`` may be a NumPy array (uploaded once) or a device
     tensor; dtype float32/float64/complex64/complex128, or bfloat16 with
@@ -177,53 +248,17 @@ class MatrixMult(LocalOperator):
         _lib.ctx()
         self.A = A.to("cuda").contiguous()
         self.shape = (int(A.shape[0]), int(A.shape[1]))
-        self._tdtype = self.A.dtype
-        self._xdtype = torch.float32 if self._tdtype is torch.bfloat16 else self._tdtype
-        self.dtype = _lib.numpy_dtype(self._xdtype)
+        self._tdtype = torch.float32 if self.A.dtype is torch.bfloat16 else self.A.dtype
+        self.dtype = _lib.numpy_dtype(self._tdtype)
 
-    def _apply(self, x: torch.Tensor, op: int, out=None) -> torch.Tensor:
+    def _launch(self, x, y, dt, adjoint):
         m, n = self.shape
-        x = x.reshape(-1)
-        nin, nout = (n, m) if op == _lib.OP_N else (m, n)
-        if x.numel() != nin:
-            raise ValueError(f"dimension mismatch: operator {self.shape}, vector {x.numel()}")
-        if x.dtype.is_complex and not self._xdtype.is_complex:
-            # real operator, complex data: result_type(op, x) is complex (the reference's NumPy promotion) --
-            # apply to the real and imaginary parts instead of dropping the imaginary one
-            rdt = torch.promote_types(self._xdtype, _REAL_OF[x.dtype])
-            yr = self._apply(x.real.contiguous(), op).to(rdt)
-            yi = self._apply(x.imag.contiguous(), op).to(rdt)
-            y = torch.complex(yr, yi)
-            return y if out is None else _store(out, y)
-        if x.dtype != self._xdtype:
-            x = x.to(self._xdtype)
-        if not x.is_contiguous():
-            x = x.contiguous()
-        direct = out is not None and out.dtype == self._xdtype and out.is_contiguous() and out.numel() == nout
-        if out is not None and out.numel() != nout:
-            raise ValueError(f"dimension mismatch: operator {self.shape}, out {out.numel()}")
-        y = out if direct else torch.empty(nout, dtype=self._xdtype, device=x.device)
         _lib.check(_lib.lib.b2_gemv(_lib.ctx(), self.A.data_ptr(), n, m, n, x.data_ptr(), y.data_ptr(),
-                                    op, _lib.code(self._tdtype), _lib.code(self._xdtype), _lib.stream()),
-                   "b2_gemv")
-        if out is not None and not direct:       # caller's buffer has another dtype (e.g. mixed-dtype BlockDiag)
-            return _store(out, y)
-        return y
-
-    def _matvec(self, x, out=None):
-        return self._apply(x, _lib.OP_N, out)
-
-    def _rmatvec(self, x, out=None):
-        return self._apply(x, _lib.OP_H, out)
-
-    def matvec(self, x, out=None):
-        return self._apply(x, _lib.OP_N, out)
-
-    def rmatvec(self, x, out=None):
-        return self._apply(x, _lib.OP_H, out)
+                                    _lib.OP_H if adjoint else _lib.OP_N, _lib.code(self.A.dtype), _lib.code(dt),
+                                    _lib.stream()), "b2_gemv")
 
 
-class _AxisDerivative(LocalOperator):
+class _AxisDerivative(_AxisOperator):
     """Rank-local derivative along one axis of a C-ordered ``dims`` block (the role of
     pylops.FirstDerivative / pylops.SecondDerivative inside MPIBlockDiag in MPILaplacian / MPIGradient,
     Laplacian.py:97-126, Gradient.py:101-119).  One batched stencil launch (b2_derivative_axis)."""
@@ -231,10 +266,7 @@ class _AxisDerivative(LocalOperator):
 
     def __init__(self, dims, axis: int = 0, sampling: float = 1.0, kind: str = "centered", edge: bool = False,
                  order: int = 3, dtype=np.float64):
-        self.dims = tuple(int(d) for d in (dims if np.ndim(dims) else (dims,)))
-        self.axis = axis % len(self.dims)
-        n = int(np.prod(self.dims))
-        self.shape = (n, n)
+        super().__init__(dims, axis, dtype)
         self.sampling, self.edge, self.order = float(sampling), bool(edge), int(order)
         kinds = {"forward": _lib.FD_FORWARD, "backward": _lib.FD_BACKWARD, "centered": _lib.FD_CENTERED}
         if kind not in kinds:
@@ -242,53 +274,12 @@ class _AxisDerivative(LocalOperator):
         if self._deriv == 1 and kind == "centered" and order not in (3, 5):
             raise NotImplementedError("'order' must be '3, or '5'")
         self._kind = kinds[kind]
-        self._tdtype = _lib.torch_dtype(dtype)
-        self.dtype = _lib.numpy_dtype(self._tdtype)
-        _lib.ctx()
 
-    def _along(self, dims, axis):
-        """the same operator on a ``dims`` block along ``axis`` (``prod(dims)`` unchanged)"""
-        return _along(self, dims, axis)
-
-    def _apply(self, x: torch.Tensor, adjoint: int, out=None) -> torch.Tensor:
-        x = x.reshape(-1)
-        tdt = self._tdtype
-        if x.dtype.is_complex and not tdt.is_complex:
-            tdt = _CPLX_OF[torch.promote_types(tdt, _REAL_OF[x.dtype])]     # real taps on complex data
-        if x.dtype != tdt:
-            x = x.to(tdt)
-        if not x.is_contiguous():
-            x = x.contiguous()
-        direct = out is not None and out.dtype == tdt and out.is_contiguous() and out.numel() == x.numel()
-        y = out if direct else torch.empty_like(x)
-        n_outer = int(np.prod(self.dims[:self.axis])) if self.axis else 1
-        n_axis = self.dims[self.axis]
-        n_inner = int(np.prod(self.dims[self.axis + 1:])) if self.axis + 1 < len(self.dims) else 1
-        cx = tdt.is_complex
-        real = _REAL_OF.get(tdt, tdt)
-        if cx and n_inner == 1:
-            # complex along the innermost axis: the (re, im) pairs are the "inner" dimension
-            n_inner = 2
-        elif cx:
-            n_inner *= 2
+    def _launch(self, x, y, dt, adjoint):
+        n_outer, n_axis, n_inner, real = self._lines(dt)
         _lib.check(_lib.lib.b2_derivative_axis(_lib.ctx(), x.data_ptr(), y.data_ptr(), n_outer, n_axis, n_inner,
                                                self._deriv, self._kind, self.order, int(self.edge), self.sampling,
                                                adjoint, _lib.code(real), _lib.stream()), "b2_derivative_axis")
-        if out is not None and not direct:
-            return _store(out, y)
-        return y
-
-    def _matvec(self, x, out=None):
-        return self._apply(x, 0, out)
-
-    def _rmatvec(self, x, out=None):
-        return self._apply(x, 1, out)
-
-    def matvec(self, x, out=None):
-        return self._apply(x, 0, out)
-
-    def rmatvec(self, x, out=None):
-        return self._apply(x, 1, out)
 
 
 class FirstDerivative(_AxisDerivative):
@@ -303,7 +294,7 @@ class SecondDerivative(_AxisDerivative):
         super().__init__(dims, axis=axis, sampling=sampling, kind=kind, edge=edge, order=3, dtype=dtype)
 
 
-class Convolve1D(LocalOperator):
+class Convolve1D(_AxisOperator):
     """Rank-local 1-D convolution along ``axis`` of a C-ordered ``dims`` block with a stationary real filter ``h``:
     the role of pylops.signalprocessing.Convolve1D inside MPIBlockDiag (tutorials/reflectivity.py:74-76).  For each
     line ``x`` of length ``n`` along ``axis``::
@@ -326,62 +317,16 @@ class Convolve1D(LocalOperator):
         self.offset = int(offset)
         if self.nh < 1 or not 0 <= self.offset <= self.nh - 1:
             raise ValueError(f"offset must be in [0, nh - 1] = [0, {self.nh - 1}], got {offset}")
-        self.dims = tuple(int(d) for d in (dims if np.ndim(dims) else (dims,)))
-        self.axis = axis % len(self.dims)
+        super().__init__(dims, axis, dtype)
         self.method = method
-        n = int(np.prod(self.dims))
-        self.shape = (n, n)
-        self._tdtype = _lib.torch_dtype(dtype)
-        self.dtype = _lib.numpy_dtype(self._tdtype)
-        _lib.ctx()
         # taps in both real precisions, uploaded once
         self._h = {t: torch.as_tensor(h.astype(_lib.numpy_dtype(t))).to("cuda") for t in (torch.float32, torch.float64)}
 
-    def _along(self, dims, axis):
-        """the same operator on a ``dims`` block along ``axis`` (``prod(dims)`` unchanged)"""
-        return _along(self, dims, axis)
-
-    def _launch(self, x, y, n_outer, n_axis, n_inner, real, adjoint):
+    def _launch(self, x, y, dt, adjoint):
+        n_outer, n_axis, n_inner, real = self._lines(dt)
         _lib.check(_lib.lib.b2_convolve_axis(_lib.ctx(), x.data_ptr(), y.data_ptr(), n_outer, n_axis, n_inner,
                                              self._h[real].data_ptr(), self.nh, self.offset, adjoint,
                                              _lib.code(real), _lib.stream()), "b2_convolve_axis")
-
-    def _apply(self, x: torch.Tensor, adjoint: int, out=None) -> torch.Tensor:
-        x = x.reshape(-1)
-        tdt = self._tdtype
-        if x.dtype.is_complex and not tdt.is_complex:
-            tdt = _CPLX_OF[torch.promote_types(tdt, _REAL_OF[x.dtype])]     # real taps on complex data
-        if x.dtype != tdt:
-            x = x.to(tdt)
-        if not x.is_contiguous():
-            x = x.contiguous()
-        if x.numel() != self.shape[1]:
-            raise ValueError(f"dimension mismatch: operator {self.shape}, vector {x.numel()}")
-        direct = (out is not None and out.dtype == tdt and out.is_contiguous() and out.numel() == x.numel()
-                  and out.data_ptr() != x.data_ptr())
-        y = out if direct else torch.empty_like(x)
-        n_outer = int(np.prod(self.dims[:self.axis])) if self.axis else 1
-        n_axis = self.dims[self.axis]
-        n_inner = int(np.prod(self.dims[self.axis + 1:])) if self.axis + 1 < len(self.dims) else 1
-        real = _REAL_OF.get(tdt, tdt)
-        if tdt.is_complex:
-            n_inner *= 2                                  # (re, im) pairs: the same real map on both parts
-        self._launch(x, y, n_outer, n_axis, n_inner, real, adjoint)
-        if out is not None and not direct:
-            return _store(out, y)
-        return y
-
-    def _matvec(self, x, out=None):
-        return self._apply(x, 0, out)
-
-    def _rmatvec(self, x, out=None):
-        return self._apply(x, 1, out)
-
-    def matvec(self, x, out=None):
-        return self._apply(x, 0, out)
-
-    def rmatvec(self, x, out=None):
-        return self._apply(x, 1, out)
 
 
 class PoststackLinearModelling(Convolve1D):
@@ -413,7 +358,8 @@ class PoststackLinearModelling(Convolve1D):
         self.kind = kind
         self._kind = _lib.FD_CENTERED if kind == "centered" else _lib.FD_FORWARD
 
-    def _launch(self, x, y, n_outer, n_axis, n_inner, real, adjoint):
+    def _launch(self, x, y, dt, adjoint):
+        n_outer, n_axis, n_inner, real = self._lines(dt)
         _lib.check(_lib.lib.b2_poststack_axis(_lib.ctx(), x.data_ptr(), y.data_ptr(), n_outer, n_axis, n_inner,
                                               self._h[real].data_ptr(), self.nh, self.offset, self._kind, adjoint,
                                               _lib.code(real), _lib.stream()), "b2_poststack_axis")
@@ -445,17 +391,6 @@ class Transpose(LocalOperator):
         return x.reshape(self.dimsd).permute(tuple(int(a) for a in np.argsort(self.axes))).contiguous().reshape(-1)
 
 
-def _along(op, dims, axis):
-    import copy
-    new = copy.copy(op)
-    new.dims = tuple(int(d) for d in dims)
-    new.axis = int(axis) % len(new.dims)
-    return new
-
-
-_AXIS_OPERATORS = (_AxisDerivative, Convolve1D)      # PoststackLinearModelling is a Convolve1D
-
-
 def _traveltime_tables(z, x, srcs, recs, vel):
     """analytic (constant-velocity) traveltime tables of pylops.waveeqprocessing.Kirchhoff, in float64, computed with
     pylops' NumPy expressions: ``trav_srcs[ii, isrc] = sqrt((X - sx)**2 + (Z - sz)**2) / vel`` on the raveled
@@ -468,7 +403,7 @@ def _traveltime_tables(z, x, srcs, recs, vel):
     return trav_srcs.astype(np.float64), trav_recs.astype(np.float64)
 
 
-class Kirchhoff(LocalOperator):
+class Kirchhoff(_KernelOperator):
     """Rank-local Kirchhoff demigration, pylops.waveeqprocessing.Kirchhoff (pylops 2.x) with ``mode="analytic"`` in
     2-D: the ``Demop`` of tutorials/lsm.py inside MPIVStack.  The model is the image ``(nx, nz)``, the data the traces
     ``(ns, nr, nt)``.  For every (image point, trace) pair the traveltime ``trav`` indexes the trace at
@@ -520,57 +455,25 @@ class Kirchhoff(LocalOperator):
         self.cop = Convolve1D((self.ns * self.nr, self.nt), wav, offset=int(wavcenter), axis=1, dtype=self.dtype)
         self._ws = {self._tdtype: torch.empty(self.shape[0], dtype=self._tdtype, device="cuda")}
 
-    def _workspace(self, real):
-        ws = self._ws.get(real)
-        if ws is None:                          # data of the other precision: one more workspace, kept
-            ws = self._ws[real] = torch.empty(self.shape[0], dtype=real, device="cuda")
-        return ws
+    def _compute_dtype(self, xdt):
+        """float32 / float64 data are applied in ``promote(dtype, xdt)``; complex data part by part"""
+        return torch.promote_types(self._tdtype, xdt) if xdt in (torch.float32, torch.float64) else self._tdtype
 
     def _kirch(self, x, y, real, adjoint):
         _lib.check(_lib.lib.b2_kirchhoff(_lib.ctx(), x.data_ptr(), y.data_ptr(), self._ts.data_ptr(),
                                          self._tr.data_ptr(), self.ni, self.ns, self.nr, self.nt, self.dt,
-                                         int(adjoint), _lib.code(real), _lib.stream()), "b2_kirchhoff")
+                                         adjoint, _lib.code(real), _lib.stream()), "b2_kirchhoff")
 
-    def _apply(self, x: torch.Tensor, adjoint: int, out=None) -> torch.Tensor:
-        x = x.reshape(-1)
-        nin, nout = (self.shape[0], self.shape[1]) if adjoint else (self.shape[1], self.shape[0])
-        if x.numel() != nin:
-            raise ValueError(f"dimension mismatch: operator {self.shape}, vector {x.numel()}")
-        if out is not None and out.numel() != nout:
-            raise ValueError(f"dimension mismatch: operator {self.shape}, out {out.numel()}")
-        if x.dtype.is_complex:
-            # real operator, complex data: the same real map on the real and imaginary parts
-            y = torch.complex(self._apply(x.real.contiguous(), adjoint), self._apply(x.imag.contiguous(), adjoint))
-            return y if out is None else _store(out, y)
-        real = torch.promote_types(self._tdtype, x.dtype) if x.dtype in (torch.float32, torch.float64) else self._tdtype
-        if x.dtype != real:
-            x = x.to(real)
-        if not x.is_contiguous():
-            x = x.contiguous()
-        direct = (out is not None and out.dtype == real and out.is_contiguous() and out.data_ptr() != x.data_ptr())
-        y = out if direct else torch.empty(nout, dtype=real, device=x.device)
-        ws = self._workspace(real)
+    def _launch(self, x, y, dt, adjoint):
+        ws = self._ws.get(dt)
+        if ws is None:                          # data of the other precision: one more workspace, kept
+            ws = self._ws[dt] = torch.empty(self.shape[0], dtype=dt, device="cuda")
         if adjoint:
-            self.cop._launch(x, ws, self.ns * self.nr, self.nt, 1, real, 1)
-            self._kirch(ws, y, real, True)
+            self.cop._launch(x, ws, dt, 1)
+            self._kirch(ws, y, dt, 1)
         else:
-            self._kirch(x, ws, real, False)
-            self.cop._launch(ws, y, self.ns * self.nr, self.nt, 1, real, 0)
-        if out is not None and not direct:
-            return _store(out, y)
-        return y
-
-    def _matvec(self, x, out=None):
-        return self._apply(x, 0, out)
-
-    def _rmatvec(self, x, out=None):
-        return self._apply(x, 1, out)
-
-    def matvec(self, x, out=None):
-        return self._apply(x, 0, out)
-
-    def rmatvec(self, x, out=None):
-        return self._apply(x, 1, out)
+            self._kirch(x, ws, dt, 0)
+            self.cop._launch(ws, y, dt, 0)
 
 
 class LSM:

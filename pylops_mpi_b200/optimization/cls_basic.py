@@ -22,6 +22,7 @@ import torch
 from .. import _lib
 from ..Distributed import allreduce_
 from ..DistributedArray import DistributedArray
+from ..local import _KernelOperator
 
 
 class Solver:
@@ -46,9 +47,7 @@ class Solver:
 
 _GRAPH_SAFE_TYPES = ("MPIBlockDiag", "MPIVStack", "MPIHStack", "MPIFirstDerivative", "MPISecondDerivative",
                      "_MPISummaMatrixMult", "_MPIBlockMatrixMult", "_AdjointLinearOperator", "_TransposedLinearOperator",
-                     "_ProductLinearOperator", "_ScaledLinearOperator", "_SumLinearOperator", "_ConjLinearOperator",
-                     "MatrixMult", "FirstDerivative", "SecondDerivative", "Convolve1D",
-                     "PoststackLinearModelling", "Kirchhoff")
+                     "_ProductLinearOperator", "_ScaledLinearOperator", "_SumLinearOperator", "_ConjLinearOperator")
 
 
 _GRAPH_POOL = {}
@@ -94,8 +93,11 @@ def _reset_capture_state():
 
 def _graph_safe(Op) -> bool:
     """may an apply of ``Op`` be captured once in a CUDA graph and replayed?  Conservative whitelist: operators of
-    this package whose apply is a fixed sequence of kernel launches / collectives with no host-side per-call state
-    (MPIFredholm1's fused mode toggles double buffers on the host, third-party operators are unknown -> eager)"""
+    this package whose apply is a fixed sequence of kernel launches / collectives with no host-side per-call state,
+    the rank-local kernel operators by type, the others by name (MPIFredholm1's fused mode toggles double buffers on
+    the host, third-party operators are unknown -> eager)"""
+    if isinstance(Op, _KernelOperator):
+        return True
     name = type(Op).__name__
     if name not in _GRAPH_SAFE_TYPES:
         return False

@@ -553,7 +553,7 @@ def test_real_block_applied_to_complex_data_keeps_imaginary_part(pm):
 
 
 def test_local_operator_typeerror_is_not_swallowed(pm):
-    """a TypeError raised INSIDE an operator must propagate (out= support is detected by signature, not by catching)"""
+    """a TypeError raised INSIDE an operator must propagate (out= support is detected by type, not by catching)"""
     class Bad(pm.local.LocalOperator):
         shape = (4, 4)
         dtype = np.float64

@@ -273,15 +273,19 @@ def test_strict_parity_mode_raises_exactly_where_the_reference_does(dims, P):
         D._strict_check(x, dst)
 
 
-def test_cgls_graph_whitelist_is_conservative():
-    """CGLS replays its iteration as a CUDA graph only for operator trees made of whitelisted classes; anything unknown
-    (user operators, MPIFredholm1's host-toggled fused mode, MDC's FFT wrappers) keeps the eager path"""
+def test_cgls_graph_safety_is_conservative_and_typed():
+    """CGLS replays its iteration as a CUDA graph only for operator trees made of the package's rank-local kernel
+    operators (recognised by type) and whitelisted MPI classes; anything unknown (user operators, including one that
+    merely shares a kernel operator's class name, MPIFredholm1's host-toggled fused mode, MDC's FFT wrappers) keeps the
+    eager path"""
+    from pylops_mpi_b200 import local
     from pylops_mpi_b200.optimization.cls_basic import _graph_safe
 
     def make(name, **attrs):
         return type(name, (), {"shape": (4, 4), **attrs})()
-    blk = make("MatrixMult")
+    blk = object.__new__(local.MatrixMult)                                   # a kernel operator, no device needed
     assert _graph_safe(make("MPIBlockDiag", ops=[blk]))
+    assert not _graph_safe(make("MPIBlockDiag", ops=[make("MatrixMult")]))  # safe by type, not by class name
     assert _graph_safe(make("_ProductLinearOperator", args=(make("MPIBlockDiag", ops=[blk]), make("MPIFirstDerivative"))))
     assert _graph_safe(make("_ScaledLinearOperator", args=(make("MPIVStack", ops=[blk]), 2.0)))
     assert not _graph_safe(make("MPIFredholm1"))
