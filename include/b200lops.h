@@ -87,12 +87,14 @@ int b2_fill(b2_ctx* ctx, void* out, const double v[2], size_t n, int dtype, void
 /* out_dev[0..1] = sum_i op(x_i) * y_i  (re, im); op = conj when conj_x (numpy.vdot) */
 int b2_dot(b2_ctx* ctx, const void* x, const void* y, size_t n, int dtype, int conj_x,
            double* out_dev, void* stream);
-/* out_dev[0] = local partial for the requested norm kind (p only for SUM_POW) */
+/* out_dev[0] = local partial for the requested norm kind (p only for SUM_POW).  A NaN element makes every kind but
+ * COUNT_NONZERO return NaN, MAX_ABS and MIN_ABS included (as np.max / np.linalg.norm); COUNT_NONZERO counts it. */
 int b2_norm_partial(b2_ctx* ctx, const void* x, size_t n, int dtype, int kind, double p,
                     double* out_dev, void* stream);
 /* axis-wise variant (DistributedArray.norm(ord, axis=...), DistributedArray.py:688-758, 796-807): x is the local block
  * viewed as [n_outer][n_axis][n_inner]; out_dev[o * n_inner + i] = float64 partial over the middle axis for the same
- * norm kinds (the caller combines partials across ranks when the axis is the partition axis and takes the root) */
+ * norm kinds and the same NaN rule as b2_norm_partial (the caller combines partials across ranks when the axis is the
+ * partition axis and takes the root); n_axis == 0 writes each kind's identity (0, or +inf for MIN_ABS) */
 int b2_norm_axis(b2_ctx* ctx, const void* x, size_t n_outer, size_t n_axis, size_t n_inner, int dtype, int kind,
                  double p, double* out_dev, void* stream);
 /* k dot products <x_j, y_j> in ONE launch: out_dev[0..k) for real dtypes, out_dev[0..2k) as
@@ -116,7 +118,8 @@ int b2_history_push(const double* src_dev, int nvals, int stride, double* hist_d
  *   u = base + alpha*g (g may be NULL);  v = threshold_kind(u, thresh) (_apply_thresh, cls_sparsity.py:21-46);
  *   xnew = v;  znew = v + c*(v - xold) (znew may be NULL; FISTA's auxiliary model, :640-644);
  *   sums_dev[0] = sum|v - xold|^2 (0 if xold NULL), sums_dev[1] = sum|v| -- local partials of the update norm
- *   (:331) and the l1 cost (:333).  xnew/znew may alias base/xold.  HALF is real-only. */
+ *   (:331) and the l1 cost (:333).  xnew/znew may alias base/xold.  HALF is real-only.  A NaN in u gives NaN in xnew
+ *   under every kind (complex SOFT: both components), as pylops' NumPy thresholds do, and so NaN sums. */
 int b2_sparse_update(b2_ctx* ctx, const void* base, const void* g, double alpha, const void* xold,
                      double thresh, int kind, void* xnew, void* znew, double c, double* sums_dev,
                      size_t n, int dtype, void* stream);

@@ -12,12 +12,12 @@ constexpr int EW_UNROLL = 4;
 // ---- real-coefficient linear combination on real data ---------------------
 template <typename T, bool HAS_Y>
 __global__ void __launch_bounds__(EW_THREADS)
-lincomb_vec_kernel(T* __restrict__ out, const T* x, const T* y, T a, T b,
+lincomb_vec_kernel(T* __restrict__ out, const T* x, const T* y, double a_scale, double b_scale,
                    const double* __restrict__ a_dev, const double* __restrict__ b_dev,
                    size_t nvec, size_t n) {
   constexpr int V = Vec16<T>::N;
-  if (a_dev) a = (T)((double)a * *a_dev);
-  if (b_dev) b = (T)((double)b * *b_dev);
+  // a = a_scale * (*a_dev) in double, rounded to T once (the same coefficient axpby_norm2_kernel uses)
+  const T a = (T)(a_dev ? a_scale * *a_dev : a_scale), b = (T)(b_dev ? b_scale * *b_dev : b_scale);
   const size_t stride = (size_t)gridDim.x * EW_THREADS;
   size_t i = (size_t)blockIdx.x * EW_THREADS + threadIdx.x;
   for (; i + (EW_UNROLL - 1) * stride < nvec; i += EW_UNROLL * stride) {
@@ -57,10 +57,9 @@ lincomb_vec_kernel(T* __restrict__ out, const T* x, const T* y, T a, T b,
 
 template <typename T, bool HAS_Y>
 __global__ void __launch_bounds__(EW_THREADS)
-lincomb_scalar_kernel(T* out, const T* x, const T* y, T a, T b, const double* a_dev,
+lincomb_scalar_kernel(T* out, const T* x, const T* y, double a_scale, double b_scale, const double* a_dev,
                       const double* b_dev, size_t n) {
-  if (a_dev) a = (T)((double)a * *a_dev);
-  if (b_dev) b = (T)((double)b * *b_dev);
+  const T a = (T)(a_dev ? a_scale * *a_dev : a_scale), b = (T)(b_dev ? b_scale * *b_dev : b_scale);
   const size_t stride = (size_t)gridDim.x * EW_THREADS;
   for (size_t i = (size_t)blockIdx.x * EW_THREADS + threadIdx.x; i < n; i += stride)
     out[i] = HAS_Y ? a * x[i] + b * y[i] : a * x[i];
@@ -134,15 +133,15 @@ int lincomb_real(b2_ctx* ctx, T* out, const T* x, const T* y, double a, double b
     size_t nvec = n / V;
     int grid = ew_grid(ctx, (nvec + EW_UNROLL - 1) / EW_UNROLL);
     if (y)
-      lincomb_vec_kernel<T, true><<<grid, EW_THREADS, 0, st>>>(out, x, y, (T)a, (T)b, a_dev, b_dev, nvec, n);
+      lincomb_vec_kernel<T, true><<<grid, EW_THREADS, 0, st>>>(out, x, y, a, b, a_dev, b_dev, nvec, n);
     else
-      lincomb_vec_kernel<T, false><<<grid, EW_THREADS, 0, st>>>(out, x, y, (T)a, (T)b, a_dev, b_dev, nvec, n);
+      lincomb_vec_kernel<T, false><<<grid, EW_THREADS, 0, st>>>(out, x, y, a, b, a_dev, b_dev, nvec, n);
   } else {
     int grid = ew_grid(ctx, n);
     if (y)
-      lincomb_scalar_kernel<T, true><<<grid, EW_THREADS, 0, st>>>(out, x, y, (T)a, (T)b, a_dev, b_dev, n);
+      lincomb_scalar_kernel<T, true><<<grid, EW_THREADS, 0, st>>>(out, x, y, a, b, a_dev, b_dev, n);
     else
-      lincomb_scalar_kernel<T, false><<<grid, EW_THREADS, 0, st>>>(out, x, y, (T)a, (T)b, a_dev, b_dev, n);
+      lincomb_scalar_kernel<T, false><<<grid, EW_THREADS, 0, st>>>(out, x, y, a, b, a_dev, b_dev, n);
   }
   B2_LAUNCH_CHECK();
   return B2_OK;

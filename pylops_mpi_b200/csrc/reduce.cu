@@ -15,11 +15,15 @@ constexpr int RED_THREADS = 256;
 constexpr int RED_UNROLL = 4;
 enum { MODE_SUM = 0, MODE_MAX = 1, MODE_MIN = 2 };
 
+// max / min that return NaN when either operand is NaN, as np.max and np.linalg.norm(x, inf) do (fmax / fmin drop it)
+__device__ __forceinline__ double nan_max(double a, double b) { return (a > b || a != a) ? a : b; }
+__device__ __forceinline__ double nan_min(double a, double b) { return (a < b || a != a) ? a : b; }
+
 template <int MODE>
 __device__ __forceinline__ double comb(double a, double b) {
   if (MODE == MODE_SUM) return a + b;
-  if (MODE == MODE_MAX) return fmax(a, b);
-  return fmin(a, b);
+  if (MODE == MODE_MAX) return nan_max(a, b);
+  return nan_min(a, b);
 }
 template <int MODE>
 __device__ __forceinline__ double ident() {
@@ -491,13 +495,13 @@ __device__ __forceinline__ double axis_fold(double acc, double a, int kind, doub
     case B2_NRM_COUNT_NONZERO: return acc + (a != 0.0 ? 1.0 : 0.0);
     case B2_NRM_SUM_ABS: return acc + a;
     case B2_NRM_SUM_SQ: return acc + a * a;
-    case B2_NRM_MAX_ABS: return fmax(acc, a);
-    case B2_NRM_MIN_ABS: return fmin(acc, a);
+    case B2_NRM_MAX_ABS: return nan_max(acc, a);
+    case B2_NRM_MIN_ABS: return nan_min(acc, a);
     default: return acc + pow(a, p);
   }
 }
 __device__ __forceinline__ double axis_merge(double a, double b, int kind) {
-  return kind == B2_NRM_MAX_ABS ? fmax(a, b) : (kind == B2_NRM_MIN_ABS ? fmin(a, b) : a + b);
+  return kind == B2_NRM_MAX_ABS ? nan_max(a, b) : (kind == B2_NRM_MIN_ABS ? nan_min(a, b) : a + b);
 }
 template <typename T>
 __global__ void __launch_bounds__(256)

@@ -38,6 +38,9 @@ template <> struct M<float> {
   static __device__ __forceinline__ float acs(float a) { return acosf(a); }
   static __device__ __forceinline__ float cs(float a) { return cosf(a); }
   static __device__ __forceinline__ float fm(float a, float b, float c) { return fmaf(a, b, c); }
+  // the hard cut rounded DOWN: a <= cut holds for a float a exactly when it holds in float64, as in pylops, which
+  // compares |x| with np.sqrt(2 * thresh), a float64 scalar
+  static __device__ __forceinline__ float cut(double c) { return __double2float_rd(c); }
 };
 template <> struct M<double> {
   static __device__ __forceinline__ double abs(double x) { return fabs(x); }
@@ -49,6 +52,7 @@ template <> struct M<double> {
   static __device__ __forceinline__ double acs(double a) { return acos(a); }
   static __device__ __forceinline__ double cs(double a) { return cos(a); }
   static __device__ __forceinline__ double fm(double a, double b, double c) { return fma(a, b, c); }
+  static __device__ __forceinline__ double cut(double c) { return c; }
 };
 
 template <typename C>
@@ -61,7 +65,10 @@ template <typename C>
 __device__ __forceinline__ C thr_real(C u, const SpConst<C>& k) {
   const C a = M<C>::abs(u);
   switch (k.kind) {
-    case B2_THRESH_SOFT: return M<C>::cps(M<C>::max(a - k.thresh, (C)0), u);
+    case B2_THRESH_SOFT: {  // max(a - t, 0) that keeps a NaN, as np.maximum does (fmax would return 0)
+      const C d = a - k.thresh;
+      return M<C>::cps(d <= (C)0 ? (C)0 : d, u);
+    }
     case B2_THRESH_HARD: return a <= k.hard_cut ? (C)0 : u;
     case B2_THRESH_HALF: {
       if (a <= k.half_cut) return (C)0;
@@ -79,7 +86,10 @@ template <typename C>
 __device__ __forceinline__ C thr_cx(C& ur, C& ui, const SpConst<C>& k) {
   const C a = M<C>::hyp(ur, ui);
   C s = (C)1;
-  if (k.kind == B2_THRESH_SOFT) s = a > (C)0 ? M<C>::max(a - k.thresh, (C)0) / a : (C)0;
+  if (k.kind == B2_THRESH_SOFT) {  // a NaN |u| gives s = NaN, so both components come out NaN, as in pylops
+    const C d = a - k.thresh;
+    s = d <= (C)0 ? (C)0 : d / a;
+  }
   else if (k.kind == B2_THRESH_HARD) s = a <= k.hard_cut ? (C)0 : (C)1;
   ur *= s;
   ui *= s;
@@ -128,7 +138,7 @@ sparse_update_kernel(const __grid_constant__ SpParams p, double* __restrict__ pa
   const bool has_g = g != nullptr, has_xo = xo != nullptr, has_zn = zn != nullptr;
   const bool xo_is_base = xo == base;
   SpConst<T> k;
-  k.alpha = (T)p.alpha; k.thresh = (T)p.thresh; k.c = (T)p.c; k.hard_cut = (T)p.hard_cut; k.half_cut = (T)p.half_cut;
+  k.alpha = (T)p.alpha; k.thresh = (T)p.thresh; k.c = (T)p.c; k.hard_cut = M<T>::cut(p.hard_cut); k.half_cut = (T)p.half_cut;
   k.kind = p.kind;
   double acc[2] = {0.0, 0.0};
   const size_t stride = (size_t)gridDim.x * SP_THREADS;
@@ -266,7 +276,7 @@ extern "C" int b2_sparse_update(b2_ctx* ctx, const void* base, const void* g, do
   p.base = base; p.g = g; p.xold = xold; p.xnew = xnew; p.znew = znew;
   p.alpha = alpha; p.thresh = thresh; p.c = c; p.kind = kind;
   p.hard_cut = sqrt(2.0 * thresh);
-  p.half_cut = (cbrt(54.0) / 4.0) * pow(thresh, 2.0 / 3.0);
+  p.half_cut = (pow(54.0, 1.0 / 3.0) / 4.0) * pow(thresh, 2.0 / 3.0);  // pylops' 54 ** (1/3), not cbrt(54)
   p.n_real = cx ? 2 * n : n;
   cudaStream_t st = (cudaStream_t)stream;
   switch (dtype) {
