@@ -163,7 +163,7 @@ int b2_convolve_axis(b2_ctx* ctx, const void* x, void* y, size_t n_outer, size_t
 int b2_poststack_axis(b2_ctx* ctx, const void* x, void* y, size_t n_outer, size_t n_axis, size_t n_inner,
                       const void* h, int nh, int offset, int kind, int adjoint, int dtype, void* stream);
 /* rank-local Kirchhoff demigration, spreading / stacking stage: pylops.waveeqprocessing.Kirchhoff (mode="analytic",
- * 2-D, dynamic=False) before its wavelet convolution (run that as b2_convolve_axis on the [ns*nr][nt] traces).
+ * 2-D or 3-D, dynamic=False) before its wavelet convolution (run that as b2_convolve_axis on the [ns*nr][nt] traces).
  * Tables are float64 device arrays in the kernel's layout: trav_srcs [ns][ni], trav_recs [nr][ni] (a trace reads
  * contiguous image points).  Forward: x is the image [ni], y the traces [ns*nr][nt] (trace isrc*nr + irec), every
  * sample written; adjoint: the reverse.  Per pair q = (trav_srcs + trav_recs) / dt in float64 (one add, one IEEE
@@ -174,6 +174,27 @@ int b2_poststack_axis(b2_ctx* ctx, const void* x, void* y, size_t n_outer, size_
  * error */
 int b2_kirchhoff(b2_ctx* ctx, const void* x, void* y, const double* trav_srcs, const double* trav_recs, size_t ni,
                  size_t ns, size_t nr, size_t nt, double dt, int adjoint, int dtype, void* stream);
+/* b2_kirchhoff over the image points [i0, i0 + nc) of an [ni] image, with that chunk's tables trav_srcs [ns][nc],
+ * trav_recs [nr][nc].  Forward: x is the whole image (x[i0 .. i0+nc) is read), y the traces, overwritten
+ * (accumulate 0) or added into (accumulate 1); adjoint: x the traces, y the whole image, of which y[i0 .. i0+nc) is
+ * written.  i0 must be a multiple of 32: then chunks tiling [0, ni), applied in ascending order with accumulate 0
+ * for the first and 1 after, give b2_kirchhoff's result bit for bit in F32 and F64.  B2_ERR_ARG: as b2_kirchhoff,
+ * plus nc = 0, i0 not a multiple of 32, i0 + nc > ni, accumulate not 0 / 1, accumulate 1 with adjoint; y is
+ * untouched on every error */
+int b2_kirchhoff_chunk(b2_ctx* ctx, const void* x, void* y, const double* trav_srcs, const double* trav_recs,
+                       size_t ni, size_t i0, size_t nc, size_t ns, size_t nr, size_t nt, double dt, int adjoint,
+                       int accumulate, int dtype, void* stream);
+/* analytic (constant-velocity) traveltime table of pylops.waveeqprocessing.Kirchhoff, in b2_kirchhoff_chunk's
+ * layout: table[p][j] = |grid point i0 + j - point p| / vel for p < n, j < nc (row stride nc).  Axes are float64
+ * device arrays; y = NULL for 2-D (ny ignored), where the grid is meshgrid(x, z, indexing="ij") raveled,
+ * ii = ix * nz + iz, and pts is [2][n] with rows (x, z); in 3-D meshgrid(y, x, z, indexing="ij"),
+ * ii = (iy * nx + ix) * nz + iz, pts [3][n] with rows (y, x, z).  NumPy's operations in NumPy's order, rounded to
+ * nearest: 2-D sqrt((x-px)*(x-px) + (z-pz)*(z-pz)) / vel, 3-D sqrt(((x-px)*(x-px) + (z-pz)*(z-pz)) + (y-py)*(y-py))
+ * / vel, equal to the float64 NumPy table bit for bit.  No allocation.  B2_ERR_ARG: a null pointer (y excepted), a
+ * zero size (ny when y is given), i0 + nc > ny * nx * nz; table is untouched on every error */
+int b2_kirchhoff_tables(b2_ctx* ctx, const double* y, const double* x, const double* z, size_t ny, size_t nx,
+                        size_t nz, const double* pts, size_t n, double vel, size_t i0, size_t nc, double* table,
+                        void* stream);
 /* Peer-memory halo exchange fused INTO the stencil kernel (replaces the add_ghost_cells Send/Recv pairs of
  * DistributedArray.py:876-953 as used by FirstDerivative.py:221-247, 276-319 and SecondDerivative.py): every rank
  * owns a box of b2_halo_bytes(cap) bytes in IPC-mapped memory (b2_symm_alloc + b2_ipc_*); boxes_host[r] is rank r's

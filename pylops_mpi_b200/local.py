@@ -391,36 +391,59 @@ class Transpose(LocalOperator):
         return x.reshape(self.dimsd).permute(tuple(int(a) for a in np.argsort(self.axes))).contiguous().reshape(-1)
 
 
-def _traveltime_tables(z, x, srcs, recs, vel):
-    """analytic (constant-velocity) traveltime tables of pylops.waveeqprocessing.Kirchhoff, in float64, computed with
-    pylops' NumPy expressions: ``trav_srcs[ii, isrc] = sqrt((X - sx)**2 + (Z - sz)**2) / vel`` on the raveled
-    ``meshgrid(x, z, indexing="ij")`` grid (``ii = ix * nz + iz``), and the same for the receivers"""
-    X, Z = np.meshgrid(x, z, indexing="ij")
-    X, Z = X.ravel(), Z.ravel()
+def _traveltime_tables(z, x, srcs, recs, vel, y=None):
+    """analytic (constant-velocity) traveltime tables of pylops.waveeqprocessing.Kirchhoff, in float64, computed on
+    the host with pylops' NumPy expressions: ``trav_srcs[ii, isrc] = sqrt((X - sx)**2 + (Z - sz)**2) / vel`` on the
+    raveled ``meshgrid(x, z, indexing="ij")`` grid (``ii = ix * nz + iz``), and the same for the receivers.  With
+    ``y`` (3-D): the grid ``meshgrid(y, x, z, indexing="ij")`` (``ii = (iy * nx + ix) * nz + iz``), points with rows
+    ``(y, x, z)``, and ``(Y - sy)**2`` added last.  :class:`Kirchhoff` builds the same tables on the device
+    (b2_kirchhoff_tables); this is their host reference."""
     srcs, recs = np.asarray(srcs), np.asarray(recs)
-    trav_srcs = np.sqrt((X[:, None] - srcs[0][None]) ** 2 + (Z[:, None] - srcs[1][None]) ** 2) / vel
-    trav_recs = np.sqrt((X[:, None] - recs[0][None]) ** 2 + (Z[:, None] - recs[1][None]) ** 2) / vel
-    return trav_srcs.astype(np.float64), trav_recs.astype(np.float64)
+    if y is None:
+        X, Z = np.meshgrid(x, z, indexing="ij")
+        X, Z = X.ravel(), Z.ravel()
+        trav_srcs = np.sqrt((X[:, None] - srcs[0][None]) ** 2 + (Z[:, None] - srcs[1][None]) ** 2) / vel
+        trav_recs = np.sqrt((X[:, None] - recs[0][None]) ** 2 + (Z[:, None] - recs[1][None]) ** 2) / vel
+        return trav_srcs.astype(np.float64), trav_recs.astype(np.float64)
+    Y, X, Z = np.meshgrid(y, x, z, indexing="ij")
+    Y, X, Z = Y.ravel(), X.ravel(), Z.ravel()
+
+    def table(pts):
+        dist2 = (X[:, None] - pts[1][None]) ** 2 + (Z[:, None] - pts[2][None]) ** 2
+        dist2 += (Y[:, None] - pts[0][None]) ** 2
+        return (np.sqrt(dist2) / vel).astype(np.float64)
+
+    return table(srcs), table(recs)
+
+
+# Device memory the resident traveltime tables of one Kirchhoff operator may take, (ns + nr) * ni * 8 bytes.  Above
+# it the operator keeps one chunk of image points' tables (a multiple of 32 points within the budget) and rebuilds
+# them for each chunk on every apply.  Read when an operator is constructed.
+KIRCHHOFF_TABLE_BYTES = 4 << 30
 
 
 class Kirchhoff(_KernelOperator):
     """Rank-local Kirchhoff demigration, pylops.waveeqprocessing.Kirchhoff (pylops 2.x) with ``mode="analytic"`` in
-    2-D: the ``Demop`` of tutorials/lsm.py inside MPIVStack.  The model is the image ``(nx, nz)``, the data the traces
+    2-D or, with ``y``, 3-D: the ``Demop`` of tutorials/lsm.py inside MPIVStack.  The model is the image ``(nx, nz)``
+    (3-D: ``(ny, nx, nz)``, with ``srcs`` / ``recs`` of shape ``(3, n)``, rows ``(y, x, z)``), the data the traces
     ``(ns, nr, nt)``.  For every (image point, trace) pair the traveltime ``trav`` indexes the trace at
     ``it = int(trav / dt)`` with weights ``1 - d`` and ``d`` on samples ``it`` and ``it + 1`` (``d = trav / dt - it``,
     pairs with ``it >= nt - 1`` are dropped); the traces are then convolved with ``wav`` (``Convolve1D`` with
     ``offset=wavcenter`` along time).
 
-    The float64 traveltime tables are computed on the host at construction, with pylops' expressions, and uploaded
-    once; a workspace of ``ns * nr * nt`` samples holds the traces between the two stages.  Forward: b2_kirchhoff
-    (spreading) into the workspace, then b2_convolve_axis into the output; adjoint: the reverse (csrc/kirchhoff.cu,
-    csrc/convolve.cu).  Only the analytic, 2-D, static (``dynamic=False``) operator without wavelet filtering,
-    apertures, or user tables is provided; ``engine`` is accepted and ignored."""
+    The float64 traveltime tables are built on the device (b2_kirchhoff_tables), equal bit for bit to pylops' NumPy
+    tables.  While ``(ns + nr) * ni * 8`` bytes fit in :data:`KIRCHHOFF_TABLE_BYTES` they are built once at
+    construction and stay resident; above it (``chunked``) the operator holds one chunk of image points' tables and
+    each apply builds and applies them chunk by chunk (b2_kirchhoff_chunk), with the same result bit for bit.  A
+    workspace of ``ns * nr * nt`` samples holds the traces between the two stages.  Forward: spreading into the
+    workspace, then b2_convolve_axis into the output; adjoint: the reverse (csrc/kirchhoff.cu, csrc/convolve.cu).
+    Only the analytic, static (``dynamic=False``) operator without wavelet filtering, apertures, or user tables is
+    provided; ``engine`` is accepted and ignored."""
 
     def __init__(self, z, x, t, srcs, recs, vel, wav, wavcenter, y=None, mode="eikonal", wavfilter=False,
                  dynamic=False, trav=None, amp=None, aperture=None, angleaperture=90, snell=None, engine="numpy",
                  dtype="float64", name="K"):
-        for opt, val, default in (("y", y, None), ("wavfilter", wavfilter, False), ("dynamic", dynamic, False),
+        for opt, val, default in (("wavfilter", wavfilter, False), ("dynamic", dynamic, False),
                                   ("trav", trav, None), ("amp", amp, None), ("aperture", aperture, None),
                                   ("angleaperture", angleaperture, 90), ("snell", snell, None)):
             if not (val is default or (default is not None and np.ndim(val) == 0 and val == default)):
@@ -431,27 +454,47 @@ class Kirchhoff(_KernelOperator):
             raise ValueError("vel must be scalar for mode=analytical")
         z, x, t = (np.asarray(a) for a in (z, x, t))
         srcs, recs = np.asarray(srcs), np.asarray(recs)
-        if srcs.ndim != 2 or recs.ndim != 2 or srcs.shape[0] != 2 or recs.shape[0] != 2:
-            raise NotImplementedError("Kirchhoff: only 2-D geometries (srcs, recs of shape (2, n)) are supported")
+        nd = 2 if y is None else 3
+        if srcs.ndim != 2 or recs.ndim != 2 or srcs.shape[0] != nd or recs.shape[0] != nd:
+            raise NotImplementedError(
+                f"Kirchhoff: y={'None' if y is None else 'given'} needs srcs and recs of shape ({nd}, n) with rows "
+                f"{'(x, z)' if y is None else '(y, x, z)'} (y=None: 2-D, shape (2, n); y given: 3-D, shape "
+                f"(3, n)); got srcs {srcs.shape}, recs {recs.shape}")
         wav = wav.detach().cpu().numpy() if isinstance(wav, torch.Tensor) else np.asarray(wav)
         if np.iscomplexobj(wav) or wav.ndim != 1:
             raise NotImplementedError("Kirchhoff: only a real 1-D wavelet is supported")
+        self.ny = 1 if y is None else np.asarray(y).size
         self.nx, self.nz, self.nt = x.size, z.size, t.size
         self.ns, self.nr = srcs.shape[1], recs.shape[1]
-        self.ni = self.nx * self.nz
+        self.ni = self.ny * self.nx * self.nz
         self.dt = float(t[1] - t[0])
-        self.dims, self.dimsd = (self.nx, self.nz), (self.ns, self.nr, self.nt)
+        self.dims = (self.nx, self.nz) if y is None else (self.ny, self.nx, self.nz)
+        self.dimsd = (self.ns, self.nr, self.nt)
         self.shape = (self.ns * self.nr * self.nt, self.ni)
         self.engine = engine
         self._tdtype = _lib.torch_dtype(dtype)
         self.dtype = _lib.numpy_dtype(self._tdtype)
         if self._tdtype not in (torch.float32, torch.float64):
             raise NotImplementedError(f"Kirchhoff: dtype {dtype} is not supported (float32 or float64)")
-        trav_srcs, trav_recs = _traveltime_tables(z, x, srcs, recs, vel)
         _lib.ctx()
-        # kernel layout: (ns, ni) and (nr, ni), a trace reads contiguous image points
-        self._ts = torch.as_tensor(np.ascontiguousarray(trav_srcs.T)).to("cuda")
-        self._tr = torch.as_tensor(np.ascontiguousarray(trav_recs.T)).to("cuda")
+
+        def dev(a):
+            return torch.as_tensor(np.ascontiguousarray(a, dtype=np.float64)).to("cuda")
+
+        # axes and point coordinates in float64 (the table builder's inputs), points as rows ((y,) x, z)
+        self._axes = (None if y is None else dev(y), dev(x), dev(z))
+        self._srcs, self._recs = dev(srcs), dev(recs)
+        self._vel = float(vel)
+        # image points per chunk: all of them while the tables fit in the budget, else a multiple of 32 that fits
+        per_point = (self.ns + self.nr) * 8
+        nc = self.ni if per_point * self.ni <= KIRCHHOFF_TABLE_BYTES else KIRCHHOFF_TABLE_BYTES // per_point // 32 * 32
+        self._nc = min(self.ni, max(32, nc))
+        self.chunked = self._nc < self.ni
+        # kernel layout: (ns, nc) and (nr, nc), a trace reads contiguous image points
+        self._ts = torch.empty((self.ns, self._nc), dtype=torch.float64, device="cuda")
+        self._tr = torch.empty((self.nr, self._nc), dtype=torch.float64, device="cuda")
+        if not self.chunked:
+            self._tables(0, self.ni)
         self.cop = Convolve1D((self.ns * self.nr, self.nt), wav, offset=int(wavcenter), axis=1, dtype=self.dtype)
         self._ws = {self._tdtype: torch.empty(self.shape[0], dtype=self._tdtype, device="cuda")}
 
@@ -459,10 +502,27 @@ class Kirchhoff(_KernelOperator):
         """float32 / float64 data are applied in ``promote(dtype, xdt)``; complex data part by part"""
         return torch.promote_types(self._tdtype, xdt) if xdt in (torch.float32, torch.float64) else self._tdtype
 
+    def _tables(self, i0, nc):
+        """the tables of image points [i0, i0 + nc) into ``_ts`` / ``_tr``, rows of nc points"""
+        ay, ax, az = self._axes
+        for pts, tab in ((self._srcs, self._ts), (self._recs, self._tr)):
+            _lib.check(_lib.lib.b2_kirchhoff_tables(_lib.ctx(), _lib.ptr(ay), ax.data_ptr(), az.data_ptr(), self.ny,
+                                                    self.nx, self.nz, pts.data_ptr(), pts.shape[1], self._vel, i0, nc,
+                                                    tab.data_ptr(), _lib.stream()), "b2_kirchhoff_tables")
+
     def _kirch(self, x, y, real, adjoint):
-        _lib.check(_lib.lib.b2_kirchhoff(_lib.ctx(), x.data_ptr(), y.data_ptr(), self._ts.data_ptr(),
-                                         self._tr.data_ptr(), self.ni, self.ns, self.nr, self.nt, self.dt,
-                                         adjoint, _lib.code(real), _lib.stream()), "b2_kirchhoff")
+        if not self.chunked:
+            _lib.check(_lib.lib.b2_kirchhoff(_lib.ctx(), x.data_ptr(), y.data_ptr(), self._ts.data_ptr(),
+                                             self._tr.data_ptr(), self.ni, self.ns, self.nr, self.nt, self.dt,
+                                             adjoint, _lib.code(real), _lib.stream()), "b2_kirchhoff")
+            return
+        for i0 in range(0, self.ni, self._nc):
+            nc = min(self._nc, self.ni - i0)
+            self._tables(i0, nc)
+            _lib.check(_lib.lib.b2_kirchhoff_chunk(_lib.ctx(), x.data_ptr(), y.data_ptr(), self._ts.data_ptr(),
+                                                   self._tr.data_ptr(), self.ni, i0, nc, self.ns, self.nr, self.nt,
+                                                   self.dt, adjoint, int(i0 > 0 and not adjoint), _lib.code(real),
+                                                   _lib.stream()), "b2_kirchhoff_chunk")
 
     def _launch(self, x, y, dt, adjoint):
         ws = self._ws.get(dt)
