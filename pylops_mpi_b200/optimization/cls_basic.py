@@ -5,10 +5,11 @@ reference takes from pylops (callbacks, timing, banner) is restated minimally.
 Two execution modes, same numbers:
   * generic: the reference's exact sequence of DistributedArray operations;
   * fused (default on device arrays): identical recurrences, but axpy-style
-    updates run in place (no temporaries) and reductions that the reference
-    issues back to back are computed in one launch + one Allreduce
-    (q.q and c.c together; s.s and x.x together), cutting the five
-    host-synchronised reductions per iteration (:389-401) to three.
+    updates run in place (no temporaries), the reductions they feed are fused
+    into them and the step scalars stay on the device.  CGLS has ONE fused
+    iteration (``CGLS._body``): ``step()`` runs it eagerly and reads its
+    scalars with one host synchronisation, ``run()`` replays it as a CUDA
+    graph and reads them once per block, so every mode gives the same bits.
 """
 from __future__ import annotations
 
@@ -124,23 +125,17 @@ def _absdot(a: DistributedArray, b: DistributedArray) -> float:
 
 def _self_dots(arrs: Sequence[DistributedArray]) -> List[float]:
     """[|a . conj(a)| for a in arrs] in ONE kernel launch + ONE Allreduce + ONE host sync"""
-    import ctypes as C
     k = len(arrs)
-    a0 = arrs[0]
     views = [a._scatter_view() for a in arrs]
-    n = views[0].numel()
-    same = all(v.numel() == n and v.dtype == views[0].dtype for v in views) and \
-        all(a.sub_comm is a0.sub_comm for a in arrs)
+    same = all(v.numel() == views[0].numel() and v.dtype == views[0].dtype for v in views) and \
+        all(a.sub_comm is arrs[0].sub_comm for a in arrs)
     if not same or k > 4:
         return [_absdot(a, a) for a in arrs]
-    cx = views[0].dtype.is_complex
     out = torch.zeros(2 * k, dtype=torch.float64, device=views[0].device)
-    ptrs = (C.c_void_p * k)(*[v.data_ptr() if n else None for v in views])
-    _lib.check(_lib.lib.b2_dot_multi(_lib.ctx(), k, ptrs, ptrs, n, _lib.code(views[0].dtype), 1,
-                                     out.data_ptr(), _lib.stream()), "b2_dot_multi")
-    allreduce_(a0.sub_comm, out, "sum")
+    _dots_device(arrs, out)
+    allreduce_(arrs[0].sub_comm, out, "sum")
     res = out.cpu().numpy()
-    if cx:
+    if views[0].dtype.is_complex:
         return [float(np.abs(complex(res[2 * i], res[2 * i + 1]))) for i in range(k)]
     return [float(np.abs(res[i])) for i in range(k)]
 
@@ -310,14 +305,11 @@ class CGLS(Solver):
             r.axpy_(-damp, x)                       # r = Op^H s - damp * x   (:341-342)
         self.rank = x.rank
         self.c = r.copy()
-        self.q = self.Op.matvec(self.c)
         self.kold = _self_dots([r])[0]
-        # device-resident scalars for the fused step: [qq, cc | k, ss, xx | a, b | kold] (x2 if complex)
-        # slot stride of the packed device scalars: (re, im) pairs as soon as ANY of the arrays is complex (a real
-        # model with complex-typed data, as in MPIMDC, must not let a complex dot spill into its neighbour's slot)
         self._st = 2 if (x._tdtype.is_complex or self.s._tdtype.is_complex or self.c._tdtype.is_complex) else 1
         self._dev = torch.zeros(16, dtype=torch.float64, device=x.local_array.device)
-        self._dev[14] = self.kold
+        self._dev[self._slots()[-1]] = self.kold
+        self._cc_ready = False                      # the first body computes c.c itself
         self.cost = []
         self.cost1 = []
         ss, xx = _self_dots([self.s, x]) if self.s.local_shape == x.local_shape else \
@@ -369,54 +361,41 @@ class CGLS(Solver):
         return x
 
     def step(self, x, show: bool = False):
-        """One CGLS iteration (cls_basic.py:370-404) with the scalars a, b kept on the device:
-        2 Allreduces and ONE host synchronisation per iteration (the reference: 5 and 5)."""
+        """One CGLS iteration (cls_basic.py:370-404): the fused body run eagerly, 2 Allreduces and ONE host
+        synchronisation (the reference: 5 and 5)."""
         if self._gen:
             return self._step_generic(x, show)
-        dev, st = self._dev, self._st
-        QQ, CC, K, SS, XX, A_, B_, KOLD = 0, st, 4, 4 + st, 4 + 2 * st, 12, 13, 14
-        sub = self.c.sub_comm
-        if getattr(self, "_q_stale", False):       # a block run (rotated order) left q one matvec behind
-            self.q = self.Op.matvec(self.c)
-            self._q_stale = False
-        # a = |kold / (q.q + damp c.c)|                                                  (:389)
-        _dots_device([self.q], dev, QQ)
-        _dots_device([self.c], dev, CC)
-        allreduce_(sub, dev[0:2 * st], "sum")
-        _scalar_div(dev, A_, dev, KOLD, dev, QQ, dev, CC, self.damp)
-        _lincomb_dev(x, dev, A_, 1.0, self.c, None, 0, 1.0, x)            # x += a c       (:390)
-        _lincomb_dev(self.s, dev, A_, -1.0, self.q, None, 0, 1.0, self.s)  # s -= a q       (:391)
-        r = self.Op.rmatvec(self.s)                                        # r = Op^H s - damp x
-        if self.damp != 0.0:
-            r.axpy_(-self.damp, x)
-        _dots_device([r], dev, K)
-        _dots_device([self.s], dev, SS)
-        _dots_device([x], dev, XX)
-        allreduce_(sub, dev[4:4 + 3 * st], "sum")
-        _scalar_div(dev, B_, dev, K, dev, KOLD)                            # b = k / kold   (:395)
-        _lincomb_dev(self.c, None, 0, 1.0, r, dev, B_, 1.0, self.c)        # c = r + b c    (:396)
-        self.q = self.Op.matvec(self.c)
-        host = dev[4:4 + 3 * st].cpu().numpy()                             # the one sync of the iteration
-        dev[KOLD:KOLD + 1].copy_(dev[K:K + 1])
-        k, ss, xx = (float(abs(host[i * st])) for i in range(3))
-        self.kold = k
-        self.iiter += 1
-        self.cost.append(float(np.sqrt(ss)))
-        self.cost1.append(np.sqrt(float(self.cost[self.iiter] ** 2 + self.damp * xx)))
+        hist = torch.empty((1, 3), dtype=torch.float64, device=self._dev.device)
+        self._body(x, hist, torch.zeros(1, dtype=torch.int64, device=hist.device))
+        self._absorb(hist[0].cpu().numpy())
         if show and self.rank == 0:
             self._print_step(x)
         return x
 
-    # ---- block execution: iterations without host round trips, replayed as ONE CUDA graph per iteration -----------
+    def _slots(self):
+        """offsets in ``_dev`` of the fused iteration's scalars [q.q, c.c | k, s.s, x.x | a, b | kold]; dots take
+        (re, im) pairs as soon as ANY of the arrays is complex (a real model with complex-typed data, as in MPIMDC,
+        must not let a complex dot spill into its neighbour's slot)"""
+        st = self._st
+        return 0, st, 4, 4 + st, 4 + 2 * st, 12, 13, 14
+
+    def _absorb(self, row) -> None:
+        """host-side bookkeeping of one iteration from its history row (k, s.s, x.x)"""
+        k, ss, xx = row
+        self.kold = float(k)
+        self.iiter += 1
+        self.cost.append(float(np.sqrt(ss)))
+        self.cost1.append(np.sqrt(float(self.cost[self.iiter] ** 2 + self.damp * xx)))
+
     def _body(self, x, hist: torch.Tensor, it_dev: torch.Tensor):
         """one CGLS iteration in ROTATED order (q = Op c first): every array that crosses iterations (x, s, c) is
-        updated in place and q, r live and die inside the body, so the captured graph can be replayed verbatim.
-        Same recurrences and the same kernels as :meth:`step`; the three per-iteration scalars go to ``hist``."""
+        updated in place and q, r live and die inside the body, so a captured graph can be replayed verbatim.  No
+        host synchronisation: the three per-iteration scalars go to ``hist[it_dev]``."""
         dev, st = self._dev, self._st
-        QQ, CC, K, SS, XX, A_, B_, KOLD = 0, st, 4, 4 + st, 4 + 2 * st, 12, 13, 14
+        QQ, CC, K, SS, XX, A_, B_, KOLD = self._slots()
         sub = self.c.sub_comm
-        self.q = self.Op.matvec(self.c)
-        _dots_device([self.q], dev, QQ)
+        q = self.Op.matvec(self.c)
+        _dots_device([q], dev, QQ)
         if not self._cc_ready:                      # c.c normally comes fused with the update of c (end of the body)
             _dots_device([self.c], dev, CC)
         allreduce_(sub, dev[0:2 * st], "sum")
@@ -424,7 +403,7 @@ class CGLS(Solver):
         # x += a c (+ x.x), s -= a q (+ s.s): update and the reduction the cost needs, one pass each
         if not _lincomb_dev_norm2(x, dev, A_, 1.0, self.c, None, 0, 1.0, x, dev, XX):
             _dots_device([x], dev, XX)
-        if not _lincomb_dev_norm2(self.s, dev, A_, -1.0, self.q, None, 0, 1.0, self.s, dev, SS):
+        if not _lincomb_dev_norm2(self.s, dev, A_, -1.0, q, None, 0, 1.0, self.s, dev, SS):
             _dots_device([self.s], dev, SS)
         r = self.Op.rmatvec(self.s)
         if self.damp != 0.0:
@@ -438,120 +417,95 @@ class CGLS(Solver):
                                             hist.shape[0], dev.data_ptr() + 8 * KOLD, dev.data_ptr() + 8 * K,
                                             _lib.stream()), "b2_history_push")
 
+    def _iterate(self, x, hist: torch.Tensor, it_dev: torch.Tensor):
+        """one iteration of a block run: the first runs eagerly (every kernel of the body gets loaded, lazy
+        workspaces and communicators exist), then the body is captured once as a CUDA graph and replayed"""
+        if self._graph is None and self._capture and self._warm:
+            t_cap = time.perf_counter()
+            try:
+                # manual capture on a side stream (torch.cuda.graph() would add a device synchronise, a
+                # gc.collect() and an empty_cache() -- milliseconds, comparable to a whole 50-iteration solve)
+                pool = _graph_pool()
+                t_pool = time.perf_counter()
+                g = torch.cuda.CUDAGraph()
+                main = torch.cuda.current_stream()
+                side = torch.cuda.Stream()
+                side.wait_stream(main)
+                with torch.cuda.stream(side):
+                    # one process-wide memory pool for all captures: the temporaries of the first capture are
+                    # cudaMalloc'ed (slow when peers have this device mapped: measured 3.1 ms at 2 GPUs vs 0.65 ms
+                    # at 1), later captures reuse the cached blocks
+                    # thread_local error mode: NCCL's helper threads keep polling CUDA while we capture
+                    # (observed at 8 ranks: a "global"-mode capture was invalidated and left torch's RNG state
+                    # stuck in capture mode)
+                    g.capture_begin(pool=pool, capture_error_mode="thread_local")   # records only
+                    t_begin = time.perf_counter()
+                    try:
+                        self._body(x, hist, it_dev)
+                    finally:
+                        t_body = time.perf_counter()
+                        g.capture_end()
+                main.wait_stream(side)
+                self._graph = g
+                t_end = time.perf_counter()
+                self.graph_capture_ms = (t_end - t_cap) * 1e3
+                self.graph_capture_breakdown_ms = {"pool": (t_pool - t_cap) * 1e3, "begin": (t_begin - t_pool) * 1e3,
+                                                   "body": (t_body - t_begin) * 1e3, "end": (t_end - t_body) * 1e3}
+            except Exception as exc:               # not capturable (host sync inside an operator ...): stay eager
+                self._capture = False
+                self.graph_error = repr(exc)[:300]
+                print(f"[b200 cgls] CUDA-graph capture failed, running eagerly: {self.graph_error}", file=sys.stderr)
+                torch.cuda.synchronize()
+                _reset_capture_state()
+        if self._graph is not None:
+            self._graph.replay()
+            self.graph_replays += 1
+        else:
+            self._body(x, hist, it_dev)
+            self._warm = True
+
     def _run_blocks(self, x, niter: int):
-        """remaining iterations in blocks: the body is captured ONCE in a CUDA graph (after one eager warm-up
-        iteration) and replayed; the host reads the scalar history once per block.  With tol > 0 a block is at
-        most 8 iterations and is re-run from a checkpoint up to the stopping iteration, so x, cost and the
-        iteration count are exactly those of the reference's per-iteration test ``kold > tol`` (cls_basic.py:436)."""
+        """remaining iterations in blocks of :meth:`_iterate`; the host reads the scalar history once per block.
+        With tol > 0 a block is at most 8 iterations and is re-run from a checkpoint up to the stopping iteration,
+        so x, cost and the iteration count are exactly those of the reference's per-iteration test ``kold > tol``
+        (cls_basic.py:436)."""
         device = x.local_array.device
-        total = niter - self.iiter
-        hist = torch.zeros((total + 2, 3), dtype=torch.float64, device=device)
+        it0 = self.iiter
+        hist = torch.zeros((niter - it0 + 2, 3), dtype=torch.float64, device=device)
         it_dev = torch.zeros(1, dtype=torch.int64, device=device)
-        done = [0]          # iterations whose scalars are in hist
-
-        def absorb(upto: int):
-            """move hist[done:upto] to the host-side cost arrays; returns the first stop index or None"""
-            rows = hist[done[0]:upto].cpu().numpy()
-            stop = None
-            for i, (k, ss, xx) in enumerate(rows):
-                self.kold = float(k)
-                self.iiter += 1
-                self.cost.append(float(np.sqrt(ss)))
-                self.cost1.append(np.sqrt(float(self.cost[self.iiter] ** 2 + self.damp * xx)))
-                if not (self.iiter < niter and self.kold > self.tol):
-                    stop = done[0] + i + 1
-                    break
-            done[0] = upto if stop is None else stop
-            return stop
-
-        def rewind(ckpt, upto_it: int):
-            xs, ss_, cs = ckpt
-            for dst, src in ((x, xs), (self.s, ss_), (self.c, cs)):
-                dst.local_array.copy_(src)
-            self._dev[14] = self._kold_ckpt
-            it_dev.fill_(upto_it)
-            if self._cc_ready:                      # the fused c.c partial belongs to the restored c again
-                _dots_device([self.c], self._dev, self._st)
-
-        use_graph = _graph_safe(self.Op)
-        state = {"graph": None, "use": use_graph, "warm": 0}
-        self.graph_replays, self.graph_error = 0, (None if use_graph else "operator not on the graph-safe list")
-        self._cc_ready = False                      # first body computes c.c itself
-
-        def one():
-            """one iteration: the first runs eagerly (every kernel of the body gets loaded, lazy workspaces and
-            communicators exist), then the body is captured once and replayed"""
-            if state["graph"] is None and state["use"] and state["warm"] >= 1:
-                t_cap = time.perf_counter()
-                try:
-                    # manual capture on a side stream (torch.cuda.graph() would add a device synchronise, a
-                    # gc.collect() and an empty_cache() -- milliseconds, comparable to a whole 50-iteration solve)
-                    pool = _graph_pool()
-                    t_pool = time.perf_counter()
-                    g = torch.cuda.CUDAGraph()
-                    main = torch.cuda.current_stream()
-                    if state.get("stream") is None:
-                        state["stream"] = torch.cuda.Stream()
-                    side = state["stream"]
-                    side.wait_stream(main)
-                    with torch.cuda.stream(side):
-                        # one process-wide memory pool for all captures: the temporaries of the first capture are
-                        # cudaMalloc'ed (slow when peers have this device mapped: measured 3.1 ms at 2 GPUs vs 0.65 ms
-                        # at 1), later captures reuse the cached blocks
-                        # thread_local error mode: NCCL's helper threads keep polling CUDA while we capture
-                        # (observed at 8 ranks: a "global"-mode capture was invalidated and left torch's RNG state
-                        # stuck in capture mode)
-                        g.capture_begin(pool=pool, capture_error_mode="thread_local")   # records only
-                        t_begin = time.perf_counter()
-                        try:
-                            self._body(x, hist, it_dev)
-                        finally:
-                            t_body = time.perf_counter()
-                            g.capture_end()
-                    main.wait_stream(side)
-                    state["graph"] = g
-                    self.graph_replays = 0
-                    t_end = time.perf_counter()
-                    self.graph_capture_ms = (t_end - t_cap) * 1e3
-                    self.graph_capture_breakdown_ms = {"pool": (t_pool - t_cap) * 1e3, "begin": (t_begin - t_pool) * 1e3,
-                                                       "body": (t_body - t_begin) * 1e3, "end": (t_end - t_body) * 1e3}
-                except Exception as exc:               # not capturable (host sync inside an operator ...): stay eager
-                    state["use"] = False
-                    self.graph_error = repr(exc)[:300]
-                    print(f"[b200 cgls] CUDA-graph capture failed, running eagerly: {self.graph_error}", file=sys.stderr)
-                    torch.cuda.synchronize()
-                    _reset_capture_state()
-            if state["graph"] is not None:
-                state["graph"].replay()
-                self.graph_replays += 1
-            else:
-                self._body(x, hist, it_dev)
-                state["warm"] += 1
-
-        block = total if self.tol <= 0.0 else min(total, 8)
+        self._graph, self._warm, self._capture = None, False, _graph_safe(self.Op)
+        self.graph_replays, self.graph_error = 0, (None if self._capture else "operator not on the graph-safe list")
+        block = niter - it0 if self.tol <= 0.0 else 8
         while self.iiter < niter and self.kold > self.tol:
             n = min(block, niter - self.iiter)
-            start = done[0]
-            ckpt = tuple(a.local_array.clone() for a in (x, self.s, self.c))
-            self._kold_ckpt = float(self.kold)
+            start = self.iiter - it0
+            live = (x.local_array, self.s.local_array, self.c.local_array, self._dev)
+            ckpt, cc_ready = [a.clone() for a in live], self._cc_ready
             for _ in range(n):
-                one()
-            stop = absorb(start + n)
-            if stop is not None and stop < start + n:
+                self._iterate(x, hist, it_dev)
+            for i, row in enumerate(hist[start:start + n].cpu().numpy()):
+                self._absorb(row)
+                if not (self.iiter < niter and self.kold > self.tol):
+                    break
+            if i + 1 < n:
                 # the stopping test fired inside the block: redo exactly the iterations up to it from the checkpoint
-                rewind(ckpt, start)
-                for _ in range(stop - start):
-                    one()
+                for dst, src in zip(live, ckpt):
+                    dst.copy_(src)
+                it_dev.fill_(start)
+                if self._cc_ready and not cc_ready:     # c.c of the restored c, as the first body computed it
+                    _dots_device([self.c], self._dev, self._slots()[1])
+                for _ in range(i + 1):
+                    self._iterate(x, hist, it_dev)
             del ckpt
-        self._q_stale = True        # rotated order: q is one matvec behind c (and lives in the graph's memory pool)
-        self.q = None
+        self._graph = None
         return x
 
     def run(self, x, niter: Optional[int] = None, show: bool = False, itershow=(10, 10, 10)):
         niter = self.niter if niter is None else niter
         if niter is None:
             raise ValueError("niter must not be None")
-        plain_callback = type(self).callback is Solver.callback and not self.callbacks
+        # a callback, overridden in a subclass or set on the instance (cgls(callback=...)), sees every iteration
+        plain_callback = type(self).callback is Solver.callback and "callback" not in vars(self) and not self.callbacks
         if not self._gen and not show and plain_callback and niter - self.iiter > 0:
             return self._run_blocks(x, niter)
         while self.iiter < niter and self.kold > self.tol:

@@ -571,8 +571,8 @@ def test_cgls_graph_replay_matches_step_loop(pm, layout):
     for _ in range(25):
         xb = b.step(xb)
     b.finalize()
-    np.testing.assert_allclose(host(xa.asarray()), host(xb.asarray()), rtol=1e-12, atol=1e-12)
-    np.testing.assert_allclose(np.asarray(a.cost), np.asarray(b.cost), rtol=1e-12)
+    np.testing.assert_array_equal(host(xa.asarray()), host(xb.asarray()))
+    np.testing.assert_array_equal(np.asarray(a.cost), np.asarray(b.cost))
 
 
 @pytest.mark.gpu
