@@ -39,7 +39,7 @@ enum { B2_THRESH_NONE = 0, B2_THRESH_SOFT = 1, B2_THRESH_HARD = 2, B2_THRESH_HAL
 
 /* error codes >= 2000 are library-level */
 enum { B2_OK = 0, B2_ERR_DTYPE = 2001, B2_ERR_ARG = 2002, B2_ERR_HALO = 2003,
-       B2_ERR_WORKSPACE = 2004, B2_ERR_UNSUPPORTED = 2005, B2_ERR_ALIGN = 2006 };
+       B2_ERR_WORKSPACE = 2004, B2_ERR_UNSUPPORTED = 2005, B2_ERR_ALIGN = 2006, B2_ERR_CONVERGE = 2007 };
 
 /* per-device context: SM count + the reduction workspace (per-CTA partials, ticket counter) shared by b2_dot /
  * b2_norm_partial / b2_dot_multi / b2_sparse_update / the transposed b2_gemv.  Calls that use the workspace must be
@@ -195,6 +195,24 @@ int b2_kirchhoff_chunk(b2_ctx* ctx, const void* x, void* y, const double* trav_s
 int b2_kirchhoff_tables(b2_ctx* ctx, const double* y, const double* x, const double* z, size_t ny, size_t nx,
                         size_t nz, const double* pts, size_t n, double vel, size_t i0, size_t nc, double* table,
                         void* stream);
+/* eikonal traveltime tables for pylops.waveeqprocessing.Kirchhoff(mode="eikonal") in b2_kirchhoff's layout:
+ * table[p][ii] (row stride ny * nx * nz, float64) is the first-arrival time from grid node idx_host[p] = (iy, ix, iz)
+ * (a HOST array [n][3]) through the velocity model vel [ny][nx][nz] (float64, ii = (iy * nx + ix) * nz + iz; 2-D is
+ * ny = 1) on a grid of spacings dy, dx, dz.  The values are the iterate after max_iter Jacobi steps of the
+ * first-order Godunov upwind update written out in csrc/eikonal.cu (T = 0 at the node, +inf elsewhere at the start),
+ * rounded to nearest operation by operation: equal bit for bit to its NumPy restatement.  work is a device buffer
+ * of b2_eikonal_work_bytes(ny, nx, nz, n) bytes, 8-byte aligned; info_host, if not NULL, receives 4 host words: the
+ * Jacobi steps that changed a value (capped at max_iter), the passes run, the (tile, point) blocks computed and the
+ * blocks of all passes.  Reads the device several times (construction-time, not capturable).  No allocation.
+ * B2_ERR_ARG: a null pointer (info_host excepted), a zero size or max_iter, a node outside the grid, a spacing that
+ * is not finite and positive, a velocity that is not finite and positive (table is untouched on these);
+ * B2_ERR_CONVERGE: the max_iter-th iterate is not the fixed point (table holds that iterate) */
+int b2_eikonal_tables(b2_ctx* ctx, const double* vel, size_t ny, size_t nx, size_t nz, double dy, double dx,
+                      double dz, const long long* idx_host, size_t n, size_t max_iter, double* table, void* work,
+                      long long* info_host, void* stream);
+/* bytes of b2_eikonal_tables' work buffer for n points on an ny x nx x nz grid, about (n + 1) * ny * nx * nz * 8
+ * (one more iterate and the slowness); 0 for a zero or too large size */
+size_t b2_eikonal_work_bytes(size_t ny, size_t nx, size_t nz, size_t n);
 /* Peer-memory halo exchange fused INTO the stencil kernel (replaces the add_ghost_cells Send/Recv pairs of
  * DistributedArray.py:876-953 as used by FirstDerivative.py:221-247, 276-319 and SecondDerivative.py): every rank
  * owns a box of b2_halo_bytes(cap) bytes in IPC-mapped memory (b2_symm_alloc + b2_ipc_*); boxes_host[r] is rank r's

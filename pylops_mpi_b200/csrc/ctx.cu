@@ -16,6 +16,7 @@ extern "C" const char* b2_strerror(int code) {
       case B2_ERR_WORKSPACE: return "b200lops: internal workspace too small";
       case B2_ERR_UNSUPPORTED: return "b200lops: unsupported kind/order";
       case B2_ERR_ALIGN: return "b200lops: pointer alignment requirement not met";
+      case B2_ERR_CONVERGE: return "b200lops: iteration did not reach its fixed point within max_iter";
       default: return "b200lops: unknown library error";
     }
   }

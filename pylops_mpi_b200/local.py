@@ -9,6 +9,7 @@ reference test / BASELINE config uses, applied by the b2_gemv kernels.
 from __future__ import annotations
 
 import copy
+import ctypes as C
 import math
 
 import numpy as np
@@ -417,41 +418,84 @@ def _traveltime_tables(z, x, srcs, recs, vel, y=None):
 
 
 # Device memory the resident traveltime tables of one Kirchhoff operator may take, (ns + nr) * ni * 8 bytes.  Above
-# it the operator keeps one chunk of image points' tables (a multiple of 32 points within the budget) and rebuilds
-# them for each chunk on every apply.  Read when an operator is constructed.
+# it an analytic operator keeps one chunk of image points' tables (a multiple of 32 points within the budget) and
+# rebuilds them for each chunk on every apply; eikonal and byot operators raise ValueError (with mode="eikonal" the
+# solver's work buffer counts too).  Read when an operator is constructed.
 KIRCHHOFF_TABLE_BYTES = 4 << 30
 
 
-class Kirchhoff(_KernelOperator):
-    """Rank-local Kirchhoff demigration, pylops.waveeqprocessing.Kirchhoff (pylops 2.x) with ``mode="analytic"`` in
-    2-D or, with ``y``, 3-D: the ``Demop`` of tutorials/lsm.py inside MPIVStack.  The model is the image ``(nx, nz)``
-    (3-D: ``(ny, nx, nz)``, with ``srcs`` / ``recs`` of shape ``(3, n)``, rows ``(y, x, z)``), the data the traces
-    ``(ns, nr, nt)``.  For every (image point, trace) pair the traveltime ``trav`` indexes the trace at
-    ``it = int(trav / dt)`` with weights ``1 - d`` and ``d`` on samples ``it`` and ``it + 1`` (``d = trav / dt - it``,
-    pairs with ``it >= nt - 1`` are dropped); the traces are then convolved with ``wav`` (``Convolve1D`` with
-    ``offset=wavcenter`` along time).
+def _uniform_spacing(name, a):
+    """the sampling of a uniform, increasing axis (1.0 for a one-point axis), else ValueError"""
+    if a.size < 2:
+        return 1.0
+    d = float(a[1] - a[0])
+    if not (d > 0.0 and np.isfinite(d)) or not np.allclose(np.diff(a), d, rtol=1e-6, atol=0.0):
+        raise ValueError(f"Kirchhoff: mode='eikonal' needs uniform, increasing axes; {name} is not")
+    return d
 
-    The float64 traveltime tables are built on the device (b2_kirchhoff_tables), equal bit for bit to pylops' NumPy
-    tables.  While ``(ns + nr) * ni * 8`` bytes fit in :data:`KIRCHHOFF_TABLE_BYTES` they are built once at
-    construction and stay resident; above it (``chunked``) the operator holds one chunk of image points' tables and
-    each apply builds and applies them chunk by chunk (b2_kirchhoff_chunk), with the same result bit for bit.  A
-    workspace of ``ns * nr * nt`` samples holds the traces between the two stages.  Forward: spreading into the
-    workspace, then b2_convolve_axis into the output; adjoint: the reverse (csrc/kirchhoff.cu, csrc/convolve.cu).
-    Only the analytic, static (``dynamic=False``) operator without wavelet filtering, apertures, or user tables is
-    provided; ``engine`` is accepted and ignored."""
+
+def _user_table(name, tab, ni, n):
+    """one byot table, pylops' shape (ni, n), in any real dtype -> the kernel layout (n, ni), float64, on the device"""
+    tab = tab if isinstance(tab, torch.Tensor) else torch.as_tensor(np.asarray(tab))
+    if tab.is_complex() or tab.dtype == torch.bool or tab.dim() != 2 or tuple(tab.shape) != (ni, n):
+        raise ValueError(f"Kirchhoff: mode='byot' needs {name} as a real array of shape ({ni}, {n}); got "
+                         f"{tab.dtype} {tuple(tab.shape)}")
+    return tab.to(device="cuda", dtype=torch.float64).t().contiguous()
+
+
+class Kirchhoff(_KernelOperator):
+    """Rank-local Kirchhoff demigration, pylops.waveeqprocessing.Kirchhoff (pylops 2.x) in 2-D or, with ``y``, 3-D:
+    the ``Demop`` of tutorials/lsm.py inside MPIVStack.  The model is the image ``(nx, nz)`` (3-D: ``(ny, nx, nz)``,
+    with ``srcs`` / ``recs`` of shape ``(3, n)``, rows ``(y, x, z)``), the data the traces ``(ns, nr, nt)``.  For
+    every (image point, trace) pair the traveltime ``trav`` indexes the trace at ``it = int(trav / dt)`` with weights
+    ``1 - d`` and ``d`` on samples ``it`` and ``it + 1`` (``d = trav / dt - it``, pairs with ``it >= nt - 1`` are
+    dropped); the traces are then convolved with ``wav`` (``Convolve1D`` with ``offset=wavcenter`` along time).
+
+    The float64 traveltime tables come from ``mode``:
+
+    - ``"analytic"``: constant velocity, scalar ``vel``.  Built on the device (b2_kirchhoff_tables), equal bit for
+      bit to pylops' NumPy tables.  While ``(ns + nr) * ni * 8`` bytes fit in :data:`KIRCHHOFF_TABLE_BYTES` they are
+      built once at construction and stay resident; above it (``chunked``) the operator holds one chunk of image
+      points' tables and each apply builds and applies them chunk by chunk (b2_kirchhoff_chunk), with the same
+      result bit for bit.
+    - ``"eikonal"``: ``vel`` a finite, positive velocity model of the image's shape on uniform axes.  Each source and
+      receiver is snapped to its nearest grid node (half to even) and its first-arrival times are solved on the
+      device (b2_eikonal_tables, a first-order Godunov upwind scheme iterated to its fixed point, ``max_iter = ni``),
+      once at construction.  pylops uses scikit-fmm here, whose second-order scheme puts the zero level set half a
+      cell from the node: the tables differ from pylops' by O(h / v), most near the source.  Pass scikit-fmm's
+      tables through ``"byot"`` to reproduce pylops exactly.
+    - ``"byot"``: ``trav=(trav_srcs, trav_recs)`` of pylops' shapes ``(ni, ns)`` / ``(ni, nr)``, NumPy arrays or
+      torch tensors of any real dtype, converted to float64 once; ``vel`` is ignored.
+
+    ``trav_srcs`` / ``trav_recs`` are ``(ni, ns)`` / ``(ni, nr)`` views of the resident device tables (not of a
+    chunked analytic operator).  A workspace of ``ns * nr * nt`` samples holds the traces between the two stages.
+    Forward: spreading into the workspace, then b2_convolve_axis into the output; adjoint: the reverse
+    (csrc/kirchhoff.cu, csrc/convolve.cu).  Only the static (``dynamic=False``) operator without wavelet filtering
+    or apertures is provided; ``engine`` is accepted and ignored."""
 
     def __init__(self, z, x, t, srcs, recs, vel, wav, wavcenter, y=None, mode="eikonal", wavfilter=False,
                  dynamic=False, trav=None, amp=None, aperture=None, angleaperture=90, snell=None, engine="numpy",
                  dtype="float64", name="K"):
         for opt, val, default in (("wavfilter", wavfilter, False), ("dynamic", dynamic, False),
-                                  ("trav", trav, None), ("amp", amp, None), ("aperture", aperture, None),
+                                  ("amp", amp, None), ("aperture", aperture, None),
                                   ("angleaperture", angleaperture, 90), ("snell", snell, None)):
             if not (val is default or (default is not None and np.ndim(val) == 0 and val == default)):
                 raise NotImplementedError(f"Kirchhoff: {opt}={val!r} is not supported (only its default {default!r})")
-        if mode != "analytic":
-            raise NotImplementedError(f"Kirchhoff: mode={mode!r} is not supported (only mode='analytic')")
-        if np.ndim(vel) != 0:
+        if mode not in ("analytic", "eikonal", "byot"):
+            raise NotImplementedError(f"Kirchhoff: mode={mode!r} is not supported (analytic, eikonal or byot)")
+        if trav is not None and mode != "byot":
+            raise NotImplementedError(f"Kirchhoff: trav is only used with mode='byot' (mode={mode!r})")
+        if mode == "analytic" and np.ndim(vel) != 0:
             raise ValueError("vel must be scalar for mode=analytical")
+        if mode == "eikonal" and np.ndim(vel) == 0:
+            raise NotImplementedError("Kirchhoff: mode='eikonal' needs a velocity model of the image's shape; a "
+                                      "scalar vel (constant velocity) is mode='analytic'")
+        if mode == "byot":
+            if trav is None:
+                raise NotImplementedError("Kirchhoff: mode='byot' needs trav=(trav_srcs, trav_recs)")
+            if isinstance(trav, (np.ndarray, torch.Tensor)) or len(trav) != 2:
+                raise NotImplementedError("Kirchhoff: trav as one (ni, ns * nr) table is not supported: pass "
+                                          "trav=(trav_srcs, trav_recs) of shapes (ni, ns) and (ni, nr)")
         z, x, t = (np.asarray(a) for a in (z, x, t))
         srcs, recs = np.asarray(srcs), np.asarray(recs)
         nd = 2 if y is None else 3
@@ -463,6 +507,7 @@ class Kirchhoff(_KernelOperator):
         wav = wav.detach().cpu().numpy() if isinstance(wav, torch.Tensor) else np.asarray(wav)
         if np.iscomplexobj(wav) or wav.ndim != 1:
             raise NotImplementedError("Kirchhoff: only a real 1-D wavelet is supported")
+        self.mode = mode
         self.ny = 1 if y is None else np.asarray(y).size
         self.nx, self.nz, self.nt = x.size, z.size, t.size
         self.ns, self.nr = srcs.shape[1], recs.shape[1]
@@ -477,7 +522,28 @@ class Kirchhoff(_KernelOperator):
         if self._tdtype not in (torch.float32, torch.float64):
             raise NotImplementedError(f"Kirchhoff: dtype {dtype} is not supported (float32 or float64)")
         _lib.ctx()
+        table_bytes = (self.ns + self.nr) * self.ni * 8
+        if mode == "analytic":
+            self._analytic(y, x, z, srcs, recs, vel)
+        else:
+            if mode == "byot":
+                self._check_budget(table_bytes, "")
+                self._ts = _user_table("trav_srcs", trav[0], self.ni, self.ns)
+                self._tr = _user_table("trav_recs", trav[1], self.ni, self.nr)
+            else:
+                self._eikonal(y, x, z, srcs, recs, vel, table_bytes)
+            self._nc, self.chunked = self.ni, False
+        self.cop = Convolve1D((self.ns * self.nr, self.nt), wav, offset=int(wavcenter), axis=1, dtype=self.dtype)
+        self._ws = {self._tdtype: torch.empty(self.shape[0], dtype=self._tdtype, device="cuda")}
 
+    @staticmethod
+    def _check_budget(need, what):
+        if need > KIRCHHOFF_TABLE_BYTES:
+            raise ValueError(f"Kirchhoff: the resident traveltime tables{what} need {need} bytes, more than "
+                             f"KIRCHHOFF_TABLE_BYTES = {KIRCHHOFF_TABLE_BYTES}; only mode='analytic' can rebuild "
+                             f"its tables in chunks")
+
+    def _analytic(self, y, x, z, srcs, recs, vel):
         def dev(a):
             return torch.as_tensor(np.ascontiguousarray(a, dtype=np.float64)).to("cuda")
 
@@ -495,8 +561,71 @@ class Kirchhoff(_KernelOperator):
         self._tr = torch.empty((self.nr, self._nc), dtype=torch.float64, device="cuda")
         if not self.chunked:
             self._tables(0, self.ni)
-        self.cop = Convolve1D((self.ns * self.nr, self.nt), wav, offset=int(wavcenter), axis=1, dtype=self.dtype)
-        self._ws = {self._tdtype: torch.empty(self.shape[0], dtype=self._tdtype, device="cuda")}
+
+    def _eikonal(self, y, x, z, srcs, recs, vel, table_bytes):
+        """the eikonal tables, solved on the device in batches of points whose work buffer fits the budget"""
+        vel = vel.detach().cpu().numpy() if isinstance(vel, torch.Tensor) else np.asarray(vel)
+        if tuple(vel.shape) != self.dims:
+            raise ValueError(f"Kirchhoff: mode='eikonal' needs vel of the image shape {self.dims}; got {vel.shape}")
+        if not (np.issubdtype(vel.dtype, np.integer) or np.issubdtype(vel.dtype, np.floating)):
+            raise ValueError(f"Kirchhoff: mode='eikonal' needs a real vel; got {vel.dtype}")
+        vel = np.ascontiguousarray(vel, dtype=np.float64)
+        if not (np.all(np.isfinite(vel)) and np.all(vel > 0)):
+            raise ValueError("Kirchhoff: mode='eikonal' needs a finite, positive vel")
+        axes = ((("y", np.asarray(y, dtype=np.float64)),) if y is not None else ()) + \
+            (("x", np.asarray(x, dtype=np.float64)), ("z", np.asarray(z, dtype=np.float64)))
+        h = [_uniform_spacing(nm, a) for nm, a in axes]
+        h = [1.0] * (3 - len(h)) + h
+        full = (self.ny, self.nx, self.nz)
+
+        def nodes(name, pts):
+            """grid nodes (n, 3) of the points: round((p - axis[0]) / d), half to even, as pylops"""
+            cols = [np.round((np.asarray(p, dtype=np.float64) - a[0]) / d).astype(np.int64)
+                    for p, (_, a), d in zip(pts, axes, h[3 - len(axes):])]
+            if len(cols) == 2:
+                cols.insert(0, np.zeros_like(cols[0]))
+            nd = np.ascontiguousarray(np.stack(cols, axis=1), dtype=np.int64)
+            bad = np.any((nd < 0) | (nd >= np.asarray(full)), axis=1)
+            if bad.any():
+                raise ValueError(f"Kirchhoff: {name} {np.flatnonzero(bad).tolist()} lie outside the image grid")
+            return nd
+
+        idx_s, idx_r = nodes("sources", srcs), nodes("receivers", recs)
+        wb = _lib.lib.b2_eikonal_work_bytes
+        if table_bytes + wb(*full, 1) > KIRCHHOFF_TABLE_BYTES:
+            self._check_budget(table_bytes + wb(*full, 1), " with the eikonal solver's work buffer")
+        nb = max(self.ns, self.nr)                       # points per solve: as many as the budget allows
+        while table_bytes + wb(*full, nb) > KIRCHHOFF_TABLE_BYTES:
+            nb = max(1, nb // 2)
+        self._ts = torch.empty((self.ns, self.ni), dtype=torch.float64, device="cuda")
+        self._tr = torch.empty((self.nr, self.ni), dtype=torch.float64, device="cuda")
+        dvel = torch.as_tensor(vel).to("cuda")
+        work = torch.empty(wb(*full, nb), dtype=torch.uint8, device="cuda")
+        info = (C.c_longlong * 4)()
+        self.eikonal_info = {"iterations": 0, "passes": 0, "blocks": 0, "blocks_all": 0}
+        for idx, tab in ((idx_s, self._ts), (idx_r, self._tr)):
+            for p0 in range(0, len(idx), nb):
+                part = np.ascontiguousarray(idx[p0:p0 + nb])
+                _lib.check(_lib.lib.b2_eikonal_tables(_lib.ctx(), dvel.data_ptr(), *full, *h, part.ctypes.data,
+                                                      len(part), self.ni, tab[p0].data_ptr(), work.data_ptr(),
+                                                      info, _lib.stream()), "b2_eikonal_tables")
+                for k, v in zip(("iterations", "passes", "blocks", "blocks_all"), info):
+                    self.eikonal_info[k] = max(self.eikonal_info[k], v) if k == "iterations" else \
+                        self.eikonal_info[k] + v
+
+    @property
+    def trav_srcs(self) -> torch.Tensor:
+        """(ni, ns) float64 device view of the resident source tables (pylops' layout)"""
+        if self.chunked:
+            raise AttributeError("Kirchhoff: a chunked analytic operator keeps no resident trav_srcs")
+        return self._ts.t()
+
+    @property
+    def trav_recs(self) -> torch.Tensor:
+        """(ni, nr) float64 device view of the resident receiver tables (pylops' layout)"""
+        if self.chunked:
+            raise AttributeError("Kirchhoff: a chunked analytic operator keeps no resident trav_recs")
+        return self._tr.t()
 
     def _compute_dtype(self, xdt):
         """float32 / float64 data are applied in ``promote(dtype, xdt)``; complex data part by part"""
