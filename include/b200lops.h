@@ -114,6 +114,44 @@ int b2_scalar_div(double* out_dev, const double* num_dev, const double* den1_dev
 int b2_history_push(const double* src_dev, int nvals, int stride, double* hist_dev, void* it_dev, size_t cap,
                     double* copy_dst_dev, const double* copy_src_dev, void* stream);
 
+/* ---- LSQR (optimization/cls_basic.py LSQR; the definition is scipy.sparse.linalg.lsqr, Paige & Saunders 1982) ----
+ * The solver state is one float64 DEVICE array of B2_LSQR_NSTATE doubles at these offsets.  BB / DD and AA are the
+ * (all-reduced) reductions the kernels read: BB = |U|^2 (complex dtypes: BB+1 = 0, as b2_lincomb_dev_norm2 writes it),
+ * DD = |dk|^2 of the previous update, AA = |V|^2.  u and v are kept unnormalised (U = u', V = v' of lsqr.py, norms
+ * beta and alfa); the coefficient slots fold scipy's normalisations into the next combination:
+ *   U <- INV_ALFA * (A V) - CUB * U      V <- CVA * (A^H U) - CVB * V       (b2_lincomb_dev_norm2, b scale -1)
+ * The host fills the constants and the state after scipy's initialisation; every other slot is the kernels'. */
+enum { B2_LSQR_BB = 0, B2_LSQR_DD = 2, B2_LSQR_AA = 4,
+       B2_LSQR_ALFA = 8, B2_LSQR_BETA, B2_LSQR_RHOBAR, B2_LSQR_PHIBAR, B2_LSQR_ANORM, B2_LSQR_DDNORM, B2_LSQR_RES2,
+       B2_LSQR_XXNORM, B2_LSQR_Z, B2_LSQR_CS2, B2_LSQR_SN2, B2_LSQR_ITN, B2_LSQR_ISTOP, B2_LSQR_PENDING,
+       B2_LSQR_STOPPED,
+       B2_LSQR_DAMP = 24, B2_LSQR_DAMPSQ, B2_LSQR_ATOL, B2_LSQR_BTOL, B2_LSQR_CTOL, B2_LSQR_BNORM, B2_LSQR_ITER_LIM,
+       B2_LSQR_R1NORM = 32, B2_LSQR_R2NORM, B2_LSQR_ACOND, B2_LSQR_ARNORM, B2_LSQR_XNORM, B2_LSQR_TEST1,
+       B2_LSQR_TEST2, B2_LSQR_TT1, B2_LSQR_RTOL,
+       B2_LSQR_CUB = 42, B2_LSQR_CVA, B2_LSQR_CVB,
+       B2_LSQR_T1 = 48, B2_LSQR_T2, B2_LSQR_INV_RHO, B2_LSQR_INV_ALFA,     /* b2_lsqr_update's coef_dev */
+       B2_LSQR_SCRATCH = 52, B2_LSQR_NSTATE = 56,
+       B2_LSQR_HIST = 9 /* history row: r1norm r2norm anorm acond arnorm xnorm test1 test2 istop */ };
+/* One scalar step of lsqr.py's loop, one thread, scipy's operations in scipy's order with round-to-nearest intrinsics
+ * (csrc/lsqr.cu writes the sequence out), so the state equals a float64 NumPy transcription bit for bit.
+ *   phase 0 (after BB, DD are reduced): finish the pending iteration -- ddnorm += DD, acond, test3, istop, history
+ *           row itn-1 into hist_dev[(itn-1) * B2_LSQR_HIST ...] when itn-1 < cap, STOPPED = 1 if istop != 0 -- then
+ *           beta = sqrt(BB) and the v-step coefficients CVA, CVB;
+ *   phase 1 (after AA is reduced): itn += 1, anorm, alfa = sqrt(AA), the rotations, T1 / T2 / INV_RHO / INV_ALFA,
+ *           the xnorm recurrence, r1norm, r2norm, arnorm, test1, test2, CUB; the iteration is then pending;
+ *   phase 2: finish the pending iteration only (after the last iteration of a block; DD reduced).
+ * Every phase is a no-op once STOPPED.  B2_ERR_ARG: null state, phase outside 0..2, null hist with cap > 0. */
+int b2_lsqr_scalars(double* state_dev, int phase, double* hist_dev, size_t cap, void* stream);
+/* LSQR model-side update in ONE pass (lsqr.py:467-476), coef_dev = state + B2_LSQR_T1 (t1, t2, inv_rho, inv_alfa):
+ *   dk = inv_rho w;  x += t1 w;  var += dk^2 (var may be NULL: calc_var=False);  w = inv_alfa v + t2 w;
+ *   *dd_dev = sum |dk|^2 (float64, local partial, deterministic last-CTA fold; shares the ctx reduction workspace).
+ * Complex data are arrays of 2n reals except var += dk^2, NumPy's complex square (re = dr dr - di di, im = dr di +
+ * di dr).  Products and sums are rounded in T one by one (no contraction).  16-byte accesses when x, w, v, var are
+ * 16-byte aligned.  When stop_dev is non-NULL and *stop_dev != 0 nothing is written (the LSQR STOPPED slot).
+ * B2_ERR_ARG: null ctx / coef / dd, or (n > 0) a null or aliased x, w, v, var; B2_ERR_DTYPE: not F32/F64/C64/C128. */
+int b2_lsqr_update(b2_ctx* ctx, void* x, void* w, const void* v, void* var, size_t n, int dtype,
+                   const double* coef_dev, const double* stop_dev, double* dd_dev, void* stream);
+
 /* ---- ISTA / FISTA model update ("next" row; optimization/cls_sparsity.py:270-343, 578-662) in ONE pass:
  *   u = base + alpha*g (g may be NULL);  v = threshold_kind(u, thresh) (_apply_thresh, cls_sparsity.py:21-46);
  *   xnew = v;  znew = v + c*(v - xold) (znew may be NULL; FISTA's auxiliary model, :640-644);

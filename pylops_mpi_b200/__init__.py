@@ -16,8 +16,8 @@ from .waveeqprocessing import MPIMDC  # noqa: F401
 from .StackedArray import StackedDistributedArray  # noqa: F401
 from .StackedLinearOperator import MPIStackedLinearOperator  # noqa: F401
 from .basicoperators import MPIStackedBlockDiag, MPIStackedVStack, MPIGradient  # noqa: F401
-from .optimization.basic import cg, cgls  # noqa: F401
-from .optimization.cls_basic import CG, CGLS  # noqa: F401
+from .optimization.basic import cg, cgls, lsqr  # noqa: F401
+from .optimization.cls_basic import CG, CGLS, LSQR  # noqa: F401
 from .optimization.sparsity import ista, fista  # noqa: F401
 from .optimization.cls_sparsity import ISTA, FISTA  # noqa: F401
 from .optimization.eigs import power_iteration  # noqa: F401

@@ -80,6 +80,8 @@ def _load():
         "b2_dot_multi": ([vp, i, C.POINTER(vp), C.POINTER(vp), sz, i, i, vp, vp], i),
         "b2_scalar_div": ([vp, vp, vp, vp, d, vp], i),
         "b2_history_push": ([vp, i, i, vp, vp, sz, vp, vp, vp], i),
+        "b2_lsqr_scalars": ([vp, i, vp, sz, vp], i),
+        "b2_lsqr_update": ([vp, vp, vp, vp, vp, sz, i, vp, vp, vp, vp], i),
         "b2_sparse_update": ([vp, vp, vp, d, vp, d, i, vp, vp, d, vp, sz, i, vp], i),
         "b2_first_derivative": ([vp, vp, vp, vp, i, vp, i, sz, sz, sz, sz, i, i, i, d, i, i, vp], i),
         "b2_first_derivative_halo": ([i, i, i, C.POINTER(i), C.POINTER(i)], i),

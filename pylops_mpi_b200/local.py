@@ -668,7 +668,7 @@ class Kirchhoff(_KernelOperator):
 class LSM:
     """pylops.waveeqprocessing.LSM (pylops 2.x) for ``kind="kirchhoff"``: builds the demigration operator ``Demop``, a
     :class:`Kirchhoff` with ``kwargs_mod`` passed through -- the only part tutorials/lsm.py uses (each rank's
-    ``lsm.Demop`` goes into MPIVStack).  ``solve`` is not provided: run ``cgls`` on the stacked operator."""
+    ``lsm.Demop`` goes into MPIVStack) -- and ``solve``, which inverts this rank's sources on their own."""
 
     def __init__(self, z, x, t, srcs, recs, vel, wav, wavcenter, y=None, kind="kirchhoff", dottest=False,
                  **kwargs_mod):
@@ -678,6 +678,33 @@ class LSM:
             raise NotImplementedError("LSM: dottest=True is not supported (run utils.dottest on Demop)")
         self.y, self.x, self.z, self.t = y, x, z, t
         self.Demop = Kirchhoff(z, x, t, srcs, recs, vel, wav, wavcenter, y=y, **kwargs_mod)
+
+    def solve(self, d, solver=None, **kwargs_solver):
+        """pylops' ``LSM.solve``: invert the data ``d`` (``ns * nr * nt`` values, NumPy or torch) of this rank's
+        sources, rank-local as in pylops.  ``Demop`` runs inside ``MPIVStack`` on a one-rank communicator with a
+        BROADCAST model from ``x0 = 0``, through this package's ``lsqr`` (``solver=None``) or ``cgls``, with
+        ``kwargs_solver`` passed on.  Returns the image, a device tensor of shape ``Demop.dims``."""
+        from . import comm as _comm
+        from .basicoperators.VStack import MPIVStack
+        from .DistributedArray import DistributedArray, Partition
+        from .optimization.basic import cgls, lsqr
+        if solver is None:
+            solver = lsqr
+        if solver is not lsqr and solver is not cgls:
+            raise NotImplementedError(f"LSM.solve: solver={solver!r} is not supported (lsqr or cgls of this package)")
+        one = _comm.Comm(rank=0, size=1)
+        Op = MPIVStack([self.Demop], base_comm=one)
+        dt = _lib.torch_dtype(self.Demop.dtype)
+        dev = torch.device("cuda", torch.cuda.current_device())
+        dloc = torch.as_tensor(d).to(device=dev, dtype=dt).reshape(-1)
+        if dloc.numel() != Op.shape[0]:
+            raise ValueError(f"LSM.solve: d has {dloc.numel()} values, Demop has {Op.shape[0]} rows")
+        dd = DistributedArray(global_shape=Op.shape[0], base_comm=one, dtype=dt)
+        dd.local_array[:] = dloc
+        x0 = DistributedArray(global_shape=Op.shape[1], base_comm=one, partition=Partition.BROADCAST, dtype=dt)
+        x0.local_array.zero_()
+        x = solver(Op, dd, x0=x0, **kwargs_solver)[0]
+        return x.local_array.reshape(self.Demop.dims)
 
 
 class FFT(LocalOperator):

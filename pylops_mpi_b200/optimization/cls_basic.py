@@ -10,6 +10,7 @@ Two execution modes, same numbers:
     iteration (``CGLS._body``): ``step()`` runs it eagerly and reads its
     scalars with one host synchronisation, ``run()`` replays it as a CUDA
     graph and reads them once per block, so every mode gives the same bits.
+    LSQR (an extension: the reference has none) is built the same way.
 """
 from __future__ import annotations
 
@@ -24,6 +25,10 @@ from .. import _lib
 from ..Distributed import allreduce_
 from ..DistributedArray import DistributedArray
 from ..local import _KernelOperator
+from ..utils.partition import local_split_sizes, offsets
+from .lsqr_host import (_AA, _ALFA, _ATOL, _BB, _BETA, _BNORM, _BTOL, _CS2, _CTOL, _CUB, _CVA, _CVB, _DAMP,
+                        _DAMPSQ, _DD, _INV_ALFA, _INV_RHO, _ITER_LIM, _ITN, _NHIST, _NSTATE, _PHIBAR, _RHOBAR,
+                        _SCRATCH, _STOPPED, _T1, _T2, lsqr_scalars_host)
 
 
 class Solver:
@@ -280,7 +285,69 @@ class CG(Solver):
         return x, self.iiter, self.cost
 
 
-class CGLS(Solver):
+class _DeviceLoopSolver(Solver):
+    """a solver with ONE fused device iteration ``_body(*args)`` (no host synchronisation inside): ``_iterate`` runs
+    the first iteration of a block run eagerly, then captures the body once as a CUDA graph and replays it"""
+
+    def _iterate(self, *args):
+        """one iteration of a block run: the first runs eagerly (every kernel of the body gets loaded, lazy
+        workspaces and communicators exist), then the body is captured once as a CUDA graph and replayed"""
+        if self._graph is None and self._capture and self._warm:
+            t_cap = time.perf_counter()
+            try:
+                # manual capture on a side stream (torch.cuda.graph() would add a device synchronise, a
+                # gc.collect() and an empty_cache() -- milliseconds, comparable to a whole 50-iteration solve)
+                pool = _graph_pool()
+                t_pool = time.perf_counter()
+                g = torch.cuda.CUDAGraph()
+                main = torch.cuda.current_stream()
+                side = torch.cuda.Stream()
+                side.wait_stream(main)
+                with torch.cuda.stream(side):
+                    # one process-wide memory pool for all captures: the temporaries of the first capture are
+                    # cudaMalloc'ed (slow when peers have this device mapped: measured 3.1 ms at 2 GPUs vs 0.65 ms
+                    # at 1), later captures reuse the cached blocks
+                    # thread_local error mode: NCCL's helper threads keep polling CUDA while we capture
+                    # (observed at 8 ranks: a "global"-mode capture was invalidated and left torch's RNG state
+                    # stuck in capture mode)
+                    g.capture_begin(pool=pool, capture_error_mode="thread_local")   # records only
+                    t_begin = time.perf_counter()
+                    try:
+                        self._body(*args)
+                    finally:
+                        t_body = time.perf_counter()
+                        g.capture_end()
+                main.wait_stream(side)
+                self._graph = g
+                t_end = time.perf_counter()
+                self.graph_capture_ms = (t_end - t_cap) * 1e3
+                self.graph_capture_breakdown_ms = {"pool": (t_pool - t_cap) * 1e3, "begin": (t_begin - t_pool) * 1e3,
+                                                   "body": (t_body - t_begin) * 1e3, "end": (t_end - t_body) * 1e3}
+            except Exception as exc:               # not capturable (host sync inside an operator ...): stay eager
+                self._capture = False
+                self.graph_error = repr(exc)[:300]
+                print(f"[b200 {type(self).__name__.lower()}] CUDA-graph capture failed, running eagerly: "
+                      f"{self.graph_error}", file=sys.stderr)
+                torch.cuda.synchronize()
+                _reset_capture_state()
+        if self._graph is not None:
+            self._graph.replay()
+            self.graph_replays += 1
+        else:
+            self._body(*args)
+            self._warm = True
+
+    def _start_blocks(self):
+        self._graph, self._warm, self._capture = None, False, _graph_safe(self.Op)
+        self.graph_replays, self.graph_error = 0, (None if self._capture else "operator not on the graph-safe list")
+
+    def _plain_callback(self) -> bool:
+        """no callback to call per iteration: neither overridden in a subclass nor set on the instance
+        (cgls(callback=...)) nor given as ``callbacks``"""
+        return type(self).callback is Solver.callback and "callback" not in vars(self) and not self.callbacks
+
+
+class CGLS(_DeviceLoopSolver):
     """cls_basic.py:252-531"""
 
     def _print_step(self, x) -> None:
@@ -417,53 +484,6 @@ class CGLS(Solver):
                                             hist.shape[0], dev.data_ptr() + 8 * KOLD, dev.data_ptr() + 8 * K,
                                             _lib.stream()), "b2_history_push")
 
-    def _iterate(self, x, hist: torch.Tensor, it_dev: torch.Tensor):
-        """one iteration of a block run: the first runs eagerly (every kernel of the body gets loaded, lazy
-        workspaces and communicators exist), then the body is captured once as a CUDA graph and replayed"""
-        if self._graph is None and self._capture and self._warm:
-            t_cap = time.perf_counter()
-            try:
-                # manual capture on a side stream (torch.cuda.graph() would add a device synchronise, a
-                # gc.collect() and an empty_cache() -- milliseconds, comparable to a whole 50-iteration solve)
-                pool = _graph_pool()
-                t_pool = time.perf_counter()
-                g = torch.cuda.CUDAGraph()
-                main = torch.cuda.current_stream()
-                side = torch.cuda.Stream()
-                side.wait_stream(main)
-                with torch.cuda.stream(side):
-                    # one process-wide memory pool for all captures: the temporaries of the first capture are
-                    # cudaMalloc'ed (slow when peers have this device mapped: measured 3.1 ms at 2 GPUs vs 0.65 ms
-                    # at 1), later captures reuse the cached blocks
-                    # thread_local error mode: NCCL's helper threads keep polling CUDA while we capture
-                    # (observed at 8 ranks: a "global"-mode capture was invalidated and left torch's RNG state
-                    # stuck in capture mode)
-                    g.capture_begin(pool=pool, capture_error_mode="thread_local")   # records only
-                    t_begin = time.perf_counter()
-                    try:
-                        self._body(x, hist, it_dev)
-                    finally:
-                        t_body = time.perf_counter()
-                        g.capture_end()
-                main.wait_stream(side)
-                self._graph = g
-                t_end = time.perf_counter()
-                self.graph_capture_ms = (t_end - t_cap) * 1e3
-                self.graph_capture_breakdown_ms = {"pool": (t_pool - t_cap) * 1e3, "begin": (t_begin - t_pool) * 1e3,
-                                                   "body": (t_body - t_begin) * 1e3, "end": (t_end - t_body) * 1e3}
-            except Exception as exc:               # not capturable (host sync inside an operator ...): stay eager
-                self._capture = False
-                self.graph_error = repr(exc)[:300]
-                print(f"[b200 cgls] CUDA-graph capture failed, running eagerly: {self.graph_error}", file=sys.stderr)
-                torch.cuda.synchronize()
-                _reset_capture_state()
-        if self._graph is not None:
-            self._graph.replay()
-            self.graph_replays += 1
-        else:
-            self._body(x, hist, it_dev)
-            self._warm = True
-
     def _run_blocks(self, x, niter: int):
         """remaining iterations in blocks of :meth:`_iterate`; the host reads the scalar history once per block.
         With tol > 0 a block is at most 8 iterations and is re-run from a checkpoint up to the stopping iteration,
@@ -473,8 +493,7 @@ class CGLS(Solver):
         it0 = self.iiter
         hist = torch.zeros((niter - it0 + 2, 3), dtype=torch.float64, device=device)
         it_dev = torch.zeros(1, dtype=torch.int64, device=device)
-        self._graph, self._warm, self._capture = None, False, _graph_safe(self.Op)
-        self.graph_replays, self.graph_error = 0, (None if self._capture else "operator not on the graph-safe list")
+        self._start_blocks()
         block = niter - it0 if self.tol <= 0.0 else 8
         while self.iiter < niter and self.kold > self.tol:
             n = min(block, niter - self.iiter)
@@ -505,8 +524,7 @@ class CGLS(Solver):
         if niter is None:
             raise ValueError("niter must not be None")
         # a callback, overridden in a subclass or set on the instance (cgls(callback=...)), sees every iteration
-        plain_callback = type(self).callback is Solver.callback and "callback" not in vars(self) and not self.callbacks
-        if not self._gen and not show and plain_callback and niter - self.iiter > 0:
+        if not self._gen and not show and self._plain_callback() and niter - self.iiter > 0:
             return self._run_blocks(x, niter)
         while self.iiter < niter and self.kold > self.tol:
             showstep = bool(show and (self.iiter < itershow[0] or niter - self.iiter < itershow[1]
@@ -531,3 +549,243 @@ class CGLS(Solver):
         x = self.run(x, niter, show=show, itershow=itershow)
         self.finalize(show)
         return x, self.istop, self.iiter, self.r1norm, self.r2norm, self.cost
+
+
+# ---- LSQR -----------------------------------------------------------------------------------------------------------
+def _zeros_like(a):
+    if isinstance(a, DistributedArray):
+        return a.zeros_like()
+    from ..StackedArray import StackedDistributedArray
+    return StackedDistributedArray([_zeros_like(d) for d in a.distarrays], a.base_comm)
+
+
+class LSQR(_DeviceLoopSolver):
+    """LSQR (Paige & Saunders 1982) with pylops 2.x's ``LSQR`` interface: ``setup / step / run / finalize / solve``.
+    An extension: pylops-mpi has no LSQR.  The iterates, stopping tests, ``istop`` (0-7) and the estimates are those
+    of ``scipy.sparse.linalg.lsqr`` with ``iter_lim = niter`` and the same ``damp, atol, btol, conlim, calc_var, x0``.
+
+    ONE fused iteration (``_body``) runs every mode: u and v stay unnormalised with their scales folded into the
+    device coefficients of the next combination, the scalar recurrence runs on the device (``b2_lsqr_scalars``) and
+    the model-side update is one pass (``b2_lsqr_update``).  ``run()`` replays the body as a CUDA graph in blocks
+    and reads the scalar history once per block; a stop inside a block sets a device flag that turns the rest of
+    the block into no-ops for x, w, var and the scalars.  ``step()`` runs the same body eagerly."""
+
+    _BLOCK = 8
+
+    def _print_step(self, x) -> None:
+        x0 = (x if isinstance(x, DistributedArray) else x[0]).local_array.reshape(-1)[0].item()
+        strx = f"{x0:1.2e}   " if isinstance(x0, complex) else f"{x0:11.4e}        "
+        print(f"{self.iiter:6g}       " + strx + f"{self.r1norm:10.3e} {self.r2norm:10.3e}  {self.test1:8.1e} "
+              f"{self.test2:8.1e} {self.anorm:8.1e} {self.acond:8.1e}")
+        sys.stdout.flush()
+
+    def setup(self, y, x0=None, damp: float = 0.0, atol: float = 1e-8, btol: float = 1e-8, conlim: float = 1e8,
+              niter: int = 10, calc_var: bool = True, show: bool = False):
+        self.y, self.damp, self.atol, self.btol, self.conlim = y, damp, atol, btol, conlim
+        self.niter, self.calc_var = niter, calc_var
+        self.ctol = 1 / conlim if conlim > 0 else 0.0
+        ahu = None
+        if x0 is None:
+            self.U = y.copy()                               # scipy: u = b
+            ahu = self.Op.rmatvec(self.U)                   # A^H u: v's direction and the model's layout
+            x = _zeros_like(ahu)
+        else:
+            x = x0.copy()
+            self.U = y - self.Op.matvec(x)
+        self.rank = x.rank
+        self._gen = _generic(x, self.U)
+        if self._gen:
+            bnorm, beta = float(y.norm().item()), float(self.U.norm().item())
+        else:
+            yy, uu = _self_dots([y, self.U]) if y.local_shape == self.U.local_shape else \
+                (_self_dots([y])[0], _self_dots([self.U])[0])
+            bnorm, beta = float(np.sqrt(yy)), float(np.sqrt(uu))
+        if beta > 0:
+            self.V = (1 / beta) * (self.Op.rmatvec(self.U) if ahu is None else ahu)
+            alfa = float(self.V.norm().item()) if self._gen else float(np.sqrt(_self_dots([self.V])[0]))
+        else:
+            self.V, alfa = x.copy(), 0.0
+        inv_alfa = 1 / alfa if alfa > 0 else 1.0
+        self.W = inv_alfa * self.V                          # w = v
+        self.var = _zeros_like(x)
+        s = np.zeros(_NSTATE)
+        s[[_ALFA, _BETA, _RHOBAR, _PHIBAR, _CS2, _INV_ALFA]] = alfa, beta, alfa, beta, -1.0, inv_alfa
+        s[[_DAMP, _DAMPSQ, _ATOL, _BTOL, _CTOL, _BNORM, _ITER_LIM]] = damp, damp * damp, atol, btol, self.ctol, \
+            bnorm, niter
+        s[_CUB] = alfa * (1 / beta if beta > 0 else 1.0)
+        self.iiter, self.istop = 0, 0
+        self.r1norm = self.r2norm = beta
+        self.anorm = self.acond = self.xnorm = 0.0
+        self.arnorm = alfa * beta
+        self.test1, self.test2 = 1.0, (alfa / beta if beta > 0 else 0.0)
+        self._done = self.arnorm == 0                       # x0 solves the problem (scipy returns at once)
+        s[_STOPPED] = float(self._done)
+        self.cost: List = [self.r1norm]
+        if self._gen:
+            self._hs = s
+        else:
+            self._st = 2 if any(a._tdtype.is_complex for a in (x, self.U, self.V)) else 1
+            self._dev = torch.from_numpy(s).to(x.local_array.device)
+            self._hist = torch.zeros((max(niter, 1), _NHIST), dtype=torch.float64, device=self._dev.device)
+            self._xs = x
+        if show and self.rank == 0:
+            self._print_solver(nbar=90)
+            print(f"damp = {damp:20.14e}   calc_var = {calc_var:6g}")
+            print(f"atol = {atol:8.2e}                 conlim = {conlim:8.2e}")
+            print(f"btol = {btol:8.2e}                 niter = {niter:8g}")
+            print("-" * 90 + "\n")
+            print("    Itn          x[0]              r1norm     r2norm   Compatible   LS    Norm A   Cond A")
+        return x
+
+    # ---- fused path -------------------------------------------------------------------------------------------
+    def _scalars(self, phase: int):
+        _lib.check(_lib.lib.b2_lsqr_scalars(self._dev.data_ptr(), phase, self._hist.data_ptr(), self._hist.shape[0],
+                                            _lib.stream()), "b2_lsqr_scalars")
+
+    def _update(self, x):
+        """x += t1 w, var += dk^2, w = inv_alfa v + t2 w and DD = |dk|^2 in one pass.  A BROADCAST model is updated
+        whole on every rank, but DD is summed over this rank's share only (the re-scattered view of the
+        reductions), so the all-reduce counts each element once."""
+        from ..DistributedArray import Partition
+        dev = self._dev
+        ts = [a.local_array for a in (x, self.W, self.V)] + ([self.var.local_array] if self.calc_var else [])
+        if any(not t.is_contiguous() for t in ts) or len({t.dtype for t in ts}) != 1:
+            raise TypeError("lsqr: x, w, v and var must be contiguous and of one dtype")
+        n = ts[0].numel()
+        cuts = [0, n]
+        if x.partition is not Partition.SCATTER and x.size > 1 and n:
+            rows = ts[0].shape[0]
+            ext = offsets(local_split_sizes(rows, x.size))
+            cuts = [0, ext[x.rank] * (n // rows), ext[x.rank + 1] * (n // rows), n]
+        own = 1 if len(cuts) == 4 else 0
+        for k in range(len(cuts) - 1):
+            a, b = cuts[k], cuts[k + 1]
+            if b == a and k != own:
+                continue
+            p = [t.reshape(-1)[a:b] for t in ts]
+            ptr = [t.data_ptr() if b > a else None for t in p]
+            _lib.check(_lib.lib.b2_lsqr_update(_lib.ctx(), ptr[0], ptr[1], ptr[2], ptr[3] if self.calc_var else None,
+                                               b - a, _lib.code(ts[0].dtype), dev.data_ptr() + 8 * _T1,
+                                               dev.data_ptr() + 8 * _STOPPED,
+                                               dev.data_ptr() + 8 * (_DD if k == own else _SCRATCH), _lib.stream()),
+                       "b2_lsqr_update")
+
+    def _body(self, x):
+        """one LSQR iteration, no host synchronisation; its history row is written when the next body (or
+        :meth:`_tail`) finishes it"""
+        dev, st, sub = self._dev, self._st, x.sub_comm
+        av = self.Op.matvec(self.V)
+        if not _lincomb_dev_norm2(self.U, dev, _INV_ALFA, 1.0, av, dev, _CUB, -1.0, self.U, dev, _BB):
+            _dots_device([self.U], dev, _BB)
+        allreduce_(sub, dev[0:_DD + 1], "sum")             # BB and the previous iteration's DD
+        self._scalars(0)
+        ahu = self.Op.rmatvec(self.U)
+        if not _lincomb_dev_norm2(self.V, dev, _CVA, 1.0, ahu, dev, _CVB, -1.0, self.V, dev, _AA):
+            _dots_device([self.V], dev, _AA)
+        allreduce_(sub, dev[_AA:_AA + st], "sum")
+        self._scalars(1)
+        self._update(x)
+
+    def _tail(self, x, first: int):
+        """finish the pending iteration and absorb the history rows from iteration ``first`` on (one host read)"""
+        allreduce_(x.sub_comm, self._dev[_DD:_DD + 1], "sum")
+        self._scalars(2)
+        last = min(first + self._BLOCK, self._hist.shape[0])
+        h = torch.cat((self._dev[_ITN:_ITN + 1], self._hist[first:last].reshape(-1))).cpu().numpy()
+        itn = int(h[0])
+        for row in h[1:].reshape(-1, _NHIST)[:itn - first]:
+            self._absorb(row)
+
+    def _absorb(self, row) -> None:
+        (self.r1norm, self.r2norm, self.anorm, self.acond, self.arnorm, self.xnorm, self.test1, self.test2) = \
+            (float(v) for v in row[:8])
+        self.istop = int(row[8])
+        self.iiter += 1
+        self.cost.append(self.r1norm)
+
+    def _ensure_rows(self, niter: int):
+        if niter > self._hist.shape[0]:
+            hist = torch.zeros((niter, _NHIST), dtype=torch.float64, device=self._hist.device)
+            hist[:self._hist.shape[0]] = self._hist
+            self._hist = hist
+
+    # ---- generic path (stacked arrays): the same recurrence in DistributedArray operations -----------------------
+    def _step_generic(self, x):
+        s = self._hs
+        if s[_STOPPED]:
+            return x
+        c = lambda i: float(s[i])                                   # noqa: E731  (NumPy scalars would broadcast)
+        self.U = c(_INV_ALFA) * self.Op.matvec(self.V) - c(_CUB) * self.U
+        s[_BB] = _absdot(self.U, self.U)
+        lsqr_scalars_host(s, 0)
+        self.V = c(_CVA) * self.Op.rmatvec(self.U) - c(_CVB) * self.V
+        s[_AA] = _absdot(self.V, self.V)
+        lsqr_scalars_host(s, 1)
+        dk = c(_INV_RHO) * self.W
+        x += c(_T1) * self.W
+        if self.calc_var:
+            self.var += dk * dk
+        self.W = c(_INV_ALFA) * self.V + c(_T2) * self.W
+        s[_DD] = _absdot(dk, dk)
+        self._absorb(lsqr_scalars_host(s, 2))
+        return x
+
+    # ---- pylops interface --------------------------------------------------------------------------------------
+    def step(self, x, show: bool = False):
+        """one LSQR iteration: the fused body run eagerly, then its tests (one host synchronisation)"""
+        if self._done or self.istop != 0:
+            return x
+        if self._gen:
+            x = self._step_generic(x)
+        else:
+            self._ensure_rows(self.iiter + 1)
+            self._body(x)
+            self._tail(x, self.iiter)
+        if show and self.rank == 0:
+            self._print_step(x)
+        return x
+
+    def _run_blocks(self, x, niter: int):
+        """the remaining iterations in blocks of :meth:`_iterate` (graph replays), one history read per block"""
+        self._ensure_rows(niter)
+        self._start_blocks()
+        while self.iiter < niter and self.istop == 0:
+            first = self.iiter
+            for _ in range(min(self._BLOCK, niter - first)):
+                self._iterate(x)
+            self._tail(x, first)
+        self._graph = None
+        return x
+
+    def run(self, x, niter: Optional[int] = None, show: bool = False, itershow=(10, 10, 10)):
+        niter = self.niter if niter is None else niter
+        if self._done:
+            return x
+        if not self._gen and not show and self._plain_callback() and niter - self.iiter > 0:
+            return self._run_blocks(x, niter)
+        while self.iiter < niter and self.istop == 0:
+            showstep = bool(show and (self.iiter < itershow[0] or niter - self.iiter < itershow[1]
+                                      or self.iiter % itershow[2] == 0))
+            x = self.step(x, showstep)
+            self.callback(x)
+        return x
+
+    def finalize(self, show: bool = False) -> None:
+        self.tend = time.time()
+        self.telapsed = self.tend - self.tstart
+        self.cost = np.array(self.cost)
+        if show and self.rank == 0:
+            print(f"\nistop = {self.istop}   r1norm = {self.r1norm:8.1e}   anorm = {self.anorm:8.1e}   "
+                  f"arnorm = {self.arnorm:8.1e}")
+            print(f"itn   = {self.iiter}   r2norm = {self.r2norm:8.1e}   acond = {self.acond:8.1e}   "
+                  f"xnorm  = {self.xnorm:8.1e}")
+            self._print_finalize(nbar=90)
+
+    def solve(self, y, x0=None, damp: float = 0.0, atol: float = 1e-8, btol: float = 1e-8, conlim: float = 1e8,
+              niter: int = 10, calc_var: bool = True, show: bool = False, itershow=(10, 10, 10)):
+        x = self.setup(y=y, x0=x0, damp=damp, atol=atol, btol=btol, conlim=conlim, niter=niter, calc_var=calc_var,
+                       show=show)
+        x = self.run(x, niter, show=show, itershow=itershow)
+        self.finalize(show)
+        return (x, self.istop, self.iiter, self.r1norm, self.r2norm, self.anorm, self.acond, self.arnorm, self.xnorm,
+                self.var, self.cost)
