@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
+#include <math.h>
 #include <stdint.h>
 #include <stddef.h>
 #include "../../include/b200lops.h"
@@ -125,4 +126,94 @@ __device__ __forceinline__ double warp_min(double v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v = fmin(v, __shfl_xor_sync(0xffffffffu, v, o));
   return v;
+}
+
+// ---- deterministic grid reduction -----------------------------------------------------------------------------------
+// The fused reduction kernels (reduce.cu, sparsity.cu, lsqr.cu) run CTAs of B2_RED_THREADS threads on a grid sized by
+// b2_red_grid and end in b2_grid_fold.  Their float64 results depend on the grid size and on nothing else, so a call
+// repeats its bits; a different grid (or fold order) gives different bits.
+constexpr int B2_RED_THREADS = 256;
+enum { RED_SUM = 0, RED_MAX = 1, RED_MIN = 2 };
+
+// max / min that return NaN when either operand is NaN, as np.max and np.linalg.norm(x, inf) do (fmax / fmin drop it)
+__device__ __forceinline__ double nan_max(double a, double b) { return (a > b || a != a) ? a : b; }
+__device__ __forceinline__ double nan_min(double a, double b) { return (a < b || a != a) ? a : b; }
+
+template <int OP>
+__device__ __forceinline__ double comb(double a, double b) {
+  if (OP == RED_SUM) return a + b;
+  if (OP == RED_MAX) return nan_max(a, b);
+  return nan_min(a, b);
+}
+template <int OP>
+__device__ __forceinline__ double ident() {
+  if (OP == RED_SUM) return 0.0;
+  if (OP == RED_MAX) return 0.0;  // all candidates are |x| >= 0
+  return INFINITY;
+}
+template <int OP>
+__device__ __forceinline__ double warp_comb(double v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = comb<OP>(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
+
+// ceil(items / items_per_cta) CTAs, at least 1 and at most min(8 * SMs, B2_RED_MAX_BLOCKS)
+static inline int b2_red_grid(const b2_ctx* ctx, size_t items, size_t items_per_cta) {
+  size_t cap = (size_t)ctx->sm_count * 8;
+  if (cap > (size_t)B2_RED_MAX_BLOCKS) cap = B2_RED_MAX_BLOCKS;
+  const size_t need = (items + items_per_cta - 1) / items_per_cta;
+  return (int)(need < 1 ? 1 : (need < cap ? need : cap));
+}
+
+struct b2_fold_nothing {
+  __device__ void operator()() const {}
+};
+
+// Folds acc[0..K) of every thread of the grid into out[0..K) (out may be null); every thread of every CTA calls it,
+// as the last statement of the kernel.  A CTA reduces each accumulator with an xor-shuffle tree per warp, then the
+// per-warp values in warp 0, and writes its partial to partials[blockIdx.x * K + k].  The last CTA to take the
+// ticket folds the partials in CTA order (lane l takes CTAs l, l + 32, ..., then a shuffle tree); the thread that
+// writes out then runs last() (a caller's own extra store, made after every CTA has passed its loop) and resets the
+// ticket for the next launch.
+template <int K, int OP, typename Last = b2_fold_nothing>
+__device__ __forceinline__ void b2_grid_fold(const double* acc, double* __restrict__ partials,
+                                             unsigned int* __restrict__ ticket, double* __restrict__ out,
+                                             Last last = Last()) {
+  static_assert(K <= B2_RED_MAX_OUT, "partials hold B2_RED_MAX_OUT doubles per CTA");
+  __shared__ double smem[K][B2_RED_THREADS / 32];
+  __shared__ bool is_last;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int k = 0; k < K; ++k) {
+    const double v = warp_comb<OP>(acc[k]);
+    if (lane == 0) smem[k][warp] = v;
+  }
+  __syncthreads();
+  if (warp == 0) {
+#pragma unroll
+    for (int k = 0; k < K; ++k) {
+      const double v = warp_comb<OP>(lane < B2_RED_THREADS / 32 ? smem[k][lane] : ident<OP>());
+      if (lane == 0) partials[(size_t)blockIdx.x * K + k] = v;
+    }
+  }
+  if (threadIdx.x == 0) {
+    __threadfence();
+    is_last = (atomicAdd(ticket, 1u) == gridDim.x - 1);
+  }
+  __syncthreads();
+  if (!is_last) return;
+  __threadfence();
+  if (warp != 0) return;
+#pragma unroll
+  for (int k = 0; k < K; ++k) {
+    double v = ident<OP>();
+    for (unsigned int b = lane; b < gridDim.x; b += 32) v = comb<OP>(v, __ldcg(&partials[(size_t)b * K + k]));
+    v = warp_comb<OP>(v);
+    if (lane == 0 && out) out[k] = v;
+  }
+  if (lane == 0) {
+    last();
+    *ticket = 0u;
+  }
 }

@@ -43,7 +43,7 @@
 namespace {
 
 constexpr double EPS = 2.220446049250313e-16;   // np.finfo(np.float64).eps
-constexpr int UPD_THREADS = 256;
+constexpr int UPD_THREADS = B2_RED_THREADS;
 
 __device__ __forceinline__ double add(double a, double b) { return __dadd_rn(a, b); }
 __device__ __forceinline__ double sub(double a, double b) { return __dsub_rn(a, b); }
@@ -273,40 +273,7 @@ lsqr_update_kernel(T* __restrict__ x, T* __restrict__ w, const T* __restrict__ v
       if (VAR) var_real(var[i], dk);
     }
   }
-  // deterministic block reduce + last-CTA fold in CTA order (as reduce.cu)
-  __shared__ double smem[UPD_THREADS / 32];
-  __shared__ bool is_last;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  double s = warp_sum(acc);
-  if (lane == 0) smem[warp] = s;
-  __syncthreads();
-  if (warp == 0) {
-    s = lane < UPD_THREADS / 32 ? smem[lane] : 0.0;
-    s = warp_sum(s);
-    if (lane == 0) partials[blockIdx.x] = s;
-  }
-  if (threadIdx.x == 0) {
-    __threadfence();
-    const unsigned int t = atomicAdd(ticket, 1u);
-    is_last = (t == gridDim.x - 1);
-  }
-  __syncthreads();
-  if (is_last) {
-    __threadfence();
-    if (warp == 0) {
-      double r = 0.0;
-      for (unsigned int b = lane; b < gridDim.x; b += 32) r += __ldcg(&partials[b]);
-      r = warp_sum(r);
-      if (lane == 0) {
-        *dd = r;
-        *ticket = 0u;
-      }
-    }
-  }
-}
-
-__global__ void lsqr_dd_zero_kernel(double* dd, const double* stop) {
-  if (threadIdx.x == 0 && !(stop && *stop != 0.0)) *dd = 0.0;
+  b2_grid_fold<1, RED_SUM>(&acc, partials, ticket, dd);
 }
 
 template <typename T, bool CX, bool VAR>
@@ -316,16 +283,12 @@ int launch_update(b2_ctx* ctx, void* x, void* w, const void* v, void* var, size_
   const bool vec = b2_aligned16(x) && b2_aligned16(w) && b2_aligned16(v) && (!VAR || b2_aligned16(var)) &&
                    n_real >= (size_t)V;
   const size_t items = vec ? n_real / V : (CX ? n_real / 2 : n_real);
-  size_t grid = (items + UPD_THREADS - 1) / UPD_THREADS;
-  size_t cap = (size_t)ctx->sm_count * 8;
-  if (cap > (size_t)B2_RED_MAX_BLOCKS) cap = B2_RED_MAX_BLOCKS;
-  if (grid > cap) grid = cap;
-  if (grid < 1) grid = 1;
+  const int grid = b2_red_grid(ctx, items, UPD_THREADS);   // one item per thread: no unrolled loop
   if (vec)
-    lsqr_update_kernel<T, CX, VAR, true><<<(unsigned)grid, UPD_THREADS, 0, st>>>(
+    lsqr_update_kernel<T, CX, VAR, true><<<grid, UPD_THREADS, 0, st>>>(
         (T*)x, (T*)w, (const T*)v, (T*)var, n_real, coef, stop, ctx->red_partials, ctx->tickets, dd);
   else
-    lsqr_update_kernel<T, CX, VAR, false><<<(unsigned)grid, UPD_THREADS, 0, st>>>(
+    lsqr_update_kernel<T, CX, VAR, false><<<grid, UPD_THREADS, 0, st>>>(
         (T*)x, (T*)w, (const T*)v, (T*)var, n_real, coef, stop, ctx->red_partials, ctx->tickets, dd);
   B2_LAUNCH_CHECK();
   return B2_OK;
@@ -353,12 +316,10 @@ extern "C" int b2_lsqr_update(b2_ctx* ctx, void* x, void* w, const void* v, void
   const bool cx = (dtype == B2_C64 || dtype == B2_C128);
   if (!cx && dtype != B2_F32 && dtype != B2_F64) return B2_ERR_DTYPE;
   cudaStream_t st = (cudaStream_t)stream;
-  if (n == 0) {  // a rank may own no model elements: its ||dk||^2 is still all-reduced
-    lsqr_dd_zero_kernel<<<1, 32, 0, st>>>(dd_dev, stop_dev);
-    B2_LAUNCH_CHECK();
-    return B2_OK;
-  }
-  if (!x || !w || !v || x == w || x == v || w == v || (var && (var == x || var == w || var == v))) return B2_ERR_ARG;
+  // a rank may own no model elements (n == 0, null arrays allowed): one CTA writes its ||dk||^2 = 0 unless stopped,
+  // and it is still all-reduced
+  if (n && (!x || !w || !v || x == w || x == v || w == v || (var && (var == x || var == w || var == v))))
+    return B2_ERR_ARG;
   const size_t n_real = cx ? 2 * n : n;
   switch (dtype) {
     case B2_F32: return launch_update_var<float, false>(ctx, x, w, v, var, n_real, coef_dev, stop_dev, dd_dev, st);

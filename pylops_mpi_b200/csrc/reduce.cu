@@ -2,47 +2,22 @@
 // (reference: pylops_mpi/DistributedArray.py:654-686, 688-758).
 //
 // One launch per reduction: every CTA streams its grid-stride share with
-// 16-byte loads, accumulates in float64 registers, reduces with warp shuffles,
-// writes one partial per CTA; the last CTA to finish (ticket counter) folds the
-// partials in CTA order, so the result is deterministic for a given n.
+// 16-byte loads, accumulates in float64 registers, and b2_grid_fold (common.cuh)
+// folds the per-CTA partials in CTA order, so the result is deterministic for a given n.
 // HBM-bound: algorithmic bytes = n*sizeof(T) per operand.
 #include <math.h>
 #include "common.cuh"
 
 namespace {
 
-constexpr int RED_THREADS = 256;
+constexpr int RED_THREADS = B2_RED_THREADS;
 constexpr int RED_UNROLL = 4;
-enum { MODE_SUM = 0, MODE_MAX = 1, MODE_MIN = 2 };
-
-// max / min that return NaN when either operand is NaN, as np.max and np.linalg.norm(x, inf) do (fmax / fmin drop it)
-__device__ __forceinline__ double nan_max(double a, double b) { return (a > b || a != a) ? a : b; }
-__device__ __forceinline__ double nan_min(double a, double b) { return (a < b || a != a) ? a : b; }
-
-template <int MODE>
-__device__ __forceinline__ double comb(double a, double b) {
-  if (MODE == MODE_SUM) return a + b;
-  if (MODE == MODE_MAX) return nan_max(a, b);
-  return nan_min(a, b);
-}
-template <int MODE>
-__device__ __forceinline__ double ident() {
-  if (MODE == MODE_SUM) return 0.0;
-  if (MODE == MODE_MAX) return 0.0;  // all candidates are |x| >= 0
-  return INFINITY;
-}
-template <int MODE>
-__device__ __forceinline__ double warp_comb(double v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = comb<MODE>(v, __shfl_xor_sync(0xffffffffu, v, o));
-  return v;
-}
 
 // ---- functors --------------------------------------------------------------
 // real(acc, x, y) consumes one real element; cx(acc, xr, xi, yr, yi) one complex.
 template <bool CONJ>
 struct DotF {
-  static constexpr int NOUT_REAL = 1, NOUT_CX = 2, MODE = MODE_SUM;
+  static constexpr int NOUT_REAL = 1, NOUT_CX = 2, MODE = RED_SUM;
   static constexpr bool HAS_Y = true;
   double p;
   template <typename T>
@@ -57,7 +32,7 @@ struct DotF {
   }
 };
 struct SumSqF {
-  static constexpr int NOUT_REAL = 1, NOUT_CX = 1, MODE = MODE_SUM;
+  static constexpr int NOUT_REAL = 1, NOUT_CX = 1, MODE = RED_SUM;
   static constexpr bool HAS_Y = false;
   double p;
   template <typename T>
@@ -70,7 +45,7 @@ struct SumSqF {
   }
 };
 struct SumAbsF {
-  static constexpr int NOUT_REAL = 1, NOUT_CX = 1, MODE = MODE_SUM;
+  static constexpr int NOUT_REAL = 1, NOUT_CX = 1, MODE = RED_SUM;
   static constexpr bool HAS_Y = false;
   double p;
   template <typename T>
@@ -81,7 +56,7 @@ struct SumAbsF {
   }
 };
 struct CountNzF {
-  static constexpr int NOUT_REAL = 1, NOUT_CX = 1, MODE = MODE_SUM;
+  static constexpr int NOUT_REAL = 1, NOUT_CX = 1, MODE = RED_SUM;
   static constexpr bool HAS_Y = false;
   double p;
   template <typename T>
@@ -104,7 +79,7 @@ struct ExtAbsF {
   }
 };
 struct SumPowF {
-  static constexpr int NOUT_REAL = 1, NOUT_CX = 1, MODE = MODE_SUM;
+  static constexpr int NOUT_REAL = 1, NOUT_CX = 1, MODE = RED_SUM;
   static constexpr bool HAS_Y = false;
   double p;
   template <typename T>
@@ -183,56 +158,11 @@ reduce_kernel(F f, const T* __restrict__ x, const T* __restrict__ y, size_t n_re
              F::HAS_Y ? y[2 * i + 1] : x[2 * i + 1]);
     }
   }
-
-  // block reduce
-  __shared__ double smem[NOUT][RED_THREADS / 32];
-  __shared__ bool is_last;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-  for (int k = 0; k < NOUT; ++k) {
-    double v = warp_comb<MODE>(acc[k]);
-    if (lane == 0) smem[k][warp] = v;
-  }
-  __syncthreads();
-  if (warp == 0) {
-#pragma unroll
-    for (int k = 0; k < NOUT; ++k) {
-      double v = lane < RED_THREADS / 32 ? smem[k][lane] : ident<MODE>();
-      v = warp_comb<MODE>(v);
-      if (lane == 0) partials[(size_t)blockIdx.x * NOUT + k] = v;
-    }
-  }
-  // last-CTA fold in CTA order (deterministic)
-  if (threadIdx.x == 0) {
-    __threadfence();
-    unsigned int t = atomicAdd(ticket, 1u);
-    is_last = (t == gridDim.x - 1);
-  }
-  __syncthreads();
-  if (is_last) {
-    __threadfence();
-    if (warp == 0) {
-#pragma unroll
-      for (int k = 0; k < NOUT; ++k) {
-        double v = ident<MODE>();
-        // lane l folds CTAs l, l+32, ... in increasing order
-        for (unsigned int b = lane; b < gridDim.x; b += 32)
-          v = comb<MODE>(v, __ldcg(&partials[(size_t)b * NOUT + k]));
-        v = warp_comb<MODE>(v);
-        if (lane == 0) out[k] = v;
-      }
-      if (lane == 0) *ticket = 0u;
-    }
-  }
+  b2_grid_fold<NOUT, MODE>(acc, partials, ticket, out);
 }
 
-inline int red_grid(const b2_ctx* ctx, size_t n_items) {
-  size_t need = (n_items + (size_t)RED_THREADS * RED_UNROLL - 1) / ((size_t)RED_THREADS * RED_UNROLL);
-  size_t cap = (size_t)ctx->sm_count * 8;
-  if (cap > (size_t)B2_RED_MAX_BLOCKS) cap = B2_RED_MAX_BLOCKS;
-  if (need < 1) need = 1;
-  return (int)(need < cap ? need : cap);
-}
+// the grid of reduce_kernel, dot_multi_kernel and axpby_norm2_kernel: 1024 items (vectors or scalars) per CTA
+inline int red_grid(const b2_ctx* ctx, size_t n_items) { return b2_red_grid(ctx, n_items, RED_THREADS * RED_UNROLL); }
 
 template <typename T, bool CX, typename F>
 int launch_reduce(b2_ctx* ctx, F f, const void* x, const void* y, size_t n_real, double* out,
@@ -298,42 +228,7 @@ dot_multi_kernel(MultiPtrs p, size_t n_real, double* __restrict__ partials,
       }
     }
   }
-  __shared__ double smem[NOUT][RED_THREADS / 32];
-  __shared__ bool is_last;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-  for (int k = 0; k < NOUT; ++k) {
-    double v = warp_sum(acc[k]);
-    if (lane == 0) smem[k][warp] = v;
-  }
-  __syncthreads();
-  if (warp == 0) {
-#pragma unroll
-    for (int k = 0; k < NOUT; ++k) {
-      double v = lane < RED_THREADS / 32 ? smem[k][lane] : 0.0;
-      v = warp_sum(v);
-      if (lane == 0) partials[(size_t)blockIdx.x * NOUT + k] = v;
-    }
-  }
-  if (threadIdx.x == 0) {
-    __threadfence();
-    unsigned int t = atomicAdd(ticket, 1u);
-    is_last = (t == gridDim.x - 1);
-  }
-  __syncthreads();
-  if (is_last) {
-    __threadfence();
-    if (warp == 0) {
-#pragma unroll
-      for (int k = 0; k < NOUT; ++k) {
-        double v = 0.0;
-        for (unsigned int b = lane; b < gridDim.x; b += 32) v += __ldcg(&partials[(size_t)b * NOUT + k]);
-        v = warp_sum(v);
-        if (lane == 0) out[k] = v;
-      }
-      if (lane == 0) *ticket = 0u;
-    }
-  }
+  b2_grid_fold<NOUT, RED_SUM>(acc, partials, ticket, out);
 }
 
 template <typename T, bool CX, bool CONJ>
@@ -357,12 +252,7 @@ extern "C" int b2_dot(b2_ctx* ctx, const void* x, const void* y, size_t n, int d
                       double* out_dev, void* stream) {
   if (!ctx || !out_dev) return B2_ERR_ARG;
   cudaStream_t st = (cudaStream_t)stream;
-  if (n == 0) {
-    zero_out_kernel<<<1, 32, 0, st>>>(out_dev, 2, 0.0);
-    B2_LAUNCH_CHECK();
-    return B2_OK;
-  }
-  if (!x || !y) return B2_ERR_ARG;
+  if (n && (!x || !y)) return B2_ERR_ARG;  // n == 0 (a rank owning no elements) runs one CTA that reads nothing
   const bool cx = (dtype == B2_C64 || dtype == B2_C128);
   if (!cx) {  // imaginary part of a real dot is 0
     zero_out_kernel<<<1, 32, 0, st>>>(out_dev, 2, 0.0);
@@ -376,18 +266,13 @@ extern "C" int b2_norm_partial(b2_ctx* ctx, const void* x, size_t n, int dtype, 
                                double p, double* out_dev, void* stream) {
   if (!ctx || !out_dev) return B2_ERR_ARG;
   cudaStream_t st = (cudaStream_t)stream;
-  if (n == 0) {
-    zero_out_kernel<<<1, 32, 0, st>>>(out_dev, 1, kind == B2_NRM_MIN_ABS ? INFINITY : 0.0);
-    B2_LAUNCH_CHECK();
-    return B2_OK;
-  }
-  if (!x) return B2_ERR_ARG;
+  if (n && !x) return B2_ERR_ARG;  // n == 0 folds to the identity: 0, or +inf for the minimum
   switch (kind) {
     case B2_NRM_COUNT_NONZERO: return dispatch_reduce(ctx, CountNzF{0.0}, x, nullptr, n, dtype, out_dev, st);
     case B2_NRM_SUM_ABS: return dispatch_reduce(ctx, SumAbsF{0.0}, x, nullptr, n, dtype, out_dev, st);
     case B2_NRM_SUM_SQ: return dispatch_reduce(ctx, SumSqF{0.0}, x, nullptr, n, dtype, out_dev, st);
-    case B2_NRM_MAX_ABS: return dispatch_reduce(ctx, ExtAbsF<MODE_MAX>{0.0}, x, nullptr, n, dtype, out_dev, st);
-    case B2_NRM_MIN_ABS: return dispatch_reduce(ctx, ExtAbsF<MODE_MIN>{0.0}, x, nullptr, n, dtype, out_dev, st);
+    case B2_NRM_MAX_ABS: return dispatch_reduce(ctx, ExtAbsF<RED_MAX>{0.0}, x, nullptr, n, dtype, out_dev, st);
+    case B2_NRM_MIN_ABS: return dispatch_reduce(ctx, ExtAbsF<RED_MIN>{0.0}, x, nullptr, n, dtype, out_dev, st);
     case B2_NRM_SUM_POW: return dispatch_reduce(ctx, SumPowF{p}, x, nullptr, n, dtype, out_dev, st);
     default: return B2_ERR_ARG;
   }
@@ -397,14 +282,8 @@ extern "C" int b2_dot_multi(b2_ctx* ctx, int k, const void* const* xs, const voi
                             size_t n, int dtype, int conj_x, double* out_dev, void* stream) {
   if (!ctx || !out_dev || !xs || !ys || k < 1 || k > 4) return B2_ERR_ARG;
   cudaStream_t st = (cudaStream_t)stream;
-  if (n == 0) {
-    // a rank owning no elements: zero exactly the slots this dtype's layout uses (k doubles for real
-    // dtypes, k (re, im) pairs for complex) -- the caller packs other scalars right behind them
-    const bool cx0 = (dtype == B2_C64 || dtype == B2_C128);
-    zero_out_kernel<<<1, 32, 0, st>>>(out_dev, cx0 ? 2 * k : k, 0.0);
-    B2_LAUNCH_CHECK();
-    return B2_OK;
-  }
+  // the kernel writes exactly the slots this dtype's layout uses (k doubles for real dtypes, k (re, im) pairs for
+  // complex) -- the caller packs other scalars right behind them; n == 0 (a rank owning no elements) writes zeros
   MultiPtrs p;
   for (int i = 0; i < k; ++i) {
     p.x[i] = xs[i];
@@ -563,7 +442,7 @@ extern "C" int b2_norm_axis(b2_ctx* ctx, const void* x, size_t n_outer, size_t n
 // right after (x.x, s.s, c.c): one pass instead of an update pass plus a reduction pass, and three launches fewer
 // per iteration.  Real coefficients (device scalars), so complex arrays are processed as arrays of 2n reals; the
 // squared values are accumulated in float64 from the ROUNDED stored result, i.e. the same number a separate
-// b2_dot_multi pass over `out` would produce.  Deterministic last-CTA fold like reduce_kernel.
+// b2_dot_multi pass over `out` would produce.  Deterministic fold (b2_grid_fold) like reduce_kernel.
 namespace {
 template <typename T>
 __global__ void __launch_bounds__(RED_THREADS)
@@ -600,36 +479,11 @@ axpby_norm2_kernel(T* out, const double* a_dev, double a_scale, const T* x, cons
       acc = fma((double)o, (double)o, acc);
     }
   }
-  __shared__ double smem[RED_THREADS / 32];
-  __shared__ bool is_last;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  double v = warp_comb<MODE_SUM>(acc);
-  if (lane == 0) smem[warp] = v;
-  __syncthreads();
-  if (warp == 0) {
-    v = lane < RED_THREADS / 32 ? smem[lane] : 0.0;
-    v = warp_comb<MODE_SUM>(v);
-    if (lane == 0) partials[blockIdx.x] = v;
-  }
-  if (threadIdx.x == 0) {
-    __threadfence();
-    const unsigned int t = atomicAdd(ticket, 1u);
-    is_last = (t == gridDim.x - 1);
-  }
-  __syncthreads();
-  if (is_last) {
-    __threadfence();
-    if (warp == 0) {
-      double w = 0.0;
-      for (unsigned int bb = lane; bb < gridDim.x; bb += 32) w += __ldcg(&partials[bb]);
-      w = warp_comb<MODE_SUM>(w);
-      if (lane == 0) {
-        res[0] = w;
-        if (zero_second) res[1] = 0.0;
-        *ticket = 0u;
-      }
-    }
-  }
+  // the imaginary slot of complex data is zeroed by the thread that writes res[0], after every CTA has read *a_dev
+  // and *b_dev
+  b2_grid_fold<1, RED_SUM>(&acc, partials, ticket, res, [&] {
+    if (zero_second) res[1] = 0.0;
+  });
 }
 }  // namespace
 
@@ -641,12 +495,7 @@ extern "C" int b2_lincomb_dev_norm2(b2_ctx* ctx, void* out, const double* a_dev,
   const bool dbl = (dtype == B2_F64 || dtype == B2_C128);
   if (!cx && dtype != B2_F32 && dtype != B2_F64) return B2_ERR_DTYPE;
   cudaStream_t st = (cudaStream_t)stream;
-  if (n == 0) {
-    zero_out_kernel<<<1, 32, 0, st>>>(norm2_dev, cx ? 2 : 1, 0.0);
-    B2_LAUNCH_CHECK();
-    return B2_OK;
-  }
-  if (!out || !x || !y) return B2_ERR_ARG;
+  if (n && (!out || !x || !y)) return B2_ERR_ARG;  // n == 0 runs one CTA that reads no array and writes norm2 = 0
   const size_t n_real = cx ? 2 * n : n;
   const int V = dbl ? 2 : 4;
   const int vec = (b2_aligned16(out) && b2_aligned16(x) && b2_aligned16(y) && n_real >= (size_t)V) ? 1 : 0;

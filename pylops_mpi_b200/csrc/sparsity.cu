@@ -10,7 +10,7 @@
 
 namespace {
 
-constexpr int SP_THREADS = 256;
+constexpr int SP_THREADS = B2_RED_THREADS;
 
 struct SpParams {
   const void* base;
@@ -204,39 +204,7 @@ sparse_update_kernel(const __grid_constant__ SpParams p, double* __restrict__ pa
       acc[1] += (double)a2[1];
     }
   }
-  __shared__ double smem[2][SP_THREADS / 32];
-  __shared__ bool is_last;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-  for (int q = 0; q < 2; ++q) {
-    double v = warp_sum(acc[q]);
-    if (lane == 0) smem[q][warp] = v;
-  }
-  __syncthreads();
-  if (warp == 0) {
-#pragma unroll
-    for (int q = 0; q < 2; ++q) {
-      double v = lane < SP_THREADS / 32 ? smem[q][lane] : 0.0;
-      v = warp_sum(v);
-      if (lane == 0) partials[(size_t)blockIdx.x * 2 + q] = v;
-    }
-  }
-  if (threadIdx.x == 0) {
-    __threadfence();
-    is_last = (atomicAdd(ticket, 1u) == gridDim.x - 1);
-  }
-  __syncthreads();
-  if (is_last && warp == 0) {
-    __threadfence();
-#pragma unroll
-    for (int q = 0; q < 2; ++q) {
-      double v = 0.0;
-      for (unsigned int b = lane; b < gridDim.x; b += 32) v += __ldcg(&partials[(size_t)b * 2 + q]);
-      v = warp_sum(v);
-      if (lane == 0 && out) out[q] = v;
-    }
-    if (lane == 0) *ticket = 0u;
-  }
+  b2_grid_fold<2, RED_SUM>(acc, partials, ticket, out);
 }
 
 template <typename T, bool CX>
@@ -244,11 +212,7 @@ int launch(b2_ctx* ctx, const SpParams& p, double* sums, cudaStream_t st) {
   constexpr int V = Vec16<T>::N;
   const bool vec = b2_aligned16(p.base) && b2_aligned16(p.g) && b2_aligned16(p.xold) && b2_aligned16(p.xnew) &&
                    b2_aligned16(p.znew) && p.n_real >= (size_t)V;
-  size_t items = vec ? p.n_real / V : p.n_real;
-  size_t need = (items + (size_t)SP_THREADS * SP_UNROLL - 1) / ((size_t)SP_THREADS * SP_UNROLL);
-  size_t cap = (size_t)ctx->sm_count * 8;
-  if (cap > (size_t)B2_RED_MAX_BLOCKS) cap = B2_RED_MAX_BLOCKS;
-  int grid = (int)(need < 1 ? 1 : (need < cap ? need : cap));
+  const int grid = b2_red_grid(ctx, vec ? p.n_real / V : p.n_real, SP_THREADS * SP_UNROLL);
   if (vec)
     sparse_update_kernel<T, CX, true><<<grid, SP_THREADS, 0, st>>>(p, ctx->red_partials, ctx->tickets, sums);
   else
@@ -267,11 +231,9 @@ extern "C" int b2_sparse_update(b2_ctx* ctx, const void* base, const void* g, do
   const bool cx = dtype == B2_C64 || dtype == B2_C128;
   if (cx && kind == B2_THRESH_HALF) return B2_ERR_UNSUPPORTED;
   if (b2_dtype_size(dtype) == 0 || dtype == B2_BF16 || dtype == B2_I64) return B2_ERR_DTYPE;
-  if (n == 0) {  // a rank may own no model elements; its partial sums are still all-reduced
-    if (sums_dev) B2_CUDA(cudaMemsetAsync(sums_dev, 0, 2 * sizeof(double), (cudaStream_t)stream));
-    return B2_OK;
-  }
-  if (!base || !xnew || (znew && !xold)) return B2_ERR_ARG;
+  // a rank may own no model elements (n == 0, null arrays allowed): one CTA reads nothing and writes zero sums
+  // (if sums_dev is given), which are still all-reduced
+  if (n && (!base || !xnew || (znew && !xold))) return B2_ERR_ARG;
   SpParams p;
   p.base = base; p.g = g; p.xold = xold; p.xnew = xnew; p.znew = znew;
   p.alpha = alpha; p.thresh = thresh; p.c = c; p.kind = kind;

@@ -59,6 +59,7 @@ def sms(L):
 
 
 def red_cap(sms):
+    """the grid cap of the fused reductions, restating b2_red_grid in csrc/common.cuh"""
     return min(sms * 8, 2048)
 
 
@@ -778,7 +779,8 @@ def test_norm_axis_errors(L):
 
 def test_reductions_share_workspace_deterministically(L, sms):
     """calls with different grids back to back on one b2_ctx return the bits each returns alone, and a repeated
-    call the same bits: the last-CTA ticket is reset by every call, b2_sparse_update without sums included"""
+    call the same bits: the last-CTA ticket is reset by every call, b2_sparse_update without sums and
+    b2_lsqr_update included"""
     rng = np.random.default_rng(31)
     big = 9 * 256 * red_cap(sms) * 2 + 3
     xb = Buf(rnd(rng, big, "f64"), "f64")
@@ -789,7 +791,12 @@ def test_reductions_share_workspace_deterministically(L, sms):
     xu = Buf(rnd(rng, 700_003, "f32"), "f32")
     ou = Buf(np.zeros(700_003, np.float32), "f32")
     xc = Buf(rnd(rng, 50_001, "c128"), "c128")
-    outs = [dbuf(2) for _ in range(7)]
+    # the LSQR update with t1 = t2 = 0 and inv_alfa = 1 keeps x and sets w = v; w starts equal to v, so every call
+    # returns the same ||dk||^2
+    lv = rnd(rng, 200_003, "c64")
+    lx, lw, lvv, lvar = (Buf(a, "c64") for a in (rnd(rng, 200_003, "c64"), lv, lv, rnd(rng, 200_003, "c64")))
+    coef = Buf(np.array([0.0, 0.0, 0.75, 1.0]), "f64")
+    outs = [dbuf(2) for _ in range(8)]
     s = L.stream()
     calls = [
         lambda: L.lib.b2_norm_partial(L.ctx(), xb.ptr, big, 1, NRM_SQ, 0.0, outs[0].ptr, s),
@@ -802,6 +809,8 @@ def test_reductions_share_workspace_deterministically(L, sms):
                                        outs[3].ptr, 700_003, 0, s),
         lambda: L.lib.b2_lincomb_dev_norm2(L.ctx(), ou.ptr, None, 0.5, xu.ptr, None, 0.25, xu.ptr, 700_003, 0,
                                            outs[4].ptr, s),
+        lambda: L.lib.b2_lsqr_update(L.ctx(), lx.ptr, lw.ptr, lvv.ptr, lvar.ptr, 200_003, 2, coef.ptr, None,
+                                     outs[7].ptr, s),
         lambda: L.lib.b2_norm_partial(L.ctx(), xc.ptr, 50_001, 3, NRM_MAX, 0.0, outs[5].ptr, s),
         lambda: L.lib.b2_norm_partial(L.ctx(), xm.ptr, 300_001, 2, NRM_POW, 1.5, outs[6].ptr, s),
     ]
