@@ -175,7 +175,9 @@ int b2_first_derivative(b2_ctx* ctx, const void* x, void* y, const void* halo_lo
 /* rows of halo each side needs (1 or 2) */
 int b2_first_derivative_halo(int kind, int order, int adjoint, int* need_lo, int* need_hi);
 /* MPISecondDerivative per-rank apply (basicoperators/SecondDerivative.py:125-257): same contract as
- * b2_first_derivative (row block + up to 2 halo rows per side, exact-transpose adjoint), scale 1/sampling^2 */
+ * b2_first_derivative (row block + up to 2 halo rows per side, exact-transpose adjoint), scale 1/sampling^2.
+ * B2_ERR_HALO when n_lo / n_hi is less than the rows the block's taps read below / above it (centered with edge:
+ * two rows next to a global edge, one elsewhere) */
 int b2_second_derivative(b2_ctx* ctx, const void* x, void* y, const void* halo_lo, int n_lo,
                          const void* halo_hi, int n_hi, size_t nrows_local, size_t ncols, size_t row0,
                          size_t nrows_global, int kind, int edge, double sampling, int adjoint, int dtype,

@@ -20,7 +20,7 @@ from ..Distributed import group, send, recv
 from ..DistributedArray import DistributedArray, Partition
 from ..LinearOperator import MPILinearOperator
 from ..utils.decorators import reshaped
-from ..utils.partition import halo_plan, offsets
+from ..utils.partition import halo_launches, halo_plan, offsets
 
 _KINDS = {"forward": _lib.FD_FORWARD, "backward": _lib.FD_BACKWARD, "centered": _lib.FD_CENTERED}
 
@@ -159,10 +159,15 @@ class MPIFirstDerivative(MPILinearOperator):
                 if n_hi:
                     recv(x.base_comm, hi, x.rank + 1)
 
-        if nloc < 2 * (nl + nh) + 1:
+        steps = halo_launches(nloc, nl, nh, n_lo, n_hi)
+
+        def run(b, e, lo_n, hi_n, _after):
+            launch(b, e, lo if b == 0 else xr[b - lo_n:], lo_n, hi if e == nloc else xr[e:], hi_n)
+
+        if steps[0][4]:
             # tiny block: exchange, then one launch
             exchange()
-            launch(0, nloc, lo, n_lo, hi, n_hi)
+            run(*steps[0])
             return y
         # overlap: halo rows travel over NVLink on a side stream while the interior rows (whose
         # stencil never leaves this rank) are differentiated; two 1-2 row edge launches follow
@@ -175,14 +180,10 @@ class MPIFirstDerivative(MPILinearOperator):
             exchange()
             arrived = torch.cuda.Event()
             arrived.record(side)
-        i0, i1 = n_lo, nloc - n_hi
-        launch(i0, i1, xr[i0 - min(nl, i0):] if i0 else None, min(nl, i0),
-               xr[i1:] if i1 < nloc else None, min(nh, nloc - i1))
+        run(*steps[0])
         main.wait_event(arrived)
-        if i0:
-            launch(0, i0, lo, n_lo, xr[i0:], min(nh, nloc - i0))
-        if i1 < nloc:
-            launch(i1, nloc, xr[i1 - min(nl, i1):], min(nl, i1), hi, n_hi)
+        for s in steps[1:]:
+            run(*s)
         return y
 
 

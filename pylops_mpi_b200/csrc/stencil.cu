@@ -148,7 +148,7 @@ __device__ __forceinline__ bool load_row(const StencilParams& p, const T* x, con
   return true;
 }
 
-__device__ __forceinline__ const double* special_taps(const StencilParams& p, long long gi) {
+__host__ __device__ __forceinline__ const double* special_taps(const StencilParams& p, long long gi) {
   if (gi < SPECIAL) return p.top[gi];
   if (gi >= p.nglob - SPECIAL) return p.bot[p.nglob - 1 - gi];
   return nullptr;
@@ -451,6 +451,24 @@ int b2_fd_build_params(StencilParams* p, int n_lo, int n_hi, size_t nrows_local,
   return B2_OK;
 }
 
+// halo rows the block of p reads below (*lo) and above (*hi) itself: the non-zero taps of its first and last R
+// rows, with the same per-row tap choice as the kernels (taps never reach outside the global array)
+static void halo_reads(const StencilParams& p, int* lo, int* hi) {
+  *lo = *hi = 0;
+  auto scan = [&](long long r) {
+    const double* t = special_taps(p, p.row0 + r);
+    if (!t) t = p.interior;
+    for (int k = 0; k < NT; ++k) {
+      if (t[k] == 0.0) continue;
+      const long long s = r + k - R;   // local row read
+      if (s < 0 && -s > *lo) *lo = (int)-s;
+      if (s >= p.nloc && s - p.nloc + 1 > *hi) *hi = (int)(s - p.nloc + 1);
+    }
+  };
+  for (long long r = 0; r < p.nloc && r < R; ++r) scan(r);
+  for (long long r = (p.nloc - R > R ? p.nloc - R : R); r < p.nloc; ++r) scan(r);
+}
+
 extern "C" int b2_first_derivative(b2_ctx* ctx, const void* x, void* y, const void* halo_lo,
                                    int n_lo, const void* halo_hi, int n_hi, size_t nrows_local,
                                    size_t ncols, size_t row0, size_t nrows_global, int kind,
@@ -589,18 +607,17 @@ extern "C" int b2_second_derivative(b2_ctx* ctx, const void* x, void* y, const v
   if (n_lo < 0 || n_hi < 0 || n_lo > 8 || n_hi > 8) return B2_ERR_ARG;
   if (!halo_lo) n_lo = 0;
   if (!halo_hi) n_hi = 0;
-  int need_lo, need_hi;
-  int rc = b2_second_derivative_halo(kind, edge, adjoint, &need_lo, &need_hi);
+  int rc = b2_second_derivative_halo(kind, edge, adjoint, nullptr, nullptr);
   if (rc) return rc;
-  const long long avail_lo = (long long)row0, avail_hi = (long long)(nrows_global - row0 - nrows_local);
-  // interior rows only need the taps' reach; be strict with the tap reach of this kind
-  int reach_lo = need_lo, reach_hi = need_hi;
-  if (kind == B2_FD_CENTERED) reach_lo = reach_hi = 1;   // 2 only matters next to a global edge (checked by taps)
-  if (n_lo < (reach_lo < avail_lo ? reach_lo : avail_lo)) return B2_ERR_HALO;
-  if (n_hi < (reach_hi < avail_hi ? reach_hi : avail_hi)) return B2_ERR_HALO;
   StencilParams p;
   rc = b2_fd_build_params(&p, n_lo, n_hi, nrows_local, ncols, row0, nrows_global, kind, 3, edge, sampling, adjoint, 2);
   if (rc) return rc;
+  // the centered edge rows reach two rows away, interior rows one: check the rows this block's taps read
+  int read_lo, read_hi;
+  halo_reads(p, &read_lo, &read_hi);
+  const long long avail_lo = (long long)row0, avail_hi = (long long)(nrows_global - row0 - nrows_local);
+  if (n_lo < (read_lo < avail_lo ? read_lo : avail_lo)) return B2_ERR_HALO;
+  if (n_hi < (read_hi < avail_hi ? read_hi : avail_hi)) return B2_ERR_HALO;
   cudaStream_t st = (cudaStream_t)stream;
   switch (dtype) {
     case B2_F32: return launch_stencil<float>(ctx, x, y, halo_lo, halo_hi, p, st);

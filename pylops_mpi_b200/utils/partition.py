@@ -97,3 +97,25 @@ def halo_plan(row_sizes: Sequence[int], rank: int, need_lo: int, need_hi: int):
     send_lo = recv_counts(rank - 1)[1] if rank > 0 else 0          # what rank-1 wants above it
     send_hi = recv_counts(rank + 1)[0] if rank < size - 1 else 0   # what rank+1 wants below it
     return {"recv_lo": lo, "recv_hi": hi, "send_lo": send_lo, "send_hi": send_hi}
+
+
+def halo_launches(nloc: int, nl: int, nh: int, n_lo: int, n_hi: int):
+    """Stencil launches of one rank's block of ``nloc`` rows, for a stencil of reach (nl, nh) and n_lo / n_hi
+    received halo rows (``halo_plan``'s recv_lo / recv_hi).  Returns [(begin, end, lo, hi, after_exchange)] in
+    launch order: local rows [begin, end) with ``lo`` halo rows below ``begin`` (the received rows when begin == 0,
+    local rows otherwise) and ``hi`` rows from ``end`` on (the received rows when end == nloc).
+
+    A block too short to overlap is one launch after the exchange.  Otherwise the interior rows go first, while
+    the halo rows travel: they start at ``nl`` when rows are received below (not at ``n_lo``: a neighbour block
+    next to a global edge can send fewer rows than the reach, and row n_lo still needs ``nl`` rows below it), and
+    end at ``nloc - nh`` likewise; the one or two edge launches follow the exchange."""
+    if nloc < 2 * (nl + nh) + 1:
+        return [(0, nloc, n_lo, n_hi, True)]
+    i0 = nl if n_lo else 0
+    i1 = nloc - nh if n_hi else nloc
+    out = [(i0, i1, min(nl, i0), min(nh, nloc - i1), False)]
+    if i0:
+        out.append((0, i0, n_lo, min(nh, nloc - i0), True))
+    if i1 < nloc:
+        out.append((i1, nloc, min(nl, i1), n_hi, True))
+    return out

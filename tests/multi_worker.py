@@ -144,6 +144,32 @@ for dims, h in [((600,), 1.0), ((100, 37), 0.4), ((41, 9, 6), 0.4)]:
                   for ax, s in zip(axes, (1.0, 0.5, 2.0)))
         check(f"laplacian {dims}", host((Lop @ pm.DistributedArray.to_dist(xg)).asarray()), ref.ravel(), 1e-11, 1e-9)
 
+# ---- uneven row splits: 1-row blocks next to a global edge, applied on the split as given ---------------------
+# (_apply directly: the public matvec re-partitions to the balanced split first).  A neighbour next to a global
+# edge then sends fewer halo rows than the stencil's reach, and the overlapped exchange must still give every
+# launch the rows it reads.
+from pylops_mpi_b200.utils.partition import local_split_sizes  # noqa: E402
+N = 12 * P
+dims = (N, 5)
+uneven = [[N]] if P == 1 else [[1] + local_split_sizes(N - 1, P - 1), local_split_sizes(N - 1, P - 1) + [1]]
+if P >= 3:
+    uneven.append([1] + local_split_sizes(N - 2, P - 2) + [1])
+X = comm.bcast(rng.normal(0, 10, dims), 0)
+ops = [(pm.MPIFirstDerivative(dims, kind="centered", edge=e, order=order),
+        o.first_derivative_dense(N, 1.0, "centered", e, order), f"fd centered{order} edge={e}")
+       for order in (3, 5) for e in (False, True)]
+ops += [(pm.MPISecondDerivative(dims, kind=kind, edge=e), o.second_derivative_dense(N, 1.0, kind, e),
+         f"sd {kind} edge={e}") for kind in ("forward", "backward", "centered") for e in (False, True)]
+for rows in uneven:
+    off = np.cumsum([0] + rows)
+    xd = pm.DistributedArray(global_shape=dims, local_shapes=[(r, dims[1]) for r in rows], dtype=np.float64)
+    xd[:] = X[off[rank]:off[rank + 1]]
+    for Op, D, name in ops:
+        for adjoint in (False, True):
+            y = Op._apply(xd, adjoint=adjoint)
+            ref = ((D.T if adjoint else D) @ X)[off[rank]:off[rank + 1]]
+            check(f"{name} adj={adjoint} split={rows}", host(y.local_array), ref, 1e-12, 1e-10)
+
 # ---- BlockDiag / VStack / HStack (test_blockdiag.py:24-71, test_stack.py:29-79) ---------------------
 for ny, nx in [(101, 101), (301, 101)]:
     for dtype in (np.float64, np.complex128):
