@@ -167,21 +167,23 @@ int b2_sparse_update(b2_ctx* ctx, const void* base, const void* g, double alpha,
  * [nrows_global x ncols] array, global row offset row0.  halo_lo holds the n_lo
  * rows immediately before row0, halo_hi the n_hi rows immediately after the
  * block (the add_ghost_cells payload, DistributedArray.py:876-953); NULL / 0
- * at the global edges.  Complex arrays: pass the real dtype and 2*ncols. */
+ * at the global edges.  Complex arrays: pass the real dtype and 2*ncols.
+ * B2_ERR_HALO, for this and b2_second_derivative alike, when n_lo / n_hi is less than the rows that the taps of
+ * the block's own rows read below / above it.  That is at most the _halo reach, and no rows past a global edge. */
 int b2_first_derivative(b2_ctx* ctx, const void* x, void* y, const void* halo_lo, int n_lo,
                         const void* halo_hi, int n_hi, size_t nrows_local, size_t ncols,
                         size_t row0, size_t nrows_global, int kind, int order, int edge,
                         double sampling, int adjoint, int dtype, void* stream);
-/* rows of halo each side needs (1 or 2) */
+/* rows below / above itself that any row of the stencil reads (0 to 2), the wider of edge = 0 and 1 */
 int b2_first_derivative_halo(int kind, int order, int adjoint, int* need_lo, int* need_hi);
 /* MPISecondDerivative per-rank apply (basicoperators/SecondDerivative.py:125-257): same contract as
- * b2_first_derivative (row block + up to 2 halo rows per side, exact-transpose adjoint), scale 1/sampling^2.
- * B2_ERR_HALO when n_lo / n_hi is less than the rows the block's taps read below / above it (centered with edge:
- * two rows next to a global edge, one elsewhere) */
+ * b2_first_derivative (row block + up to 2 halo rows per side, exact-transpose adjoint, B2_ERR_HALO rule),
+ * scale 1/sampling^2 */
 int b2_second_derivative(b2_ctx* ctx, const void* x, void* y, const void* halo_lo, int n_lo,
                          const void* halo_hi, int n_hi, size_t nrows_local, size_t ncols, size_t row0,
                          size_t nrows_global, int kind, int edge, double sampling, int adjoint, int dtype,
                          void* stream);
+/* rows below / above itself that any row of the stencil reads (0 to 2) */
 int b2_second_derivative_halo(int kind, int edge, int adjoint, int* need_lo, int* need_hi);
 /* rank-local first (deriv=1) / second (deriv=2) derivative along the MIDDLE axis of a C-ordered
  * [n_outer][n_axis][n_inner] block: the non-partitioned directions of MPILaplacian / MPIGradient

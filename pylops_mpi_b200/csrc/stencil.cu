@@ -26,6 +26,10 @@ namespace {
 constexpr int R = 2;           // max stencil radius
 constexpr int NT = 2 * R + 1;  // taps per row
 constexpr int SPECIAL = 4;     // rows at each global edge with their own taps
+constexpr long long LONG_AXIS = 2000;   // an axis whose middle row is far from both edges
+
+// one derivative operator: deriv 1 or 2, kind B2_FD_*, order 3 / 5 (centered first derivative only), edge, adjoint
+struct FdOp { int deriv, kind, order, edge, adjoint; };
 
 struct StencilParams {
   double interior[NT];
@@ -117,11 +121,11 @@ void fwd_taps(long long i, long long N, int deriv, int kind, int order, int edge
   }
 }
 
-void row_taps(long long i, long long N, int deriv, int kind, int order, int edge, int adjoint, double t[NT]) {
-  if (!adjoint) { fwd_taps(i, N, deriv, kind, order, edge, t); return; }
+void row_taps(long long i, long long N, const FdOp& op, double t[NT]) {
+  if (!op.adjoint) { fwd_taps(i, N, op.deriv, op.kind, op.order, op.edge, t); return; }
   for (int k = -R; k <= R; ++k) {
     double f[NT];
-    fwd_taps(i + k, N, deriv, kind, order, edge, f);   // zero outside [0, N)
+    fwd_taps(i + k, N, op.deriv, op.kind, op.order, op.edge, f);   // zero outside [0, N)
     t[k + R] = f[-k + R];
   }
 }
@@ -410,36 +414,59 @@ int launch_stencil(b2_ctx* ctx, const void* x, void* y, const void* lo, const vo
   return B2_OK;
 }
 
+// dtype F32 / F64 (complex data: the real dtype and twice the columns)
+int launch_stencil(b2_ctx* ctx, const void* x, void* y, const void* lo, const void* hi, const StencilParams& p,
+                   int dtype, cudaStream_t st) {
+  switch (dtype) {
+    case B2_F32: return launch_stencil<float>(ctx, x, y, lo, hi, p, st);
+    case B2_F64: return launch_stencil<double>(ctx, x, y, lo, hi, p, st);
+    default: return B2_ERR_DTYPE;
+  }
+}
+
 }  // namespace
 
-extern "C" int b2_first_derivative_halo(int kind, int order, int adjoint, int* need_lo,
-                                        int* need_hi) {
-  int lo, hi;
-  if (kind == B2_FD_FORWARD) { lo = adjoint ? 1 : 0; hi = adjoint ? 0 : 1; }
-  else if (kind == B2_FD_BACKWARD) { lo = adjoint ? 0 : 1; hi = adjoint ? 1 : 0; }
-  else if (kind == B2_FD_CENTERED && order == 3) { lo = hi = 1; }
-  else if (kind == B2_FD_CENTERED && order == 5) { lo = hi = 2; }
-  else return B2_ERR_UNSUPPORTED;
+// B2_ERR_UNSUPPORTED for an operator row_taps does not define (the entry points check deriv themselves)
+static int fd_validate(const FdOp& op) {
+  if (op.kind != B2_FD_FORWARD && op.kind != B2_FD_BACKWARD && op.kind != B2_FD_CENTERED) return B2_ERR_UNSUPPORTED;
+  if (op.deriv == 1 && op.kind == B2_FD_CENTERED && op.order != 3 && op.order != 5) return B2_ERR_UNSUPPORTED;
+  return B2_OK;
+}
+
+// how far below (*need_lo) and above (*need_hi) itself any row reads through op's non-zero taps (null: not
+// written): on a long axis, rows 0..SPECIAL-1 and their mirror images have the edge taps, row SPECIAL the interior ones
+static int fd_reach(const FdOp& op, int* need_lo, int* need_hi) {
+  const int rc = fd_validate(op);
+  if (rc) return rc;
+  int lo = 0, hi = 0;
+  for (long long i = 0; i <= SPECIAL; ++i)
+    for (long long row : {i, LONG_AXIS - 1 - i}) {
+      double t[NT];
+      row_taps(row, LONG_AXIS, op, t);
+      for (int k = 0; k < NT; ++k) {
+        if (t[k] == 0.0) continue;
+        if (R - k > lo) lo = R - k;
+        if (k - R > hi) hi = k - R;
+      }
+    }
   if (need_lo) *need_lo = lo;
   if (need_hi) *need_hi = hi;
   return B2_OK;
 }
 
-int b2_fd_build_params(StencilParams* p, int n_lo, int n_hi, size_t nrows_local, size_t ncols,
-                       size_t row0, size_t nrows_global, int kind, int order, int edge,
-                       double sampling, int adjoint, int deriv = 1) {
-  if (kind != B2_FD_FORWARD && kind != B2_FD_BACKWARD && kind != B2_FD_CENTERED)
-    return B2_ERR_UNSUPPORTED;
-  if (deriv == 1 && kind == B2_FD_CENTERED && order != 3 && order != 5) return B2_ERR_UNSUPPORTED;
+static int b2_fd_build_params(StencilParams* p, int n_lo, int n_hi, size_t nrows_local, size_t ncols,
+                              size_t row0, size_t nrows_global, const FdOp& op, double sampling) {
+  const int rc = fd_validate(op);
+  if (rc) return rc;
   if (row0 + nrows_local > nrows_global) return B2_ERR_ARG;
   const long long N = (long long)nrows_global;
-  // interior taps = taps of a row far from both edges of a very long axis
-  row_taps(1000, 2000, deriv, kind, order, edge, adjoint, p->interior);
+  // interior taps = taps of a row far from both edges of a long axis
+  row_taps(LONG_AXIS / 2, LONG_AXIS, op, p->interior);
   for (int s = 0; s < SPECIAL; ++s) {
-    row_taps(s, N, deriv, kind, order, edge, adjoint, p->top[s]);
-    row_taps(N - 1 - s, N, deriv, kind, order, edge, adjoint, p->bot[s]);
+    row_taps(s, N, op, p->top[s]);
+    row_taps(N - 1 - s, N, op, p->bot[s]);
   }
-  p->scale = (deriv == 2) ? 1.0 / (sampling * sampling) : 1.0 / sampling;
+  p->scale = (op.deriv == 2) ? 1.0 / (sampling * sampling) : 1.0 / sampling;
   p->batch_stride = 0;
   p->nbatch = 1;
   p->nloc = (long long)nrows_local;
@@ -469,38 +496,55 @@ static void halo_reads(const StencilParams& p, int* lo, int* hi) {
   for (long long r = (p.nloc - R > R ? p.nloc - R : R); r < p.nloc; ++r) scan(r);
 }
 
-extern "C" int b2_first_derivative(b2_ctx* ctx, const void* x, void* y, const void* halo_lo,
-                                   int n_lo, const void* halo_hi, int n_hi, size_t nrows_local,
-                                   size_t ncols, size_t row0, size_t nrows_global, int kind,
-                                   int order, int edge, double sampling, int adjoint, int dtype,
-                                   void* stream) {
+// one rank's row block with its halo rows: b2_first_derivative and b2_second_derivative
+static int fd_block(b2_ctx* ctx, const void* x, void* y, const void* halo_lo, int n_lo, const void* halo_hi,
+                    int n_hi, size_t nrows_local, size_t ncols, size_t row0, size_t nrows_global, const FdOp& op,
+                    double sampling, int dtype, void* stream) {
   if (!ctx) return B2_ERR_ARG;
   if (nrows_local == 0 || ncols == 0) return B2_OK;
   if (!x || !y) return B2_ERR_ARG;
   if (n_lo < 0 || n_hi < 0 || n_lo > 8 || n_hi > 8) return B2_ERR_ARG;
   if (!halo_lo) n_lo = 0;
   if (!halo_hi) n_hi = 0;
-  int need_lo, need_hi;
-  int rc = b2_first_derivative_halo(kind, order, adjoint, &need_lo, &need_hi);
-  if (rc) return rc;
-  // a missing halo is only legal where the stencil would read outside the global array
-  const long long avail_lo = (long long)row0, avail_hi = (long long)(nrows_global - row0 - nrows_local);
-  if (n_lo < (need_lo < avail_lo ? need_lo : avail_lo)) return B2_ERR_HALO;
-  if (n_hi < (need_hi < avail_hi ? need_hi : avail_hi)) return B2_ERR_HALO;
   StencilParams p;
-  rc = b2_fd_build_params(&p, n_lo, n_hi, nrows_local, ncols, row0, nrows_global, kind, order,
-                          edge, sampling, adjoint);
+  const int rc = b2_fd_build_params(&p, n_lo, n_hi, nrows_local, ncols, row0, nrows_global, op, sampling);
   if (rc) return rc;
-  cudaStream_t st = (cudaStream_t)stream;
-  switch (dtype) {
-    case B2_F32: return launch_stencil<float>(ctx, x, y, halo_lo, halo_hi, p, st);
-    case B2_F64: return launch_stencil<double>(ctx, x, y, halo_lo, halo_hi, p, st);
-    default: return B2_ERR_DTYPE;
-  }
+  int read_lo, read_hi;
+  halo_reads(p, &read_lo, &read_hi);
+  if (n_lo < read_lo || n_hi < read_hi) return B2_ERR_HALO;
+  return launch_stencil(ctx, x, y, halo_lo, halo_hi, p, dtype, (cudaStream_t)stream);
 }
 
+extern "C" int b2_first_derivative_halo(int kind, int order, int adjoint, int* need_lo, int* need_hi) {
+  int lo0, hi0, lo1, hi1;   // without / with edge handling: the wider reach is reported
+  const int rc = fd_reach(FdOp{1, kind, order, 0, adjoint}, &lo0, &hi0);
+  if (rc) return rc;
+  fd_reach(FdOp{1, kind, order, 1, adjoint}, &lo1, &hi1);
+  if (need_lo) *need_lo = lo0 > lo1 ? lo0 : lo1;
+  if (need_hi) *need_hi = hi0 > hi1 ? hi0 : hi1;
+  return B2_OK;
+}
 
-extern "C" int b2_second_derivative_halo(int kind, int edge, int adjoint, int* need_lo, int* need_hi);
+extern "C" int b2_first_derivative(b2_ctx* ctx, const void* x, void* y, const void* halo_lo, int n_lo,
+                                   const void* halo_hi, int n_hi, size_t nrows_local, size_t ncols, size_t row0,
+                                   size_t nrows_global, int kind, int order, int edge, double sampling, int adjoint,
+                                   int dtype, void* stream) {
+  return fd_block(ctx, x, y, halo_lo, n_lo, halo_hi, n_hi, nrows_local, ncols, row0, nrows_global,
+                  FdOp{1, kind, order, edge, adjoint}, sampling, dtype, stream);
+}
+
+// ---- MPISecondDerivative per-rank apply (basicoperators/SecondDerivative.py:125-257) -----------------
+extern "C" int b2_second_derivative_halo(int kind, int edge, int adjoint, int* need_lo, int* need_hi) {
+  return fd_reach(FdOp{2, kind, 0, edge, adjoint}, need_lo, need_hi);
+}
+
+extern "C" int b2_second_derivative(b2_ctx* ctx, const void* x, void* y, const void* halo_lo, int n_lo,
+                                    const void* halo_hi, int n_hi, size_t nrows_local, size_t ncols, size_t row0,
+                                    size_t nrows_global, int kind, int edge, double sampling, int adjoint,
+                                    int dtype, void* stream) {
+  return fd_block(ctx, x, y, halo_lo, n_lo, halo_hi, n_hi, nrows_local, ncols, row0, nrows_global,
+                  FdOp{2, kind, 0, edge, adjoint}, sampling, dtype, stream);
+}
 
 // ---- peer-memory halo handle ------------------------------------------------------------------------------------
 struct b2_halo {
@@ -558,9 +602,9 @@ extern "C" int b2_derivative_peer(b2_ctx* ctx, b2_halo* h, const void* x, void* 
                                   double sampling, int adjoint, int dtype, void* stream) {
   if (!ctx || !h || !x || !y || (deriv != 1 && deriv != 2)) return B2_ERR_ARG;
   if (dtype != B2_F32 && dtype != B2_F64) return B2_ERR_DTYPE;
+  const FdOp op{deriv, kind, order, edge, adjoint};
   int need_lo, need_hi;
-  int rc = deriv == 1 ? b2_first_derivative_halo(kind, order, adjoint, &need_lo, &need_hi)
-                      : b2_second_derivative_halo(kind, edge, adjoint, &need_lo, &need_hi);
+  int rc = fd_reach(op, &need_lo, &need_hi);
   if (rc) return rc;
   const size_t esz = b2_dtype_size(dtype), V = 16 / esz;
   if ((long long)nrows_local < (need_lo > need_hi ? need_lo : need_hi)) return B2_ERR_HALO;
@@ -568,8 +612,7 @@ extern "C" int b2_derivative_peer(b2_ctx* ctx, b2_halo* h, const void* x, void* 
   if ((size_t)(need_lo > need_hi ? need_lo : need_hi) * ncols * esz > h->cap) return B2_ERR_WORKSPACE;
   const int n_lo = h->box[0] ? need_lo : 0, n_hi = h->box[2] ? need_hi : 0;
   StencilParams p;
-  rc = b2_fd_build_params(&p, n_lo, n_hi, nrows_local, ncols, row0, nrows_global, kind, deriv == 1 ? order : 3, edge,
-                          sampling, adjoint, deriv);
+  rc = b2_fd_build_params(&p, n_lo, n_hi, nrows_local, ncols, row0, nrows_global, op, sampling);
   if (rc) return rc;
   HaloPeer hp;
   hp.mine = h->box[1];
@@ -585,47 +628,6 @@ extern "C" int b2_derivative_peer(b2_ctx* ctx, b2_halo* h, const void* x, void* 
                          : launch_vec<double, true>(x, y, nullptr, nullptr, p, hp, st);
 }
 
-// ---- MPISecondDerivative per-rank apply (basicoperators/SecondDerivative.py:125-257) -----------------
-extern "C" int b2_second_derivative_halo(int kind, int edge, int adjoint, int* need_lo, int* need_hi) {
-  int lo, hi;
-  if (kind == B2_FD_FORWARD) { lo = adjoint ? 2 : 0; hi = adjoint ? 0 : 2; }
-  else if (kind == B2_FD_BACKWARD) { lo = adjoint ? 0 : 2; hi = adjoint ? 2 : 0; }
-  else if (kind == B2_FD_CENTERED) { lo = hi = edge ? 2 : 1; }   // the edge rows reach two rows away
-  else return B2_ERR_UNSUPPORTED;
-  if (need_lo) *need_lo = lo;
-  if (need_hi) *need_hi = hi;
-  return B2_OK;
-}
-
-extern "C" int b2_second_derivative(b2_ctx* ctx, const void* x, void* y, const void* halo_lo, int n_lo,
-                                    const void* halo_hi, int n_hi, size_t nrows_local, size_t ncols, size_t row0,
-                                    size_t nrows_global, int kind, int edge, double sampling, int adjoint,
-                                    int dtype, void* stream) {
-  if (!ctx) return B2_ERR_ARG;
-  if (nrows_local == 0 || ncols == 0) return B2_OK;
-  if (!x || !y) return B2_ERR_ARG;
-  if (n_lo < 0 || n_hi < 0 || n_lo > 8 || n_hi > 8) return B2_ERR_ARG;
-  if (!halo_lo) n_lo = 0;
-  if (!halo_hi) n_hi = 0;
-  int rc = b2_second_derivative_halo(kind, edge, adjoint, nullptr, nullptr);
-  if (rc) return rc;
-  StencilParams p;
-  rc = b2_fd_build_params(&p, n_lo, n_hi, nrows_local, ncols, row0, nrows_global, kind, 3, edge, sampling, adjoint, 2);
-  if (rc) return rc;
-  // the centered edge rows reach two rows away, interior rows one: check the rows this block's taps read
-  int read_lo, read_hi;
-  halo_reads(p, &read_lo, &read_hi);
-  const long long avail_lo = (long long)row0, avail_hi = (long long)(nrows_global - row0 - nrows_local);
-  if (n_lo < (read_lo < avail_lo ? read_lo : avail_lo)) return B2_ERR_HALO;
-  if (n_hi < (read_hi < avail_hi ? read_hi : avail_hi)) return B2_ERR_HALO;
-  cudaStream_t st = (cudaStream_t)stream;
-  switch (dtype) {
-    case B2_F32: return launch_stencil<float>(ctx, x, y, halo_lo, halo_hi, p, st);
-    case B2_F64: return launch_stencil<double>(ctx, x, y, halo_lo, halo_hi, p, st);
-    default: return B2_ERR_DTYPE;
-  }
-}
-
 // ---- rank-local derivative along the MIDDLE axis of a C-ordered [n_outer][n_axis][n_inner] block ------
 // (the non-partitioned directions of MPILaplacian / MPIGradient: Laplacian.py:97-126, Gradient.py:101-119
 //  wrap a serial pylops First/SecondDerivative per rank; here the same stencil kernel runs batched)
@@ -636,19 +638,15 @@ extern "C" int b2_derivative_axis(b2_ctx* ctx, const void* x, void* y, size_t n_
   if (n_outer == 0 || n_axis == 0 || n_inner == 0) return B2_OK;
   if (!x || !y) return B2_ERR_ARG;
   StencilParams p;
-  int rc = b2_fd_build_params(&p, 0, 0, n_axis, n_inner, 0, n_axis, kind, order, edge, sampling, adjoint, deriv);
+  int rc = b2_fd_build_params(&p, 0, 0, n_axis, n_inner, 0, n_axis, FdOp{deriv, kind, order, edge, adjoint},
+                              sampling);
   if (rc) return rc;
-  p.nbatch = 1;
   p.batch_stride = (long long)(n_axis * n_inner);
   cudaStream_t st = (cudaStream_t)stream;
   for (size_t done = 0; done < n_outer; done += 65535) {
     p.nbatch = (int)(n_outer - done < 65535 ? n_outer - done : 65535);
     const size_t off = done * n_axis * n_inner * b2_dtype_size(dtype);
-    switch (dtype) {
-      case B2_F32: rc = launch_stencil<float>(ctx, (const char*)x + off, (char*)y + off, nullptr, nullptr, p, st); break;
-      case B2_F64: rc = launch_stencil<double>(ctx, (const char*)x + off, (char*)y + off, nullptr, nullptr, p, st); break;
-      default: return B2_ERR_DTYPE;
-    }
+    rc = launch_stencil(ctx, (const char*)x + off, (char*)y + off, nullptr, nullptr, p, dtype, st);
     if (rc) return rc;
   }
   return B2_OK;

@@ -7,7 +7,8 @@ rows taken from the same global device array, so one output array holds the whol
   is one tap times 1.0, so it is compared BIT FOR BIT with the dense oracle matrices (and their transposes for
   the adjoint), for every kind / order / edge, every small N, f32 and f64, the 16-byte vector kernel and the
   generic one, and row splits with 1-row ranks next to the global edges.
-* The halo contract: a call given fewer halo rows than it reads returns B2_ERR_HALO, never a different result.
+* The halo contract: a call is refused with B2_ERR_HALO exactly when it is given fewer halo rows than the taps of
+  its rows read, and an accepted call gives the same rows as with the full halo.
 * Random data: element-wise rounding bounds against a high-precision reference, and bitwise invariance of the
   result under the row split and the kernel variant (vector vs generic).
 * The grid.y chunking of ``b2_derivative_axis`` and the multi-chunk pipeline of ``b2_first_derivative_host``.
@@ -23,7 +24,8 @@ import pylops_mpi_oracle as o
 from pylops_mpi_b200.utils.partition import halo_launches, halo_plan, local_split_sizes, offsets
 
 KINDS = {"forward": 0, "backward": 1, "centered": 2}
-B2_ERR_HALO = 2003
+B2_OK, B2_ERR_DTYPE, B2_ERR_ARG, B2_ERR_HALO = 0, 2001, 2002, 2003
+B2_ERR_WORKSPACE, B2_ERR_UNSUPPORTED, B2_ERR_ALIGN = 2004, 2005, 2006
 # (deriv, kind, order, edge): every operator the stencil kernels apply
 OPS = ([(1, k, order, e) for k, order in (("forward", 3), ("backward", 3), ("centered", 3), ("centered", 5))
         for e in (False, True)] + [(2, k, 3, e) for k in KINDS for e in (False, True)])
@@ -59,6 +61,14 @@ def reach(L, op, adjoint):
             L.check(L.lib.b2_second_derivative_halo(KINDS[kind], int(edge), int(adjoint), C.byref(lo), C.byref(hi)))
         _REACH[key] = (lo.value, hi.value)
     return _REACH[key]
+
+
+def block_reads(M, r0, r1):
+    """(rows below, rows above) the block [r0, r1) reads: the non-zeros of its rows of the operator matrix M"""
+    cols = np.nonzero(M[r0:r1])[1]
+    if cols.size == 0:
+        return 0, 0
+    return max(0, r0 - int(cols.min())), max(0, int(cols.max()) - (r1 - 1))
 
 
 def dense(op, N, h=1.0):
@@ -170,7 +180,11 @@ def test_operator_matrix_exact(L, N, dt, layout):
             Ys = device_array((len(S), N, ncols), tdt, vec, float("nan"))
             for s, rows in enumerate(S):
                 apply_split(L, op, X, Ys[s], N, list(rows), 1.0, adjoint)
-            # (b): every block again with fewer halo rows on one side: B2_ERR_HALO or the same rows
+            # (b): every block again with fewer halo rows on one side: refused exactly when the taps of its rows
+            # read a missing row (the non-zeros of the oracle matrix, sampling 1); where the oracle cannot build the
+            # matrix, B2_ERR_HALO or the same rows
+            D = dense(op, N)
+            M = None if D is None else (D.T if adjoint else D)
             cuts = []
             for s, rows, q, r0, r1 in blocks:
                 n_lo, n_hi = full_halo(L, op, adjoint, N, r0, r1)
@@ -180,7 +194,13 @@ def test_operator_matrix_exact(L, N, dt, layout):
             short = []
             for k, (s, rows, q, r0, r1, a, b, n_lo, n_hi) in enumerate(cuts):
                 rc = call(L, op, X, Zs[k], N, r0, r1, a, b, 1.0, adjoint)
-                assert rc in (0, B2_ERR_HALO), f"{name} split={rows} rank {q} halo ({a},{b}): status {rc}"
+                if M is None:
+                    assert rc in (0, B2_ERR_HALO), f"{name} split={rows} rank {q} halo ({a},{b}): status {rc}"
+                else:
+                    rl, rh = block_reads(M, r0, r1)
+                    want = B2_ERR_HALO if a < rl or b < rh else 0
+                    assert rc == want, (f"{name} split={rows} rank {q} (rows {r0}:{r1}) reads ({rl},{rh}), given "
+                                        f"({a},{b}) halo rows: status {rc}, want {want}")
                 if rc == 0:
                     short.append((k, s, rows, q, r0, r1, a, b, n_lo, n_hi))
             got = Ys.cpu().numpy()
@@ -194,9 +214,8 @@ def test_operator_matrix_exact(L, N, dt, layout):
                     f"{name} split={rows} rank {q} (rows {r0}:{r1}): {a} lo / {b} hi halo rows instead of "
                     f"{n_lo} / {n_hi} returned B2_OK with a different result")
             mats[adjoint] = got[0][:, :N]
-            D = dense(op, N)
-            if D is not None:
-                ref = (D.T if adjoint else D).astype(npdt)
+            if M is not None:
+                ref = M.astype(npdt)
                 bad = np.argwhere(mats[adjoint] != ref)
                 assert bad.size == 0, (f"{name}: matrix differs from the oracle at {bad[:4].tolist()}: "
                                        f"got {mats[adjoint][tuple(bad[0])]}, want {ref[tuple(bad[0])]}")
@@ -218,6 +237,173 @@ def test_second_derivative_short_halo_is_an_error(L):
     op = (2, "centered", 3, False)
     assert call(L, op, X, Y, 8, 2, 8, 1, 0, 1.0, True) == 0
     assert call(L, op, X, Y, 8, 2, 8, 0, 0, 1.0, True) == B2_ERR_HALO
+
+
+# (op, adjoint, block [r0, r1) of N = 8 rows, lo / hi halo rows given, status)
+SHORT_HALO_CASES = {
+    "d1_centered3_rows0to1_hi_0": ((1, "centered", 3, False), False, 0, 1, 0, 0, B2_OK),
+    "d1_centered3_adj_rows0to1_hi_0": ((1, "centered", 3, False), True, 0, 1, 0, 0, B2_ERR_HALO),
+    "d1_centered3_edge_rows0to1_hi_0": ((1, "centered", 3, True), False, 0, 1, 0, 0, B2_ERR_HALO),
+    "d1_centered5_rows0to2_hi_0": ((1, "centered", 5, False), False, 0, 2, 0, 0, B2_OK),
+    "d1_centered5_edge_rows0to1_hi_1": ((1, "centered", 5, True), False, 0, 1, 0, 1, B2_OK),
+    "d1_centered5_edge_rows0to2_hi_1": ((1, "centered", 5, True), False, 0, 2, 0, 1, B2_OK),
+    "d1_centered5_edge_rows0to3_hi_1": ((1, "centered", 5, True), False, 0, 3, 0, 1, B2_ERR_HALO),
+    "d1_forward_rows3to4_hi_0": ((1, "forward", 3, False), False, 3, 4, 1, 0, B2_ERR_HALO),
+    "d1_forward_adj_rows3to4_lo_0": ((1, "forward", 3, False), True, 3, 4, 0, 1, B2_ERR_HALO),
+    "d1_forward_adj_rows3to4_hi_0": ((1, "forward", 3, False), True, 3, 4, 1, 0, B2_OK),
+}
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("case", list(SHORT_HALO_CASES))
+def test_first_derivative_short_halo_cases(L, case):
+    """first-derivative blocks given fewer halo rows than the operator's reach: refused exactly when their own rows
+    read a missing row; an accepted block gives the rows of a full-halo call"""
+    op, adjoint, r0, r1, n_lo, n_hi, want = SHORT_HALO_CASES[case]
+    gen = torch.Generator(device="cuda").manual_seed(3)
+    X = torch.randn(8, 32, dtype=torch.float64, device="cuda", generator=gen)
+    Y = device_array((8, 32), torch.float64, True, float("nan"))
+    Z = device_array((8, 32), torch.float64, True, float("nan"))
+    assert call(L, op, X, Y, 8, r0, r1, n_lo, n_hi, 1.0, adjoint) == want
+    if want == B2_OK:
+        L.check(call(L, op, X, Z, 8, r0, r1, *full_halo(L, op, adjoint, 8, r0, r1), 1.0, adjoint))
+        assert torch.equal(Y[r0:r1], Z[r0:r1])
+
+
+def test_halo_reach_values(L):
+    """the rows below / above itself that any row of each stencil reads, (forward operator, adjoint)"""
+    first = {("forward", 3): ((0, 1), (1, 0)), ("backward", 3): ((1, 0), (0, 1)),
+             ("centered", 3): ((1, 1), (1, 1)), ("centered", 5): ((2, 2), (2, 2))}
+    second = {("forward", False): ((0, 2), (2, 0)), ("forward", True): ((0, 2), (2, 0)),
+              ("backward", False): ((2, 0), (0, 2)), ("backward", True): ((2, 0), (0, 2)),
+              ("centered", False): ((1, 1), (1, 1)), ("centered", True): ((2, 2), (2, 2))}
+
+    def halo(fn, *args):
+        lo, hi = C.c_int(-1), C.c_int(-1)
+        return fn(*args, C.byref(lo), C.byref(hi)), (lo.value, hi.value)
+
+    for (kind, order), want in first.items():
+        for adjoint in (0, 1):
+            assert halo(L.lib.b2_first_derivative_halo, KINDS[kind], order, adjoint) == (B2_OK, want[adjoint]), \
+                f"d1 {kind}{order} adj={adjoint}"
+    for (kind, edge), want in second.items():
+        for adjoint in (0, 1):
+            assert halo(L.lib.b2_second_derivative_halo, KINDS[kind], int(edge), adjoint) == (B2_OK, want[adjoint]), \
+                f"d2 {kind} edge={edge} adj={adjoint}"
+    assert L.lib.b2_first_derivative_halo(KINDS["centered"], 5, 0, None, None) == B2_OK
+    assert L.lib.b2_second_derivative_halo(KINDS["centered"], 1, 1, None, None) == B2_OK
+    for bad in (-1, 3):
+        assert halo(L.lib.b2_first_derivative_halo, bad, 3, 0)[0] == B2_ERR_UNSUPPORTED
+        assert halo(L.lib.b2_second_derivative_halo, bad, 0, 0)[0] == B2_ERR_UNSUPPORTED
+    for adjoint in (0, 1):
+        assert halo(L.lib.b2_first_derivative_halo, KINDS["centered"], 4, adjoint)[0] == B2_ERR_UNSUPPORTED
+
+
+# the argument checks of the five entry points that run the stencil kernels: every row changes one or two arguments
+# of a valid call (a None entry passes NULL) and gives the status; rows that pass every check launch on valid memory
+FD = dict(ctx=1, x=1, y=1, lo=None, n_lo=0, hi=None, n_hi=0, nloc=8, ncols=32, row0=0, nglob=8, kind=2, order=3,
+          edge=0, h=1.0, adj=0, dtype=1)
+FD_ARGS = [
+    ({}, B2_OK), ({"ctx": None}, B2_ERR_ARG), ({"ctx": None, "nloc": 0}, B2_ERR_ARG),
+    ({"nloc": 0, "x": None}, B2_OK), ({"ncols": 0, "y": None}, B2_OK), ({"x": None}, B2_ERR_ARG),
+    ({"y": None}, B2_ERR_ARG), ({"n_lo": -1}, B2_ERR_ARG), ({"n_hi": -1}, B2_ERR_ARG),
+    ({"lo": 1, "n_lo": 9}, B2_ERR_ARG), ({"hi": 1, "n_hi": 9}, B2_ERR_ARG), ({"n_lo": 9}, B2_ERR_ARG),
+    ({"kind": 3}, B2_ERR_UNSUPPORTED), ({"kind": -1}, B2_ERR_UNSUPPORTED), ({"kind": 3, "nloc": 0}, B2_OK),
+    ({"kind": 3, "dtype": 3}, B2_ERR_UNSUPPORTED), ({"dtype": 3}, B2_ERR_DTYPE), ({"dtype": 99}, B2_ERR_DTYPE),
+    ({"dtype": 99, "nloc": 0}, B2_OK), ({"row0": 4, "nloc": 8, "lo": 1, "n_lo": 1}, B2_ERR_ARG),
+]
+FD1_ARGS = FD_ARGS + [({"order": 4}, B2_ERR_UNSUPPORTED), ({"order": 4, "kind": 0}, B2_OK),
+                      ({"order": 4, "dtype": 3}, B2_ERR_UNSUPPORTED)]
+AX = dict(ctx=1, x=1, y=1, n_outer=1, n_axis=8, n_inner=32, deriv=1, kind=2, order=3, edge=0, h=1.0, adj=0, dtype=1)
+AX_ARGS = [
+    ({}, B2_OK), ({"deriv": 2}, B2_OK), ({"ctx": None}, B2_ERR_ARG), ({"deriv": 0}, B2_ERR_ARG),
+    ({"deriv": 3}, B2_ERR_ARG), ({"deriv": 0, "n_outer": 0}, B2_ERR_ARG), ({"n_outer": 0, "x": None}, B2_OK),
+    ({"n_axis": 0}, B2_OK), ({"n_inner": 0}, B2_OK), ({"x": None}, B2_ERR_ARG), ({"y": None}, B2_ERR_ARG),
+    ({"kind": 3}, B2_ERR_UNSUPPORTED), ({"kind": 3, "n_inner": 0}, B2_OK), ({"order": 4}, B2_ERR_UNSUPPORTED),
+    ({"order": 4, "deriv": 2}, B2_OK), ({"kind": 3, "dtype": 99}, B2_ERR_UNSUPPORTED), ({"dtype": 3}, B2_ERR_DTYPE),
+    ({"dtype": 99}, B2_ERR_DTYPE),
+]
+# the handle's boxes hold one 32-column float64 row per side: every row here fails before the launch
+PEER = dict(ctx=1, h=1, x=1, y=1, nloc=8, ncols=32, row0=0, nglob=8, deriv=1, kind=2, order=3, edge=0, sh=1.0, adj=0,
+            dtype=1)
+PEER_ARGS = [
+    ({"row0": 4}, B2_ERR_ARG), ({"ctx": None}, B2_ERR_ARG), ({"h": None}, B2_ERR_ARG), ({"x": None}, B2_ERR_ARG),
+    ({"y": None}, B2_ERR_ARG), ({"deriv": 0}, B2_ERR_ARG), ({"deriv": 3}, B2_ERR_ARG),
+    ({"deriv": 0, "dtype": 3}, B2_ERR_ARG), ({"dtype": 3}, B2_ERR_DTYPE), ({"dtype": 3, "kind": 3}, B2_ERR_DTYPE),
+    ({"kind": 3}, B2_ERR_UNSUPPORTED), ({"kind": -1, "nloc": 0}, B2_ERR_UNSUPPORTED),
+    ({"order": 4}, B2_ERR_UNSUPPORTED), ({"order": 4, "deriv": 2, "row0": 4}, B2_ERR_ARG),
+    ({"nloc": 0}, B2_ERR_HALO), ({"order": 5, "nloc": 1}, B2_ERR_HALO),
+    ({"deriv": 2, "edge": 1, "nloc": 1}, B2_ERR_HALO),
+    ({"ncols": 31}, B2_ERR_ALIGN), ({"ncols": 14}, B2_ERR_ALIGN), ({"x": 8}, B2_ERR_ALIGN),
+    ({"order": 5}, B2_ERR_WORKSPACE), ({"deriv": 2, "kind": 0}, B2_ERR_WORKSPACE),
+]
+HOST = dict(ctx=1, x=1, y=1, nglob=8, ncols=32, begin=0, end=8, kind=2, order=3, edge=0, h=1.0, adj=0, dtype=1)
+HOST_ARGS = [
+    ({}, B2_OK), ({"ctx": None}, B2_ERR_ARG), ({"end": 9}, B2_ERR_ARG), ({"begin": 5, "end": 4}, B2_ERR_ARG),
+    ({"begin": 4, "end": 4, "x": None}, B2_OK), ({"ncols": 0, "y": None}, B2_OK), ({"x": None}, B2_ERR_ARG),
+    ({"y": None}, B2_ERR_ARG), ({"dtype": 3}, B2_ERR_DTYPE), ({"dtype": 3, "kind": 3}, B2_ERR_DTYPE),
+    ({"kind": 3}, B2_ERR_UNSUPPORTED), ({"order": 4}, B2_ERR_UNSUPPORTED), ({"order": 4, "kind": 1}, B2_OK),
+]
+
+
+@pytest.mark.gpu
+def test_entry_point_argument_errors(L):
+    X = device_array((8, 32), torch.float64, True, 1.0)
+    Y = device_array((8, 32), torch.float64, True)
+    ptr = {"x": X.data_ptr(), "y": Y.data_ptr(), "lo": X.data_ptr(), "hi": X.data_ptr()}
+    st = L.stream()
+
+    def args(base, change, fields):
+        a = dict(base, **change)
+        out = []
+        for f in fields:
+            v = a[f]
+            if f == "ctx":
+                v = L.ctx() if v else None
+            elif f in ptr and v is not None:
+                v = ptr[f] + (v if v > 1 else 0)          # an int > 1 is a byte offset
+            out.append(v)
+        return out
+
+    fd = ["ctx", "x", "y", "lo", "n_lo", "hi", "n_hi", "nloc", "ncols", "row0", "nglob", "kind"]
+    bad = []
+    for change, want in FD1_ARGS:
+        rc = L.lib.b2_first_derivative(*args(FD, change, fd + ["order", "edge", "h", "adj", "dtype"]), st)
+        if rc != want:
+            bad.append(("b2_first_derivative", change, rc, want))
+    for change, want in FD_ARGS:
+        rc = L.lib.b2_second_derivative(*args(FD, change, fd + ["edge", "h", "adj", "dtype"]), st)
+        if rc != want:
+            bad.append(("b2_second_derivative", change, rc, want))
+    for change, want in AX_ARGS:
+        rc = L.lib.b2_derivative_axis(*args(AX, change, ["ctx", "x", "y", "n_outer", "n_axis", "n_inner", "deriv",
+                                                         "kind", "order", "edge", "h", "adj", "dtype"]), st)
+        if rc != want:
+            bad.append(("b2_derivative_axis", change, rc, want))
+    cap = 32 * 8
+    box = torch.zeros(L.lib.b2_halo_bytes(cap), dtype=torch.uint8, device="cuda")
+    boxes = (C.c_void_p * 1)(box.data_ptr())
+    h = C.c_void_p()
+    L.check(L.lib.b2_halo_create(0, 1, boxes, cap, C.byref(h)), "b2_halo_create")
+    try:
+        for change, want in PEER_ARGS:
+            a = args(PEER, change, ["ctx", "h", "x", "y", "nloc", "ncols", "row0", "nglob", "deriv", "kind", "order",
+                                    "edge", "sh", "adj", "dtype"])
+            a[1] = h if a[1] else None
+            rc = L.lib.b2_derivative_peer(*a, st)
+            if rc != want:
+                bad.append(("b2_derivative_peer", change, rc, want))
+    finally:
+        L.check(L.lib.b2_halo_destroy(h), "b2_halo_destroy")
+    xh, yh = np.ones((8, 32)), np.zeros((8, 32))
+    ptr.update(x=xh.ctypes.data, y=yh.ctypes.data)
+    for change, want in HOST_ARGS:
+        rc = L.lib.b2_first_derivative_host(*args(HOST, change, ["ctx", "x", "y", "nglob", "ncols", "begin", "end",
+                                                                 "kind", "order", "edge", "h", "adj", "dtype"]))
+        if rc != want:
+            bad.append(("b2_first_derivative_host", change, rc, want))
+    torch.cuda.synchronize()
+    assert not bad, "\n".join(f"{fn} {change}: status {rc}, want {want}" for fn, change, rc, want in bad)
 
 
 # --------------------------------------------------------------------------
