@@ -326,11 +326,12 @@ int b2_batched_gemm_allgather(b2_ctx* ctx, const void* G, const void* x, void* y
                               int npeers, size_t nsl, size_t nx, size_t ny, size_t nz, int adjoint,
                               int dtype, void* stream);
 /* Tensor-core (wgmma) plan for the same product, float32 / complex64 only (Fredholm1.py:119-129, 147-167).
- * G is operator state: plan creation splits G and G^H (the reference's `saveGt`, :105-106) ONCE into three bf16
- * planes each ("bf16x3": 24 significant bits, six MMAs per k-step -> float32-class accuracy on the bf16 tensor
- * pipe); complex64 runs as one real product over the (re,im)-interleaved views.  b2_fredholm_apply packs x
- * (one small kernel) and runs the batched product; with npeers > 0 the epilogue also stores every output
- * element to the same offset of the peers' IPC-mapped buffers (fused Allgather of Fredholm1.py:131-132,
+ * G is operator state: plan creation splits G and G^H (the reference's `saveGt`, :105-106) ONCE into two fp16
+ * planes each ("fp16x2": v*2^e = hi + lo*2^-11 with a power-of-two scale 2^e per output row, 22 significant
+ * bits, three MMAs per k-step -> float32-class accuracy on the fp16 tensor pipe); complex64 runs as one real
+ * product over the (re,im)-interleaved views.  b2_fredholm_apply packs x (one small kernel, which also takes a
+ * power-of-two scale per column of x) and runs the batched product; with npeers > 0 the epilogue also stores
+ * every output element to the same offset of the peers' IPC-mapped buffers (fused Allgather of Fredholm1.py:131-132,
  * completion = any stream-ordered cross-rank barrier after it).  The plan owns its device workspaces; applies
  * of one plan must be stream-ordered.  G must stay valid only during b2_fredholm_plan_create. */
 typedef struct b2_fredholm_plan b2_fredholm_plan;

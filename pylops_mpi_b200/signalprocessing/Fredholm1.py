@@ -5,7 +5,6 @@ written straight into the output buffer."""
 from __future__ import annotations
 
 import ctypes as C
-import os
 
 import numpy as np
 import torch
@@ -14,6 +13,10 @@ from .. import _lib
 from ..comm import COMM_WORLD, resolve
 from ..DistributedArray import DistributedArray, Partition
 from ..LinearOperator import MPILinearOperator
+
+# products per slice (nx * ny * nz) from which float32 / complex64 slices run on the tensor-core plan; smaller slices
+# take the SIMT kernel
+TC_MIN_PRODUCTS = 32768
 
 
 class MPIFredholm1(MPILinearOperator):
@@ -62,13 +65,11 @@ class MPIFredholm1(MPILinearOperator):
                     self._arena[(adjoint, b)] = (*base_comm.symm_alloc(nelem * esz), nelem)
             self._toggle = {False: 0, True: 0}
             self._flag = torch.zeros(1, dtype=torch.float64, device="cuda")   # float64 -> peer-memory all-reduce
-        # tensor-core plan (csrc/fredholm_tc.cu): float32 / complex64 products run on wgmma with fp16x2 / bf16x3 split
-        # operands (float32-class accuracy); G and G^H planes are built once here.  B2_FREDHOLM_TC=0 keeps the SIMT
-        # kernel, =1 forces the tensor-core path for every shape (tests), default: slices of >= 32768 products.
-        mode = os.environ.get("B2_FREDHOLM_TC", "auto")
+        # tensor-core plan (csrc/fredholm_tc.cu): float32 / complex64 products run on wgmma with fp16x2 split operands
+        # (float32-class accuracy) for slices of >= TC_MIN_PRODUCTS products; G and G^H planes are built once here
         self._plan = None
-        if self._tdtype in (torch.float32, torch.complex64) and mode != "0" and \
-                (mode == "1" or self.nx * self.ny * self.nz >= 32768) and self.nsl > 0:
+        if self._tdtype in (torch.float32, torch.complex64) and \
+                self.nx * self.ny * self.nz >= TC_MIN_PRODUCTS and self.nsl > 0:
             h = C.c_void_p()
             _lib.check(_lib.lib.b2_fredholm_plan_create(_lib.ctx(), self.G.data_ptr(), self.nsl, self.nx, self.ny, self.nz,
                                                         _lib.code(self._tdtype), C.byref(h)), "b2_fredholm_plan_create")

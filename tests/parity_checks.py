@@ -272,6 +272,7 @@ def run_all(pm, comm, full_size: bool = True):
 
     # ---- Fredholm1 KAT (test_fredholm.py:36-95), SIMT, tensor-core and fused peer paths -----------------------
     def fredholm_kat():
+        F1 = pm.signalprocessing.Fredholm1
         nsl, nx, ny = 21, 4, 6
         ext = [o.local_split((nsl,), P, r)[0] for r in range(P)]
         if 1 in ext or 0 in ext:
@@ -287,8 +288,9 @@ def run_all(pm, comm, full_size: bool = True):
                 refy = o.fredholm1(G_loc, xv.ravel().astype(G.dtype), nz)
                 refx = o.fredholm1(G_loc, refy, nz, adjoint=True)
                 xd = pm.DistributedArray.to_dist(xv.ravel(), partition=pm.Partition.BROADCAST)
-                for mode in ("0", "1"):
-                    os.environ["B2_FREDHOLM_TC"] = mode
+                # the default threshold keeps these shapes on the SIMT kernel, threshold 0 puts complex64 on the plan
+                for tc_min in (F1.TC_MIN_PRODUCTS, 0):
+                    saved, F1.TC_MIN_PRODUCTS = F1.TC_MIN_PRODUCTS, tc_min
                     try:
                         for fused in (False, True) if P > 1 else (False,):
                             Fr = pm.MPIFredholm1(G_loc[rank].astype(dtype), nz=nz, dtype=dtype, fused=fused)
@@ -296,12 +298,12 @@ def run_all(pm, comm, full_size: bool = True):
                                 y = Fr @ xd
                                 ok, det = _close(_host(y.local_array), refy, 1e-5, 0)
                                 if not ok:
-                                    return False, f"nz={nz} {dtype.__name__} tc={mode} fused={fused}: {det}"
+                                    return False, f"nz={nz} {dtype.__name__} tc_min={tc_min} fused={fused}: {det}"
                                 ok, det = _close(_host((Fr.H @ y).local_array), refx, 1e-4, 0)
                                 if not ok:
-                                    return False, f"adjoint nz={nz} {dtype.__name__} tc={mode} fused={fused}: {det}"
+                                    return False, f"adjoint nz={nz} {dtype.__name__} tc_min={tc_min} fused={fused}: {det}"
                     finally:
-                        os.environ.pop("B2_FREDHOLM_TC", None)
+                        F1.TC_MIN_PRODUCTS = saved
         return True, "arange KAT"
     check("MPIFredholm1 arange KAT (SIMT / tensor cores / fused peer all-gather)", fredholm_kat)
 

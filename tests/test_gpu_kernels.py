@@ -623,20 +623,17 @@ def test_gemm_bf16_worker_shapes():
 # MPIFredholm1 split-precision product on the tensor cores (b2_fredholm_plan_* / b2_fredholm_apply)
 # --------------------------------------------------------------------------
 # Componentwise, scale-invariant bound |y - y_ref| <= gamma (|op(G)| |x|), gamma = (c_split + K'/8) 2^-24, K' = real
-# contraction length (2K for complex).  c_split from the operand formats (fredholm_tc.cu): fp16x2 keeps 22 bits per
-# operand and drops lo*lo, 3 * 2^-22 per product, c_split = 16; bf16x3 represents each float exactly and drops terms
-# <= 2^-24 each, c_split = 8.  K'/8 allows 2u per fp32 tensor-core accumulation over a k16 step.
-C_SPLIT = {"h2": 16, "b3": 8}
+# contraction length (2K for complex).  c_split from the operand format (fredholm_tc.cu): fp16x2 keeps 22 bits per
+# operand and drops lo*lo, 3 * 2^-22 per product, c_split = 16.  K'/8 allows 2u per fp32 tensor-core accumulation over
+# a k16 step.
+C_SPLIT = 16
 
 
 class FredholmPlan:
-    """b2_fredholm_plan for G (torch, nsl x nx x ny, float32 or complex64) in the given split mode and pack kernel
-    choice (both read from the environment at plan creation)"""
+    """b2_fredholm_plan for G (torch, nsl x nx x ny, float32 or complex64)"""
 
-    def __init__(self, L, monkeypatch, G, nz, mode, pack_small=1):
-        monkeypatch.setenv("B2_FREDHOLM_MODE", mode)
-        monkeypatch.setenv("B2_FREDHOLM_PACK_SMALL", str(pack_small))
-        self.L, self.G, self.nz, self.mode = L, G, nz, mode
+    def __init__(self, L, G, nz):
+        self.L, self.G, self.nz = L, G, nz
         self.h = C.c_void_p()
         nsl, nx, ny = G.shape
         L.check(L.lib.b2_fredholm_plan_create(L.ctx(), G.data_ptr(), nsl, nx, ny, nz, L.code(G.dtype),
@@ -659,7 +656,7 @@ class FredholmPlan:
         self.L.lib.b2_fredholm_plan_destroy(self.h)
 
 
-def fredholm_check(G, x, y, adjoint, mode, what=""):
+def fredholm_check(G, x, y, adjoint, what=""):
     """y against op(G) x in float64 / complex128, componentwise bound above"""
     cx = G.is_complex()
     wide = torch.complex128 if cx else torch.float64
@@ -671,7 +668,7 @@ def fredholm_check(G, x, y, adjoint, mode, what=""):
     else:
         M = opG.abs() @ x.double().abs()
     kp = opG.shape[2] * (2 if cx else 1)
-    bound = (C_SPLIT[mode] + kp / 8) * 2.0 ** -24 * M
+    bound = (C_SPLIT + kp / 8) * 2.0 ** -24 * M
     d = y.to(wide) - ref
     parts = (d.real, d.imag) if cx else (d,)
     for p in parts:
@@ -698,15 +695,14 @@ def distinct_pow2(rng, n, lo=-30, hi=30):
     return np.resize(rng.permutation(np.arange(lo, hi + 1)), n)
 
 
-@pytest.mark.parametrize("mode", ["h2", "b3"])
 @pytest.mark.parametrize("cx", [False, True])
 @pytest.mark.parametrize("adjoint", [False, True])
-def test_fredholm_tc_scaled_inputs(L, monkeypatch, mode, cx, adjoint):
+def test_fredholm_tc_scaled_inputs(L, cx, adjoint):
     """rows of op(G) and columns of x scaled by distinct powers 2^[-30, 30], entries down to 2^-24 below their
     column's maximum, one all-zero row of op(G) and one all-zero column of x (exact zeros in y).  fp16x2 scales every
     row of op(G) and every column of x separately and undoes the scales in the epilogue: an off-by-one in either
     shows up here."""
-    rng = np.random.default_rng(100 + 4 * cx + 2 * adjoint + (mode == "b3"))
+    rng = np.random.default_rng(100 + 4 * cx + 2 * adjoint)
     nsl, nx, ny, nz = 3, 70, 90, 40
     m, K = (ny, nx) if adjoint else (nx, ny)
     G = sign_unit(rng, (nsl, nx, ny), cx)
@@ -723,36 +719,34 @@ def test_fredholm_tc_scaled_inputs(L, monkeypatch, mode, cx, adjoint):
     zc = 7
     x[:, :, zc] = 0
     Gd, xd = to_dev(G, cx), to_dev(x, cx)
-    with FredholmPlan(L, monkeypatch, Gd, nz, mode) as pl:
+    with FredholmPlan(L, Gd, nz) as pl:
         y = pl.apply(xd, adjoint)
-        fredholm_check(Gd, xd, y, adjoint, mode, "scaled")
+        fredholm_check(Gd, xd, y, adjoint, "scaled")
         assert bool((y[:, zr, :] == 0).all()) and bool((y[:, :, zc] == 0).all())
 
 
-@pytest.mark.parametrize("mode,eg,ex", [("h2", -118, 118), ("h2", 118, -118), ("h2", -62, -62),
-                                        ("b3", -100, 100), ("b3", 100, -100)])
+@pytest.mark.parametrize("eg,ex", [(-118, 118), (118, -118), (-62, -62)])
 @pytest.mark.parametrize("cx", [False, True])
 @pytest.mark.parametrize("adjoint", [False, True])
-def test_fredholm_tc_extreme_magnitudes(L, monkeypatch, mode, eg, ex, cx, adjoint):
+def test_fredholm_tc_extreme_magnitudes(L, eg, ex, cx, adjoint):
     """G scaled by 2^eg and x by 2^ex.  For (-118, 118) and the reverse the products are O(1): the fp16x2 scales must
     reach 2^+-126 for the scaled operands to stay finite fp16.  For (-62, -62) the result is a normal float32
-    (~2^-120) although the product of the two inverse scales is below the float32 range.  bf16x3 stops at 2^+-100, so
-    that its third plane stays a normal number."""
+    (~2^-120) although the product of the two inverse scales is below the float32 range."""
     rng = np.random.default_rng(1000 + eg + 3 * ex + 2 * cx + adjoint)
     nsl, nx, ny, nz = 2, 40, 56, 24
     G = sign_unit(rng, (nsl, nx, ny), cx) * 2.0 ** eg
     x = sign_unit(rng, (nsl, nx if adjoint else ny, nz), cx) * 2.0 ** ex
     Gd, xd = to_dev(G, cx), to_dev(x, cx)
-    with FredholmPlan(L, monkeypatch, Gd, nz, mode) as pl:
+    with FredholmPlan(L, Gd, nz) as pl:
         y = pl.apply(xd, adjoint)
         assert bool(torch.isfinite(torch.view_as_real(y) if cx else y).all()), "non-finite y for finite inputs"
-        fredholm_check(Gd, xd, y, adjoint, mode, f"G*2^{eg}, x*2^{ex}")
+        fredholm_check(Gd, xd, y, adjoint, f"G*2^{eg}, x*2^{ex}")
 
 
 @pytest.mark.parametrize("e", [-62, 80])
 @pytest.mark.parametrize("cx", [False, True])
 @pytest.mark.parametrize("adjoint", [False, True])
-def test_fredholm_tc_h2_exact_cancellation(L, monkeypatch, e, cx, adjoint):
+def test_fredholm_tc_h2_exact_cancellation(L, e, cx, adjoint):
     """fp16x2 with G and x both scaled by 2^e and products that cancel exactly: y must be exactly zero.  The inverse
     scales of a row of op(G) and a column of x then multiply to a power of two outside the float32 range (2^-152,
     2^132), which must not turn the zero into 0 * inf = NaN."""
@@ -765,14 +759,13 @@ def test_fredholm_tc_h2_exact_cancellation(L, monkeypatch, e, cx, adjoint):
     u = 1 + rng.integers(0, 1024, (nsl, K // 2, nz)) / 1024
     x = sign * np.repeat(u, 2, axis=1) * (1 - 1j if cx else 1) * 2.0 ** e
     Gd, xd = to_dev(G, cx), to_dev(x, cx)
-    with FredholmPlan(L, monkeypatch, Gd, nz, "h2") as pl:
+    with FredholmPlan(L, Gd, nz) as pl:
         y = pl.apply(xd, adjoint)
         assert bool((y == 0).all()), f"{int((y != 0).sum())} nonzero entries, e.g. {y.flatten()[torch.nonzero((y != 0).flatten())[0]].item()}"
 
 
-@pytest.mark.parametrize("mode", ["h2", "b3"])
 @pytest.mark.parametrize("cx,shape", [(True, (160, 200, 136, 40)), (False, (50, 130, 260, 300))])
-def test_fredholm_tc_multi_tile(L, monkeypatch, mode, cx, shape):
+def test_fredholm_tc_multi_tile(L, cx, shape):
     """more than two 128 x 128 output tiles per SM in both directions: CTAs move through several tiles and slices
     (ring stage / phase across tiles, accumulator reset).  The real shape packs x with the generic kernel forward
     (K = 260 > 256) and with the single-pass one in the adjoint."""
@@ -782,53 +775,56 @@ def test_fredholm_tc_multi_tile(L, monkeypatch, mode, cx, shape):
         assert nsl * -(-m // 128) * -(-n // 128) > 2 * sm_count(L)
     rng = np.random.default_rng(300 + nx)
     Gd = to_dev(sign_unit(rng, (nsl, nx, ny), cx), cx)
-    with FredholmPlan(L, monkeypatch, Gd, nz, mode) as pl:
+    with FredholmPlan(L, Gd, nz) as pl:
         for adjoint in (False, True):
             xd = to_dev(sign_unit(rng, (nsl, nx if adjoint else ny, nz), cx), cx)
-            fredholm_check(Gd, xd, pl.apply(xd, adjoint), adjoint, mode, f"adjoint={adjoint}")
+            fredholm_check(Gd, xd, pl.apply(xd, adjoint), adjoint, f"adjoint={adjoint}")
 
 
-@pytest.mark.parametrize("mode", ["h2", "b3"])
 @pytest.mark.parametrize("cx", [False, True])
 @pytest.mark.parametrize("nz", [1, 17, 33])
-def test_fredholm_tc_pack_kernels_agree(L, monkeypatch, mode, cx, nz):
-    """for contractions over <= 256 values of k both x-pack kernels apply; they must build identical planes and
-    scales, hence bit-identical y"""
+def test_fredholm_tc_pack_kernels_agree(L, cx, nz):
+    """a contraction over K <= 256 values of k packs x with the single-pass kernel.  The same product with the
+    contraction padded by zeros to K = 257 (zero columns of G and zero rows of x forward, zero rows of G and x in the
+    adjoint) packs x with the generic kernel.  The padding leaves every row and column scale unchanged and adds only
+    zero products, so both kernels must build identical planes and scales, hence bit-identical y"""
     rng = np.random.default_rng(400 + nz + 2 * cx)
-    nsl, nx, ny = 2, 100, 200
+    nsl, nx, ny, kpadded = 2, 100, 200, 257
     G = sign_unit(rng, (nsl, nx, ny), cx) * 2.0 ** rng.integers(-8, 8, (nsl, nx, 1))
     Gd = to_dev(G, cx)
     for adjoint in (False, True):
         x = sign_unit(rng, (nsl, nx if adjoint else ny, nz), cx) * 2.0 ** rng.integers(-20, 20, (1, 1, nz))
         xd = to_dev(x, cx)
+        pad = kpadded - x.shape[1]
+        Gp = np.pad(G, ((0, 0), (0, pad), (0, 0)) if adjoint else ((0, 0), (0, 0), (0, pad)))
+        xp = np.pad(x, ((0, 0), (0, pad), (0, 0)))
         ys = []
-        for ps in (1, 0):
-            with FredholmPlan(L, monkeypatch, Gd, nz, mode, pack_small=ps) as pl:
-                ys.append(pl.apply(xd, adjoint))
-        fredholm_check(Gd, xd, ys[0], adjoint, mode, "single-pass pack")
+        for g, xx in ((Gd, xd), (to_dev(Gp, cx), to_dev(xp, cx))):
+            with FredholmPlan(L, g, nz) as pl:
+                ys.append(pl.apply(xx, adjoint))
+        fredholm_check(Gd, xd, ys[0], adjoint, "single-pass pack")
         assert torch.equal(bits(torch.view_as_real(ys[0]) if cx else ys[0]),
                            bits(torch.view_as_real(ys[1]) if cx else ys[1])), f"adjoint={adjoint}"
 
 
-@pytest.mark.parametrize("mode", ["h2", "b3"])
 @pytest.mark.parametrize("cx", [False, True])
-def test_fredholm_tc_repeated_applies(L, monkeypatch, mode, cx):
+def test_fredholm_tc_repeated_applies(L, cx):
     """one plan, several applies: forward x1, forward x2 (other column scales), adjoint, forward x1 again, which must
     reproduce the first result bit for bit (no stale scales or planes from the applies in between)"""
-    rng = np.random.default_rng(500 + 2 * cx + (mode == "b3"))
+    rng = np.random.default_rng(500 + 2 * cx)
     nsl, nx, ny, nz = 3, 96, 80, 24
     Gd = to_dev(sign_unit(rng, (nsl, nx, ny), cx), cx)
     x1 = to_dev(sign_unit(rng, (nsl, ny, nz), cx) * 2.0 ** distinct_pow2(rng, nz)[None, None, :], cx)
     x2 = to_dev(sign_unit(rng, (nsl, ny, nz), cx) * 2.0 ** distinct_pow2(rng, nz)[None, None, :], cx)
     x3 = to_dev(sign_unit(rng, (nsl, nx, nz), cx) * 2.0 ** distinct_pow2(rng, nz)[None, None, :], cx)
-    with FredholmPlan(L, monkeypatch, Gd, nz, mode) as pl:
+    with FredholmPlan(L, Gd, nz) as pl:
         y1 = pl.apply(x1, False)
         y2 = pl.apply(x2, False)
         y3 = pl.apply(x3, True)
         y4 = pl.apply(x1, False)
         for y, x, adj, what in ((y1, x1, False, "x1"), (y2, x2, False, "x2"), (y3, x3, True, "adjoint"),
                                 (y4, x1, False, "x1 again")):
-            fredholm_check(Gd, x, y, adj, mode, what)
+            fredholm_check(Gd, x, y, adj, what)
         assert torch.equal(bits(torch.view_as_real(y4) if cx else y4), bits(torch.view_as_real(y1) if cx else y1))
 
 
@@ -837,15 +833,14 @@ def peer_outputs(nfloat, npeers, y_off):
     return guarded(1, nfloat, nfloat, y_off), [guarded(1, nfloat, nfloat, 4) for _ in range(npeers)]
 
 
-@pytest.mark.parametrize("mode", ["h2", "b3"])
 @pytest.mark.parametrize("cx", [False, True])
-def test_fredholm_tc_peer_epilogue(L, monkeypatch, mode, cx):
+def test_fredholm_tc_peer_epilogue(L, cx):
     """the fused all-gather epilogue on one GPU: three local buffers stand in for the peers.  y and every peer hold
     the same bits; a y one float off 8-byte alignment (scalar stores) gives the same bits as the aligned one"""
-    rng = np.random.default_rng(600 + 2 * cx + (mode == "b3"))
+    rng = np.random.default_rng(600 + 2 * cx)
     nsl, nx, ny, nz = 3, 70, 90, 40
     Gd = to_dev(sign_unit(rng, (nsl, nx, ny), cx), cx)
-    with FredholmPlan(L, monkeypatch, Gd, nz, mode) as pl:
+    with FredholmPlan(L, Gd, nz) as pl:
         for adjoint in (False, True):
             m, K = (ny, nx) if adjoint else (nx, ny)
             xd = to_dev(sign_unit(rng, (nsl, K, nz), cx) * 2.0 ** distinct_pow2(rng, nz)[None, None, :], cx)
@@ -863,7 +858,7 @@ def test_fredholm_tc_peer_epilogue(L, monkeypatch, mode, cx):
                 outs[y_off] = yv.clone()
             assert torch.equal(bits(outs[4]), bits(outs[5])), f"scalar stores differ, adjoint={adjoint}"
             y = outs[4].view(-1).view(torch.complex64) if cx else outs[4].view(-1)
-            fredholm_check(Gd, xd, y.view(nsl, m, nz), adjoint, mode, f"adjoint={adjoint}")
+            fredholm_check(Gd, xd, y.view(nsl, m, nz), adjoint, f"adjoint={adjoint}")
 
 
 @pytest.mark.parametrize("dt", ["f32", "c64", "f64"])

@@ -590,14 +590,12 @@ def test_cg_cgls_on_stacked_arrays(pm):
     np.testing.assert_allclose(host(xl10.asarray()), xo.asarray(), rtol=1e-8, atol=1e-10)
 
 
-@pytest.mark.parametrize("mode", ["h2", "b3"])
 @pytest.mark.parametrize("shape", [(21, 4, 6, 5), (5, 100, 70, 9), (2, 129, 257, 65), (3, 128, 128, 64)])
 @pytest.mark.parametrize("dtype", [np.complex64, np.float32])
-def test_fredholm1_tensor_core_path(pm, monkeypatch, mode, shape, dtype):
-    """MPIFredholm1 on the tensor cores (csrc/fredholm_tc.cu; B2_FREDHOLM_TC=1 forces it for every shape) vs the oracle in
-    complex128 / float64: 1e-5 of the largest entry per output column (north_star tolerance for complex64)"""
-    monkeypatch.setenv("B2_FREDHOLM_TC", "1")
-    monkeypatch.setenv("B2_FREDHOLM_MODE", mode)
+def test_fredholm1_tensor_core_path(pm, monkeypatch, shape, dtype):
+    """MPIFredholm1 on the tensor cores (csrc/fredholm_tc.cu; TC_MIN_PRODUCTS = 0 puts every shape there) vs the oracle
+    in complex128 / float64: 1e-5 of the largest entry per output column (north_star tolerance for complex64)"""
+    monkeypatch.setattr(pm.signalprocessing.Fredholm1, "TC_MIN_PRODUCTS", 0)
     nsl, nx, ny, nz = shape
     rng = np.random.default_rng(13)
     G = rng.standard_normal((nsl, nx, ny))
@@ -624,7 +622,7 @@ def test_fredholm1_tensor_core_path(pm, monkeypatch, mode, shape, dtype):
 
 def test_fredholm1_kat_on_tensor_cores(pm, monkeypatch):
     """tests/test_fredholm.py:36-95 arange KAT through the tensor-core path (exactly representable inputs)"""
-    monkeypatch.setenv("B2_FREDHOLM_TC", "1")
+    monkeypatch.setattr(pm.signalprocessing.Fredholm1, "TC_MIN_PRODUCTS", 0)
     for nz in (5, 1):
         for dtype in (np.float32, np.complex64):
             cx = dtype is np.complex64
