@@ -204,6 +204,24 @@ int b2_convolve_axis(b2_ctx* ctx, const void* x, void* y, size_t n_outer, size_t
  * error codes as b2_convolve_axis, plus B2_ERR_ARG for any other kind; y is untouched on every error */
 int b2_poststack_axis(b2_ctx* ctx, const void* x, void* y, size_t n_outer, size_t n_axis, size_t n_inner,
                       const void* h, int nh, int offset, int kind, int adjoint, int dtype, void* stream);
+/* rank-local NON-STATIONARY 1-D convolution along the MIDDLE axis of the same block: pylops.signalprocessing.
+ * NonStationaryConvolve1D.  hs is a device array [nfilt][nh] of real filters (the data's real dtype) at the axis
+ * samples oh + dh * f; sample j uses h_j, interpolated linearly between its two neighbouring filters in float64
+ * weights cast to the dtype (two rounded products, one rounded add), the first / last filter outside [oh, oh +
+ * dh * (nfilt - 1)].  Forward y[i] = sum_j h_j[hc + i - j] x[j], adjoint = exact transpose, both summed in ascending
+ * sample order with fma; no atomics, no allocation, repeated applies give identical bits.  dtype F32 / F64 (complex
+ * data: the real dtype and 2 * n_inner).  B2_ERR_ARG: a null pointer, x == y, a zero size, nfilt < 1, nh < 1, hc
+ * outside [0, nh), dh < 1; B2_ERR_DTYPE: another dtype; y is untouched on every error */
+int b2_nsconvolve_axis(b2_ctx* ctx, const void* x, void* y, size_t n_outer, size_t n_axis, size_t n_inner,
+                       const void* hs, int nfilt, int nh, int hc, long long oh, long long dh, int adjoint, int dtype,
+                       void* stream);
+/* the 2-D wavelet branch of pylops.avo.poststack.PoststackLinearModelling: y = C D x with D as in b2_poststack_axis
+ * and C the convolution of b2_nsconvolve_axis; adjoint x = D^T C^T y.  One launch; equals b2_derivative_axis then
+ * b2_nsconvolve_axis (adjoint: the reverse) bit for bit.  Arguments and error codes as b2_nsconvolve_axis, plus
+ * B2_ERR_ARG for a kind other than B2_FD_CENTERED / B2_FD_FORWARD */
+int b2_nspoststack_axis(b2_ctx* ctx, const void* x, void* y, size_t n_outer, size_t n_axis, size_t n_inner,
+                        const void* hs, int nfilt, int nh, int hc, long long oh, long long dh, int kind, int adjoint,
+                        int dtype, void* stream);
 /* rank-local Kirchhoff demigration, spreading / stacking stage: pylops.waveeqprocessing.Kirchhoff (mode="analytic",
  * 2-D or 3-D, dynamic=False) before its wavelet convolution (run that as b2_convolve_axis on the [ns*nr][nt] traces).
  * Tables are float64 device arrays in the kernel's layout: trav_srcs [ns][ni], trav_recs [nr][ni] (a trace reads

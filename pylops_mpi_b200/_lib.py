@@ -63,6 +63,7 @@ def _load():
             "Build it with `python -m pylops_mpi_b200.build` (needs nvcc, sm_90a).")
     lib = C.CDLL(LIB_PATH, mode=C.RTLD_GLOBAL)
     vp, sz, i, d, dp = C.c_void_p, C.c_size_t, C.c_int, C.c_double, C.POINTER(C.c_double)
+    ll = C.c_longlong
     sigs = {
         "b2_version": ([], i),
         "b2_strerror": ([i], C.c_char_p),
@@ -90,6 +91,8 @@ def _load():
         "b2_derivative_axis": ([vp, vp, vp, sz, sz, sz, i, i, i, i, d, i, i, vp], i),
         "b2_convolve_axis": ([vp, vp, vp, sz, sz, sz, vp, i, i, i, i, vp], i),
         "b2_poststack_axis": ([vp, vp, vp, sz, sz, sz, vp, i, i, i, i, i, vp], i),
+        "b2_nsconvolve_axis": ([vp, vp, vp, sz, sz, sz, vp, i, i, i, ll, ll, i, i, vp], i),
+        "b2_nspoststack_axis": ([vp, vp, vp, sz, sz, sz, vp, i, i, i, ll, ll, i, i, i, vp], i),
         "b2_kirchhoff": ([vp, vp, vp, vp, vp, sz, sz, sz, sz, d, i, i, vp], i),
         "b2_kirchhoff_chunk": ([vp, vp, vp, vp, vp, sz, sz, sz, sz, sz, sz, d, i, i, i, vp], i),
         "b2_kirchhoff_tables": ([vp, vp, vp, vp, sz, sz, sz, vp, sz, d, sz, sz, vp, vp], i),

@@ -19,8 +19,9 @@
 //           epilogue applies D^T to e from shared memory.
 // d and D^T e use the stencil kernel's arithmetic (stencil.cu: non-zero taps in ascending offset order, each an fma
 // into an accumulator that starts at 0), and e the same tap chunks as b2_convolve_axis, so the fused operator
-// equals the two-launch chain b2_derivative_axis + b2_convolve_axis bit for bit.
+// equals the two-launch chain b2_derivative_axis + b2_convolve_axis bit for bit (fd_fwd / fd_adj: fd_axis.cuh).
 #include "common.cuh"
+#include "fd_axis.cuh"
 
 namespace {
 
@@ -34,34 +35,6 @@ constexpr int DS_NONE = 0, DS_FWD = 1, DS_ADJ = 2;   // derivative stage: none, 
 // LDS.64 / LDS.128 (Vec16 is only element-aligned: the compiler would split it into conflicting scalar reads)
 template <typename T, int V>
 struct alignas(V * sizeof(T)) VecN { T v[V]; };
-
-// (D x)[j] from x[j-1], x[j], x[j+1] on a line of n samples: 0.5 (x[j+1] - x[j-1]) on [1, n-2] (centered) or
-// x[j+1] - x[j] on [0, n-2] (forward), zero elsewhere
-template <typename T>
-__device__ __forceinline__ T fd_fwd(T xm, T x0, T xp, long long j, long long n, int kind) {
-  T acc = T(0);
-  if (kind == B2_FD_CENTERED) {
-    if (j >= 1 && j <= n - 2) { acc = fma(T(-0.5), xm, acc); acc = fma(T(0.5), xp, acc); }
-  } else if (j >= 0 && j <= n - 2) {
-    acc = fma(T(-1), x0, acc);
-    acc = fma(T(1), xp, acc);
-  }
-  return acc;
-}
-
-// (D^T e)[i] from e[i-1], e[i], e[i+1]: row i of the transpose, whose taps come from the forward rows i-1, i, i+1
-template <typename T>
-__device__ __forceinline__ T fd_adj(T em, T e0, T ep, long long i, long long n, int kind) {
-  T acc = T(0);
-  if (kind == B2_FD_CENTERED) {
-    if (i - 1 >= 1 && i - 1 <= n - 2) acc = fma(T(0.5), em, acc);
-    if (i + 1 >= 1 && i + 1 <= n - 2) acc = fma(T(-0.5), ep, acc);
-  } else {
-    if (i >= 1 && i - 1 <= n - 2) acc = fma(T(1), em, acc);
-    if (i <= n - 2) acc = fma(T(-1), e0, acc);
-  }
-  return acc;
-}
 
 // ---- innermost axis (n_inner == 1) ----------------------------------------------------------------------------
 // A CTA covers L lines x S outputs (S = R * ceil(n / R) capped at the tile, L = tile / S when lines are short).

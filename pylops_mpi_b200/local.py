@@ -330,17 +330,69 @@ class Convolve1D(_AxisOperator):
                                              _lib.code(real), _lib.stream()), "b2_convolve_axis")
 
 
+class NonStationaryConvolve1D(_AxisOperator):
+    """Rank-local non-stationary 1-D convolution along ``axis`` of a C-ordered ``dims`` block,
+    pylops.signalprocessing.NonStationaryConvolve1D (pylops 2.x) inside MPIBlockDiag.  ``hs`` holds ``nfilt`` real
+    filters of odd length ``nh`` at the regularly spaced axis samples ``ih``; sample ``j`` uses ``h_j``, linearly
+    interpolated between the two filters around it (the first / last filter before ``ih[0]`` / after ``ih[-1]``)::
+
+        y[i] = sum_j h_j[nh // 2 + i - j] x[j]
+
+    and the adjoint is the exact transpose.  One b2_nsconvolve_axis launch per apply (csrc/nsconvolve.cu), whose
+    interpolated filters are pylops' bits.  ``ValueError`` for an even ``nh``, irregular or decreasing ``ih``, ``ih``
+    outside ``[0, dims[axis])`` and ``len(ih) != hs.shape[0]``; complex filters are not provided."""
+
+    def __init__(self, dims, hs, ih, axis: int = -1, dtype="float64"):
+        hs = hs.detach().cpu().numpy() if isinstance(hs, torch.Tensor) else np.asarray(hs)
+        if np.iscomplexobj(hs):
+            raise NotImplementedError("complex filters are not supported")
+        if hs.ndim != 2:
+            raise ValueError(f"hs must be a 2-D array of filters (nfilt, nh); got shape {hs.shape}")
+        if hs.shape[1] % 2 == 0:
+            raise ValueError("filters hs must have odd length")
+        ih = np.asarray(ih).ravel()
+        if len(ih) != hs.shape[0]:
+            raise ValueError(f"ih has {len(ih)} indices for {hs.shape[0]} filters")
+        if len(np.unique(np.diff(ih))) > 1:
+            raise ValueError("the indices of filters 'ih' must be regularly sampled")
+        super().__init__(dims, axis, dtype)
+        if min(ih) < 0 or max(ih) >= self.dims[self.axis]:
+            raise ValueError("the indices of filters 'ih' must be larger than 0 and smaller than `dims`")
+        self.nfilt, self.nh = int(hs.shape[0]), int(hs.shape[1])
+        self.hc = self.nh // 2
+        self.oh = int(ih[0])
+        self.dh = int(ih[1] - ih[0]) if self.nfilt > 1 else 1
+        if self.dh < 1:
+            raise ValueError("the indices of filters 'ih' must be increasing")
+        self._hs = _bank(hs)
+
+    def _launch(self, x, y, dt, adjoint):
+        n_outer, n_axis, n_inner, real = self._lines(dt)
+        _lib.check(_lib.lib.b2_nsconvolve_axis(_lib.ctx(), x.data_ptr(), y.data_ptr(), n_outer, n_axis, n_inner,
+                                               self._hs[real].data_ptr(), self.nfilt, self.nh, self.hc, self.oh,
+                                               self.dh, adjoint, _lib.code(real), _lib.stream()), "b2_nsconvolve_axis")
+
+
+def _bank(h):
+    """real taps or a filter bank in both real precisions, uploaded once"""
+    return {t: torch.as_tensor(np.ascontiguousarray(h, dtype=_lib.numpy_dtype(t))).to("cuda")
+            for t in (torch.float32, torch.float64)}
+
+
 class PoststackLinearModelling(Convolve1D):
     """Rank-local post-stack seismic modelling, pylops.avo.poststack.PoststackLinearModelling (pylops 2.x) for a
-    stationary real wavelet, as tutorials/poststack.py uses it inside MPIBlockDiag::
+    real wavelet, as tutorials/poststack.py uses it inside MPIBlockDiag::
 
         PoststackLinearModelling(wav, nt0, spatdims) == Convolve1D(dims, wav, offset=len(wav) // 2, axis=0)
                                                         * FirstDerivative(dims, axis=0, sampling=1.0, kind=kind)
 
-    on ``dims = (nt0,) + spatdims``; the adjoint is ``D^T C^T``.  The operator dtype is ``wav.dtype``; data are
-    promoted and ``out=`` is handled as in :class:`Convolve1D`.  Each apply is ONE b2_poststack_axis launch
-    (csrc/convolve.cu: the derivative is fused into the convolution kernel), equal bit for bit to the two-launch
-    chain.  ``explicit`` / ``sparse`` matrices, non-stationary (2-D) and complex wavelets are not provided."""
+    on ``dims = (nt0,) + spatdims``; the adjoint is ``D^T C^T``.  A 2-D wavelet of shape ``(nt0, nwav)`` holds one
+    wavelet per time sample (non-stationary): ``C[i, j] = wav[j, nwav // 2 + i - j]``, pylops'
+    ``nonstationary_convmtx(wav, nt0, hc=nwav // 2, pad=(nt0, nt0))`` applied matrix-free (any ``nwav``).  The
+    operator dtype is ``wav.dtype``; data are promoted and ``out=`` is handled as in :class:`Convolve1D`.  Each
+    apply is ONE launch with the derivative fused into the convolution kernel (b2_poststack_axis, csrc/convolve.cu;
+    2-D: b2_nspoststack_axis, csrc/nsconvolve.cu), equal bit for bit to the two-launch chain.  ``explicit`` /
+    ``sparse`` matrices, complex wavelets and 2-D wavelets whose first dimension is not ``nt0`` are not provided."""
 
     def __init__(self, wav, nt0: int, spatdims=None, explicit: bool = False, sparse: bool = False,
                  kind: str = "centered"):
@@ -355,12 +407,27 @@ class PoststackLinearModelling(Convolve1D):
             dims = (int(nt0), int(spatdims))
         else:
             dims = (int(nt0),) + tuple(int(d) for d in spatdims)
-        super().__init__(dims, wav, offset=len(wav) // 2, axis=0, dtype=np.result_type(wav.dtype, np.float32))
+        dtype = np.result_type(wav.dtype, np.float32)
+        self.nonstationary = wav.ndim == 2 and wav.shape[0] == int(nt0)
+        if self.nonstationary:
+            if np.iscomplexobj(wav):
+                raise NotImplementedError("complex filters are not supported")
+            _AxisOperator.__init__(self, dims, 0, dtype)
+            self.nh, self.offset, self.method = int(wav.shape[1]), int(wav.shape[1]) // 2, None
+            self._h = _bank(wav)
+        else:
+            super().__init__(dims, wav, offset=len(wav) // 2, axis=0, dtype=dtype)
         self.kind = kind
         self._kind = _lib.FD_CENTERED if kind == "centered" else _lib.FD_FORWARD
 
     def _launch(self, x, y, dt, adjoint):
         n_outer, n_axis, n_inner, real = self._lines(dt)
+        if self.nonstationary:       # the bank of nt0 wavelets at samples 0, 1, ..., nt0 - 1
+            _lib.check(_lib.lib.b2_nspoststack_axis(_lib.ctx(), x.data_ptr(), y.data_ptr(), n_outer, n_axis, n_inner,
+                                                    self._h[real].data_ptr(), self.dims[self.axis], self.nh,
+                                                    self.offset, 0, 1, self._kind, adjoint, _lib.code(real),
+                                                    _lib.stream()), "b2_nspoststack_axis")
+            return
         _lib.check(_lib.lib.b2_poststack_axis(_lib.ctx(), x.data_ptr(), y.data_ptr(), n_outer, n_axis, n_inner,
                                               self._h[real].data_ptr(), self.nh, self.offset, self._kind, adjoint,
                                               _lib.code(real), _lib.stream()), "b2_poststack_axis")
