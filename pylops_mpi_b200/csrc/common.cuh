@@ -52,6 +52,31 @@ static inline size_t b2_dtype_size(int dt) {
 
 static inline bool b2_aligned16(const void* p) { return (((uintptr_t)p) & 15u) == 0; }
 
+// ---- launch scaffold ----
+// launch(first, count) over [0, total) in groups of at most per_launch, where one grid cannot hold them all (gridDim.y
+// holds B2_GRID_Y_MAX outer indices, a 1-D grid 2^31 - 1 blocks); stops at the first launch error
+constexpr size_t B2_GRID_Y_MAX = 65535;
+template <typename F>
+int b2_launch_groups(size_t total, size_t per_launch, F launch) {
+  for (size_t first = 0; first < total; first += per_launch) {
+    launch(first, total - first < per_launch ? total - first : per_launch);
+    B2_LAUNCH_CHECK();
+  }
+  return B2_OK;
+}
+
+// a launch of Kernel with more than the default 48 KB of dynamic shared memory has to be allowed first: done once per
+// kernel, and again only for a larger size
+template <auto Kernel>
+int b2_allow_smem(size_t smem) {
+  static size_t allowed = 48 * 1024;
+  if (smem > allowed) {
+    B2_CUDA(cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    allowed = smem;
+  }
+  return B2_OK;
+}
+
 // ---- streaming 16-byte global loads / stores (read-once data: bypass L1) ----
 __device__ __forceinline__ uint4 ldg_stream16(const void* p) {
   uint4 r;
@@ -87,6 +112,11 @@ struct Vec16<double> {
   static constexpr int N = 2;
   double v[2];
 };
+
+// V consecutive elements, aligned to their size so that shared-memory reads of a whole vector compile to one
+// LDS.64 / LDS.128 (Vec16 is only element-aligned: the compiler would split it into conflicting scalar reads)
+template <typename T, int V>
+struct alignas(V * sizeof(T)) VecN { T v[V]; };
 
 template <typename T>
 __device__ __forceinline__ Vec16<T> load_vec(const T* p) {

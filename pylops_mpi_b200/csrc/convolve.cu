@@ -11,7 +11,7 @@
 // feeds R*R (innermost) or RT*RT*V (middle axis) FMAs.  Tap chunks and taps within a chunk are summed in a fixed
 // order, so repeated applies give identical bits.
 //
-// The same kernel bodies also run pylops.avo.poststack.PoststackLinearModelling, C D with D the first derivative
+// The same kernels also run pylops.avo.poststack.PoststackLinearModelling, C D with D the first derivative
 // along the axis (FirstDerivative, edge=False, sampling=1), through a compile-time derivative stage DS:
 //   DS_FWD  y = C D x: the loader stages x with one extra sample on each side and turns it into d = D x in shared
 //           memory; the correlation then runs unchanged on d.
@@ -29,12 +29,6 @@ constexpr int CV_THREADS = 256;
 constexpr int CV_KC_LINE = 128;              // taps per chunk, innermost axis
 constexpr int CV_KC_MID = 64;                // taps per chunk, middle axis
 constexpr size_t CV_SMEM_BUDGET = 32 * 1024; // bytes of staged windows per CTA (packed short lines)
-constexpr int DS_NONE = 0, DS_FWD = 1, DS_ADJ = 2;   // derivative stage: none, D before C, D^T after C^T
-
-// V consecutive elements, aligned to their size so that shared-memory reads of a whole vector compile to one
-// LDS.64 / LDS.128 (Vec16 is only element-aligned: the compiler would split it into conflicting scalar reads)
-template <typename T, int V>
-struct alignas(V * sizeof(T)) VecN { T v[V]; };
 
 // ---- innermost axis (n_inner == 1) ----------------------------------------------------------------------------
 // A CTA covers L lines x S outputs (S = R * ceil(n / R) capped at the tile, L = tile / S when lines are short).
@@ -57,8 +51,9 @@ __device__ __forceinline__ T tap(const T* __restrict__ h, int k, int nh, int adj
 // (then L == 1) thread 0 computes e[i0 - 1] and the last thread e[i0 + S], with the same tap order as the others,
 // so the 16-byte tile geometry and stores of the plain convolution are kept.
 template <typename T, int DS>
-__device__ __forceinline__ void conv_line(const T* __restrict__ x, T* __restrict__ y, const T* __restrict__ h,
-                                          const LineParams p, const int kind) {
+__global__ void __launch_bounds__(CV_THREADS)
+conv_line_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restrict__ h, const LineParams p,
+                 const int kind) {
   constexpr int R = Vec16<T>::N;
   constexpr int XH = DS == DS_FWD ? 1 : 0;  // extra staged samples on each side of the window
   extern __shared__ __align__(16) unsigned char cv_smem[];
@@ -172,19 +167,6 @@ __device__ __forceinline__ void conv_line(const T* __restrict__ x, T* __restrict
   }
 }
 
-template <typename T>
-__global__ void __launch_bounds__(CV_THREADS)
-conv_line_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restrict__ h, const LineParams p) {
-  conv_line<T, DS_NONE>(x, y, h, p, 0);
-}
-
-template <typename T, int DS>
-__global__ void __launch_bounds__(CV_THREADS)
-poststack_line_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restrict__ h, const LineParams p,
-                      const int kind) {
-  conv_line<T, DS>(x, y, h, p, kind);
-}
-
 // ---- middle axis (n_inner > 1) --------------------------------------------------------------------------------
 // CTA = 16 lanes across n_inner (V columns each) x 16 row groups of RT rows: RB = 64 output rows of COLS columns.
 // The RB + kc input rows the tile needs are staged per tap chunk; consecutive row tiles overlap in L2.
@@ -206,8 +188,9 @@ __device__ __forceinline__ VecN<T, V> ld_vec(const T* p) {
 }
 
 template <typename T, int V, int DS>
-__device__ __forceinline__ void conv_mid(const T* __restrict__ x, T* __restrict__ y, const T* __restrict__ h,
-                                         const MidParams p, const int kind) {
+__global__ void __launch_bounds__(MID_LANES * MID_GROUPS)
+conv_mid_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restrict__ h, const MidParams p,
+                const int kind) {
   constexpr int COLS = MID_LANES * V;
   constexpr int XH = DS == DS_FWD ? 1 : 0;  // extra staged rows on each side of the window
   constexpr int EH = DS == DS_ADJ ? 1 : 0;  // e rows computed on each side of the stored rows
@@ -309,19 +292,6 @@ __device__ __forceinline__ void conv_mid(const T* __restrict__ x, T* __restrict_
   }
 }
 
-template <typename T, int V>
-__global__ void __launch_bounds__(MID_LANES * MID_GROUPS)
-conv_mid_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restrict__ h, const MidParams p) {
-  conv_mid<T, V, DS_NONE>(x, y, h, p, 0);
-}
-
-template <typename T, int V, int DS>
-__global__ void __launch_bounds__(MID_LANES * MID_GROUPS)
-poststack_mid_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restrict__ h, const MidParams p,
-                     const int kind) {
-  conv_mid<T, V, DS>(x, y, h, p, kind);
-}
-
 inline int round_up(int v, int m) { return (v + m - 1) / m * m; }
 
 template <typename T, int DS>
@@ -344,18 +314,11 @@ int launch_line(const T* x, T* y, const T* h, size_t n_lines, size_t n, int nh, 
   p.vec = p.L == 1 && n % R == 0 && b2_aligned16(x);
   const size_t smem = ((size_t)p.kc + (size_t)p.L * per_line) * sizeof(T);
   const size_t max_groups = (size_t)(0x7fffffffLL / p.tiles);
-  const size_t lines_per_launch = (max_groups / p.L) * p.L;
-  for (size_t done = 0; done < n_lines; done += lines_per_launch) {
-    const size_t cnt = n_lines - done < lines_per_launch ? n_lines - done : lines_per_launch;
+  return b2_launch_groups(n_lines, (max_groups / p.L) * p.L, [&](size_t first, size_t cnt) {
     p.nlines = (long long)cnt;
     const size_t blocks = (cnt + p.L - 1) / p.L * (size_t)p.tiles;
-    if constexpr (DS == DS_NONE)
-      conv_line_kernel<T><<<(unsigned)blocks, CV_THREADS, smem, st>>>(x + done * n, y + done * n, h, p);
-    else
-      poststack_line_kernel<T, DS><<<(unsigned)blocks, CV_THREADS, smem, st>>>(x + done * n, y + done * n, h, p, kind);
-    B2_LAUNCH_CHECK();
-  }
-  return B2_OK;
+    conv_line_kernel<T, DS><<<(unsigned)blocks, CV_THREADS, smem, st>>>(x + first * n, y + first * n, h, p, kind);
+  });
 }
 
 template <typename T, int V, int DS>
@@ -374,27 +337,13 @@ int launch_mid_v(const T* x, T* y, const T* h, size_t n_outer, size_t n, size_t 
   if (nblk > 0x7fffffffLL) return B2_ERR_ARG;
   const size_t rows = (size_t)(MID_RB + p.kc) + (DS == DS_FWD ? MID_RB + p.kc + 2 : 0);   // DS_FWD: + rows of x
   const size_t smem = (size_t)p.kc * sizeof(T) + rows * MID_LANES * V * sizeof(T);
-  if constexpr (DS != DS_NONE) {
-    // DS_FWD with kc > 20 taps needs more than the default 48 KB (set once, before the first such launch)
-    static size_t smem_opt_in = 48 * 1024;
-    if (smem > smem_opt_in) {
-      const cudaError_t e = cudaFuncSetAttribute(poststack_mid_kernel<T, V, DS>,
-                                                 cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-      if (e != cudaSuccess) return (int)e;
-      smem_opt_in = smem;
-    }
-  }
-  const dim3 block(MID_LANES, MID_GROUPS);
-  for (size_t done = 0; done < n_outer; done += 65535) {
-    const unsigned cnt = (unsigned)(n_outer - done < 65535 ? n_outer - done : 65535);
-    const size_t o = done * n * ni;
-    if constexpr (DS == DS_NONE)
-      conv_mid_kernel<T, V><<<dim3((unsigned)nblk, cnt), block, smem, st>>>(x + o, y + o, h, p);
-    else
-      poststack_mid_kernel<T, V, DS><<<dim3((unsigned)nblk, cnt), block, smem, st>>>(x + o, y + o, h, p, kind);
-    B2_LAUNCH_CHECK();
-  }
-  return B2_OK;
+  const int rc = b2_allow_smem<conv_mid_kernel<T, V, DS>>(smem);   // DS_FWD with kc > 20 taps needs more than 48 KB
+  if (rc != B2_OK) return rc;
+  return b2_launch_groups(n_outer, B2_GRID_Y_MAX, [&](size_t first, size_t cnt) {
+    const size_t o = first * n * ni;
+    conv_mid_kernel<T, V, DS><<<dim3((unsigned)nblk, (unsigned)cnt), dim3(MID_LANES, MID_GROUPS), smem, st>>>(
+        x + o, y + o, h, p, kind);
+  });
 }
 
 template <typename T, int DS>
@@ -411,35 +360,29 @@ int launch_conv(const void* xv, void* yv, const void* hv, size_t n_outer, size_t
   return launch_mid_v<T, 1, DS>(x, y, h, n_outer, n, ni, nh, off, adjoint, kind, st);
 }
 
-template <typename T>
-int launch_poststack(const void* x, void* y, const void* h, size_t n_outer, size_t n, size_t ni, int nh, int off,
-                     int kind, int adjoint, cudaStream_t st) {
-  return adjoint ? launch_conv<T, DS_ADJ>(x, y, h, n_outer, n, ni, nh, off, 1, kind, st)
-                 : launch_conv<T, DS_FWD>(x, y, h, n_outer, n, ni, nh, off, 0, kind, st);
+// Both entry points.  Callers see the order of the checks: a bad kind wins over a bad dtype, and an empty block is
+// B2_OK without a launch (and before x and y are looked at)
+int conv_axis(b2_ctx* ctx, const void* x, void* y, size_t n_outer, size_t n_axis, size_t n_inner, const void* h,
+              int nh, int offset, bool fused, int kind, int adjoint, int dtype, void* stream) {
+  if (!ctx || nh < 1 || offset < 0 || offset > nh - 1 || !h) return B2_ERR_ARG;
+  if (fused && kind != B2_FD_CENTERED && kind != B2_FD_FORWARD) return B2_ERR_ARG;
+  if (dtype != B2_F32 && dtype != B2_F64) return B2_ERR_DTYPE;
+  if (n_outer == 0 || n_axis == 0 || n_inner == 0) return B2_OK;
+  if (!x || !y || x == y) return B2_ERR_ARG;
+  return ds_dispatch(dtype, fused, adjoint, [&](auto t, auto ds) {
+    return launch_conv<decltype(t), decltype(ds)::value>(x, y, h, n_outer, n_axis, n_inner, nh, offset,
+                                                         adjoint ? 1 : 0, kind, (cudaStream_t)stream);
+  });
 }
 
 }  // namespace
 
 extern "C" int b2_convolve_axis(b2_ctx* ctx, const void* x, void* y, size_t n_outer, size_t n_axis, size_t n_inner,
                                 const void* h, int nh, int offset, int adjoint, int dtype, void* stream) {
-  if (!ctx || nh < 1 || offset < 0 || offset > nh - 1 || !h) return B2_ERR_ARG;
-  if (dtype != B2_F32 && dtype != B2_F64) return B2_ERR_DTYPE;
-  if (n_outer == 0 || n_axis == 0 || n_inner == 0) return B2_OK;
-  if (!x || !y || x == y) return B2_ERR_ARG;
-  cudaStream_t st = (cudaStream_t)stream;
-  return dtype == B2_F32
-             ? launch_conv<float, DS_NONE>(x, y, h, n_outer, n_axis, n_inner, nh, offset, adjoint, 0, st)
-             : launch_conv<double, DS_NONE>(x, y, h, n_outer, n_axis, n_inner, nh, offset, adjoint, 0, st);
+  return conv_axis(ctx, x, y, n_outer, n_axis, n_inner, h, nh, offset, false, 0, adjoint, dtype, stream);
 }
 
 extern "C" int b2_poststack_axis(b2_ctx* ctx, const void* x, void* y, size_t n_outer, size_t n_axis, size_t n_inner,
                                  const void* h, int nh, int offset, int kind, int adjoint, int dtype, void* stream) {
-  if (!ctx || nh < 1 || offset < 0 || offset > nh - 1 || !h) return B2_ERR_ARG;
-  if (kind != B2_FD_CENTERED && kind != B2_FD_FORWARD) return B2_ERR_ARG;
-  if (dtype != B2_F32 && dtype != B2_F64) return B2_ERR_DTYPE;
-  if (n_outer == 0 || n_axis == 0 || n_inner == 0) return B2_OK;
-  if (!x || !y || x == y) return B2_ERR_ARG;
-  cudaStream_t st = (cudaStream_t)stream;
-  return dtype == B2_F32 ? launch_poststack<float>(x, y, h, n_outer, n_axis, n_inner, nh, offset, kind, adjoint, st)
-                         : launch_poststack<double>(x, y, h, n_outer, n_axis, n_inner, nh, offset, kind, adjoint, st);
+  return conv_axis(ctx, x, y, n_outer, n_axis, n_inner, h, nh, offset, true, kind, adjoint, dtype, stream);
 }

@@ -35,11 +35,7 @@ constexpr int NS_RT = 8;                       // rows per thread
 constexpr int NS_RB = NS_GROUPS * NS_RT;       // rows per CTA
 constexpr int NS_WS = NS_LANES + 1;            // shared row stride of the windows (transposed staging is conflict-free)
 constexpr int NS_KC = 48;                      // taps per chunk (a multiple of NS_RT)
-constexpr int DS_NONE = 0, DS_FWD = 1, DS_ADJ = 2;
 constexpr int LAY_MID = 0, LAY_LINE = 1;       // columns of n_inner / whole lines (n_inner == 1)
-
-template <typename T, int V>
-struct alignas(V * sizeof(T)) VecN { T v[V]; };
 
 struct NsParams {
   long long n;         // axis length
@@ -231,27 +227,19 @@ int launch_lay(const T* x, T* y, const T* hs, size_t n_outer, size_t n, size_t n
   const size_t rows = (size_t)NS_RB + p.kc;
   const size_t smem = (size_t)p.kc * NS_RB * sizeof(T) + rows * sizeof(RowW<T>) +
                       (rows + (DS == DS_FWD ? rows + 2 : 0)) * NS_WS * sizeof(T);
-  static size_t smem_opt_in = 48 * 1024;          // set once per instantiation, before the first larger launch
-  if (smem > smem_opt_in) {
-    const cudaError_t e = cudaFuncSetAttribute(nsconv_kernel<T, LAY, DS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                               (int)smem);
-    if (e != cudaSuccess) return (int)e;
-    smem_opt_in = smem;
-  }
+  const int rc = b2_allow_smem<nsconv_kernel<T, LAY, DS>>(smem);
+  if (rc != B2_OK) return rc;
   if constexpr (LAY == LAY_LINE) {
     // columns are whole lines: launch groups of lines so that the grid stays within 2^31 - 1 blocks
     p.sa = 1;
     p.sc = (long long)n;
     p.plane = 0;
-    const size_t max_lines = (size_t)(0x7fffffffLL / p.rtiles) * NS_LANES;
-    for (size_t done = 0; done < n_outer; done += max_lines) {
-      const size_t cnt = n_outer - done < max_lines ? n_outer - done : max_lines;
+    return b2_launch_groups(n_outer, (size_t)(0x7fffffffLL / p.rtiles) * NS_LANES, [&](size_t first, size_t cnt) {
       p.ncols = (long long)cnt;
       p.ctiles = (long long)((cnt + NS_LANES - 1) / NS_LANES);
       nsconv_kernel<T, LAY, DS><<<(unsigned)(p.ctiles * p.rtiles), NS_THREADS, smem, st>>>(
-          x + done * n, y + done * n, hs, p, adjoint, kind);
-      B2_LAUNCH_CHECK();
-    }
+          x + first * n, y + first * n, hs, p, adjoint, kind);
+    });
   } else {
     p.sa = (long long)ni;
     p.sc = 1;
@@ -260,15 +248,12 @@ int launch_lay(const T* x, T* y, const T* hs, size_t n_outer, size_t n, size_t n
     p.ctiles = (long long)((ni + NS_LANES - 1) / NS_LANES);
     const long long nblk = p.ctiles * p.rtiles;
     if (nblk > 0x7fffffffLL) return B2_ERR_ARG;
-    for (size_t done = 0; done < n_outer; done += 65535) {
-      const unsigned cnt = (unsigned)(n_outer - done < 65535 ? n_outer - done : 65535);
-      const size_t o = done * n * ni;
-      nsconv_kernel<T, LAY, DS><<<dim3((unsigned)nblk, cnt), NS_THREADS, smem, st>>>(x + o, y + o, hs, p, adjoint,
-                                                                                   kind);
-      B2_LAUNCH_CHECK();
-    }
+    return b2_launch_groups(n_outer, B2_GRID_Y_MAX, [&](size_t first, size_t cnt) {
+      const size_t o = first * n * ni;
+      nsconv_kernel<T, LAY, DS><<<dim3((unsigned)nblk, (unsigned)cnt), NS_THREADS, smem, st>>>(x + o, y + o, hs, p,
+                                                                                             adjoint, kind);
+    });
   }
-  return B2_OK;
 }
 
 template <typename T, int DS>
@@ -282,12 +267,19 @@ int launch_ns(const void* x, void* y, const void* hs, size_t n_outer, size_t n, 
   return launch_lay<T, LAY_MID, DS>(xt, yt, h, n_outer, n, ni, nfilt, nh, hc, oh, dh, adjoint, kind, st);
 }
 
-int ns_check(b2_ctx* ctx, const void* x, void* y, size_t n_outer, size_t n_axis, size_t n_inner, const void* hs,
-             int nfilt, int nh, int hc, long long dh) {
+// Both entry points.  Unlike convolve.cu's, an empty block is B2_ERR_ARG; a bad kind wins over a bad dtype
+int ns_axis(b2_ctx* ctx, const void* x, void* y, size_t n_outer, size_t n_axis, size_t n_inner, const void* hs,
+            int nfilt, int nh, int hc, long long oh, long long dh, bool fused, int kind, int adjoint, int dtype,
+            void* stream) {
   if (!ctx || !x || !y || !hs || x == y) return B2_ERR_ARG;
   if (n_outer == 0 || n_axis == 0 || n_inner == 0) return B2_ERR_ARG;
   if (nfilt < 1 || nh < 1 || hc < 0 || hc >= nh || dh < 1) return B2_ERR_ARG;
-  return B2_OK;
+  if (fused && kind != B2_FD_CENTERED && kind != B2_FD_FORWARD) return B2_ERR_ARG;
+  if (dtype != B2_F32 && dtype != B2_F64) return B2_ERR_DTYPE;
+  return ds_dispatch(dtype, fused, adjoint, [&](auto t, auto ds) {
+    return launch_ns<decltype(t), decltype(ds)::value>(x, y, hs, n_outer, n_axis, n_inner, nfilt, nh, hc, oh, dh,
+                                                       adjoint ? 1 : 0, kind, (cudaStream_t)stream);
+  });
 }
 
 }  // namespace
@@ -295,27 +287,11 @@ int ns_check(b2_ctx* ctx, const void* x, void* y, size_t n_outer, size_t n_axis,
 extern "C" int b2_nsconvolve_axis(b2_ctx* ctx, const void* x, void* y, size_t n_outer, size_t n_axis, size_t n_inner,
                                   const void* hs, int nfilt, int nh, int hc, long long oh, long long dh, int adjoint,
                                   int dtype, void* stream) {
-  const int rc = ns_check(ctx, x, y, n_outer, n_axis, n_inner, hs, nfilt, nh, hc, dh);
-  if (rc != B2_OK) return rc;
-  if (dtype != B2_F32 && dtype != B2_F64) return B2_ERR_DTYPE;
-  cudaStream_t st = (cudaStream_t)stream;
-  adjoint = adjoint ? 1 : 0;
-  return dtype == B2_F32
-             ? launch_ns<float, DS_NONE>(x, y, hs, n_outer, n_axis, n_inner, nfilt, nh, hc, oh, dh, adjoint, 0, st)
-             : launch_ns<double, DS_NONE>(x, y, hs, n_outer, n_axis, n_inner, nfilt, nh, hc, oh, dh, adjoint, 0, st);
+  return ns_axis(ctx, x, y, n_outer, n_axis, n_inner, hs, nfilt, nh, hc, oh, dh, false, 0, adjoint, dtype, stream);
 }
 
 extern "C" int b2_nspoststack_axis(b2_ctx* ctx, const void* x, void* y, size_t n_outer, size_t n_axis,
                                    size_t n_inner, const void* hs, int nfilt, int nh, int hc, long long oh,
                                    long long dh, int kind, int adjoint, int dtype, void* stream) {
-  const int rc = ns_check(ctx, x, y, n_outer, n_axis, n_inner, hs, nfilt, nh, hc, dh);
-  if (rc != B2_OK) return rc;
-  if (kind != B2_FD_CENTERED && kind != B2_FD_FORWARD) return B2_ERR_ARG;
-  if (dtype != B2_F32 && dtype != B2_F64) return B2_ERR_DTYPE;
-  cudaStream_t st = (cudaStream_t)stream;
-  if (dtype == B2_F32)
-    return adjoint ? launch_ns<float, DS_ADJ>(x, y, hs, n_outer, n_axis, n_inner, nfilt, nh, hc, oh, dh, 1, kind, st)
-                   : launch_ns<float, DS_FWD>(x, y, hs, n_outer, n_axis, n_inner, nfilt, nh, hc, oh, dh, 0, kind, st);
-  return adjoint ? launch_ns<double, DS_ADJ>(x, y, hs, n_outer, n_axis, n_inner, nfilt, nh, hc, oh, dh, 1, kind, st)
-                 : launch_ns<double, DS_FWD>(x, y, hs, n_outer, n_axis, n_inner, nfilt, nh, hc, oh, dh, 0, kind, st);
+  return ns_axis(ctx, x, y, n_outer, n_axis, n_inner, hs, nfilt, nh, hc, oh, dh, true, kind, adjoint, dtype, stream);
 }

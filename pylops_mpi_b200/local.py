@@ -295,6 +295,61 @@ class SecondDerivative(_AxisDerivative):
         super().__init__(dims, axis=axis, sampling=sampling, kind=kind, edge=edge, order=3, dtype=dtype)
 
 
+def _real_filters(h):
+    """``(host array, {real dtype: device copy})`` of real taps or of a bank of real filters, given as a NumPy array
+    or a torch tensor of any real dtype: uploaded once, in both real precisions"""
+    h = h.detach().cpu().numpy() if isinstance(h, torch.Tensor) else np.asarray(h)
+    if np.iscomplexobj(h):
+        raise NotImplementedError("complex filters are not supported")
+    return h, {t: torch.as_tensor(np.ascontiguousarray(h, dtype=_lib.numpy_dtype(t))).to("cuda")
+               for t in (torch.float32, torch.float64)}
+
+
+class _StationaryTaps:
+    """One real filter of ``nh`` taps on the device: ``y[i] = sum_k h[k] x[i + offset - k]`` along the axis of
+    ``lines`` (an axis operator's ``_lines``), optionally fused with the first derivative ``kind`` (``C D``; adjoint
+    ``D^T C^T``).  csrc/convolve.cu."""
+
+    def __init__(self, bank, offset):
+        if bank[torch.float64].dim() != 1:
+            raise NotImplementedError("only stationary (1-D) filters are supported")
+        self.nh, self.offset = bank[torch.float64].numel(), int(offset)
+        if self.nh < 1 or not 0 <= self.offset <= self.nh - 1:
+            raise ValueError(f"offset must be in [0, nh - 1] = [0, {self.nh - 1}], got {offset}")
+        self._bank = bank
+
+    def launch(self, x, y, lines, adjoint, kind=None):
+        n_outer, n_axis, n_inner, real = lines
+        head = (_lib.ctx(), x.data_ptr(), y.data_ptr(), n_outer, n_axis, n_inner, self._bank[real].data_ptr(),
+                self.nh, self.offset)
+        tail = (adjoint, _lib.code(real), _lib.stream())
+        if kind is None:
+            _lib.check(_lib.lib.b2_convolve_axis(*head, *tail), "b2_convolve_axis")
+        else:
+            _lib.check(_lib.lib.b2_poststack_axis(*head, kind, *tail), "b2_poststack_axis")
+
+
+class _FilterBank:
+    """``nfilt`` real filters of ``nh`` taps (centre ``hc``) at the axis samples ``oh, oh + dh, ...`` on the device:
+    ``y[i] = sum_j h_j[hc + i - j] x[j]`` with ``h_j`` interpolated between the filters around sample ``j``,
+    optionally fused with the first derivative ``kind``, as :class:`_StationaryTaps`.  csrc/nsconvolve.cu."""
+
+    def __init__(self, bank, hc, oh, dh):
+        self.nfilt, self.nh = (int(n) for n in bank[torch.float64].shape)
+        self.hc, self.oh, self.dh = int(hc), int(oh), int(dh)
+        self._bank = bank
+
+    def launch(self, x, y, lines, adjoint, kind=None):
+        n_outer, n_axis, n_inner, real = lines
+        head = (_lib.ctx(), x.data_ptr(), y.data_ptr(), n_outer, n_axis, n_inner, self._bank[real].data_ptr(),
+                self.nfilt, self.nh, self.hc, self.oh, self.dh)
+        tail = (adjoint, _lib.code(real), _lib.stream())
+        if kind is None:
+            _lib.check(_lib.lib.b2_nsconvolve_axis(*head, *tail), "b2_nsconvolve_axis")
+        else:
+            _lib.check(_lib.lib.b2_nspoststack_axis(*head, kind, *tail), "b2_nspoststack_axis")
+
+
 class Convolve1D(_AxisOperator):
     """Rank-local 1-D convolution along ``axis`` of a C-ordered ``dims`` block with a stationary real filter ``h``:
     the role of pylops.signalprocessing.Convolve1D inside MPIBlockDiag (tutorials/reflectivity.py:74-76).  For each
@@ -309,25 +364,12 @@ class Convolve1D(_AxisOperator):
     def __init__(self, dims, h, offset: int = 0, axis: int = -1, method=None, dtype="float64"):
         if method not in (None, "direct", "fft"):
             raise ValueError("method must be None, 'direct' or 'fft'")
-        h = h.detach().cpu().numpy() if isinstance(h, torch.Tensor) else np.asarray(h)
-        if np.iscomplexobj(h):
-            raise NotImplementedError("complex filters are not supported")
-        if h.ndim != 1:
-            raise NotImplementedError("only stationary (1-D) filters are supported")
-        self.nh = int(h.size)
-        self.offset = int(offset)
-        if self.nh < 1 or not 0 <= self.offset <= self.nh - 1:
-            raise ValueError(f"offset must be in [0, nh - 1] = [0, {self.nh - 1}], got {offset}")
+        self._conv = _StationaryTaps(_real_filters(h)[1], offset)
         super().__init__(dims, axis, dtype)
-        self.method = method
-        # taps in both real precisions, uploaded once
-        self._h = {t: torch.as_tensor(h.astype(_lib.numpy_dtype(t))).to("cuda") for t in (torch.float32, torch.float64)}
+        self.nh, self.offset, self.method = self._conv.nh, self._conv.offset, method
 
     def _launch(self, x, y, dt, adjoint):
-        n_outer, n_axis, n_inner, real = self._lines(dt)
-        _lib.check(_lib.lib.b2_convolve_axis(_lib.ctx(), x.data_ptr(), y.data_ptr(), n_outer, n_axis, n_inner,
-                                             self._h[real].data_ptr(), self.nh, self.offset, adjoint,
-                                             _lib.code(real), _lib.stream()), "b2_convolve_axis")
+        self._conv.launch(x, y, self._lines(dt), adjoint)
 
 
 class NonStationaryConvolve1D(_AxisOperator):
@@ -343,9 +385,7 @@ class NonStationaryConvolve1D(_AxisOperator):
     outside ``[0, dims[axis])`` and ``len(ih) != hs.shape[0]``; complex filters are not provided."""
 
     def __init__(self, dims, hs, ih, axis: int = -1, dtype="float64"):
-        hs = hs.detach().cpu().numpy() if isinstance(hs, torch.Tensor) else np.asarray(hs)
-        if np.iscomplexobj(hs):
-            raise NotImplementedError("complex filters are not supported")
+        hs, bank = _real_filters(hs)
         if hs.ndim != 2:
             raise ValueError(f"hs must be a 2-D array of filters (nfilt, nh); got shape {hs.shape}")
         if hs.shape[1] % 2 == 0:
@@ -358,28 +398,17 @@ class NonStationaryConvolve1D(_AxisOperator):
         super().__init__(dims, axis, dtype)
         if min(ih) < 0 or max(ih) >= self.dims[self.axis]:
             raise ValueError("the indices of filters 'ih' must be larger than 0 and smaller than `dims`")
-        self.nfilt, self.nh = int(hs.shape[0]), int(hs.shape[1])
-        self.hc = self.nh // 2
-        self.oh = int(ih[0])
-        self.dh = int(ih[1] - ih[0]) if self.nfilt > 1 else 1
-        if self.dh < 1:
+        dh = int(ih[1] - ih[0]) if len(ih) > 1 else 1
+        if dh < 1:
             raise ValueError("the indices of filters 'ih' must be increasing")
-        self._hs = _bank(hs)
+        self._conv = c = _FilterBank(bank, hs.shape[1] // 2, ih[0], dh)
+        self.nfilt, self.nh, self.hc, self.oh, self.dh = c.nfilt, c.nh, c.hc, c.oh, c.dh
 
     def _launch(self, x, y, dt, adjoint):
-        n_outer, n_axis, n_inner, real = self._lines(dt)
-        _lib.check(_lib.lib.b2_nsconvolve_axis(_lib.ctx(), x.data_ptr(), y.data_ptr(), n_outer, n_axis, n_inner,
-                                               self._hs[real].data_ptr(), self.nfilt, self.nh, self.hc, self.oh,
-                                               self.dh, adjoint, _lib.code(real), _lib.stream()), "b2_nsconvolve_axis")
+        self._conv.launch(x, y, self._lines(dt), adjoint)
 
 
-def _bank(h):
-    """real taps or a filter bank in both real precisions, uploaded once"""
-    return {t: torch.as_tensor(np.ascontiguousarray(h, dtype=_lib.numpy_dtype(t))).to("cuda")
-            for t in (torch.float32, torch.float64)}
-
-
-class PoststackLinearModelling(Convolve1D):
+class PoststackLinearModelling(_AxisOperator):
     """Rank-local post-stack seismic modelling, pylops.avo.poststack.PoststackLinearModelling (pylops 2.x) for a
     real wavelet, as tutorials/poststack.py uses it inside MPIBlockDiag::
 
@@ -400,37 +429,25 @@ class PoststackLinearModelling(Convolve1D):
             raise NotImplementedError("explicit / sparse matrices are not provided: use the matrix-free operator")
         if kind not in ("forward", "centered"):
             raise NotImplementedError(f"{kind} not an available derivative kind...")
-        wav = wav.detach().cpu().numpy() if isinstance(wav, torch.Tensor) else np.asarray(wav)
+        wav, bank = _real_filters(wav)
         if spatdims is None:
             dims = (int(nt0),)
         elif np.ndim(spatdims) == 0:
             dims = (int(nt0), int(spatdims))
         else:
             dims = (int(nt0),) + tuple(int(d) for d in spatdims)
-        dtype = np.result_type(wav.dtype, np.float32)
         self.nonstationary = wav.ndim == 2 and wav.shape[0] == int(nt0)
-        if self.nonstationary:
-            if np.iscomplexobj(wav):
-                raise NotImplementedError("complex filters are not supported")
-            _AxisOperator.__init__(self, dims, 0, dtype)
-            self.nh, self.offset, self.method = int(wav.shape[1]), int(wav.shape[1]) // 2, None
-            self._h = _bank(wav)
+        if self.nonstationary:       # the bank of nt0 wavelets at samples 0, 1, ..., nt0 - 1
+            self._conv = _FilterBank(bank, wav.shape[1] // 2, 0, 1)
         else:
-            super().__init__(dims, wav, offset=len(wav) // 2, axis=0, dtype=dtype)
+            self._conv = _StationaryTaps(bank, len(wav) // 2)
+        super().__init__(dims, 0, np.result_type(wav.dtype, np.float32))
+        self.nh, self.offset = self._conv.nh, self._conv.nh // 2
         self.kind = kind
         self._kind = _lib.FD_CENTERED if kind == "centered" else _lib.FD_FORWARD
 
     def _launch(self, x, y, dt, adjoint):
-        n_outer, n_axis, n_inner, real = self._lines(dt)
-        if self.nonstationary:       # the bank of nt0 wavelets at samples 0, 1, ..., nt0 - 1
-            _lib.check(_lib.lib.b2_nspoststack_axis(_lib.ctx(), x.data_ptr(), y.data_ptr(), n_outer, n_axis, n_inner,
-                                                    self._h[real].data_ptr(), self.dims[self.axis], self.nh,
-                                                    self.offset, 0, 1, self._kind, adjoint, _lib.code(real),
-                                                    _lib.stream()), "b2_nspoststack_axis")
-            return
-        _lib.check(_lib.lib.b2_poststack_axis(_lib.ctx(), x.data_ptr(), y.data_ptr(), n_outer, n_axis, n_inner,
-                                              self._h[real].data_ptr(), self.nh, self.offset, self._kind, adjoint,
-                                              _lib.code(real), _lib.stream()), "b2_poststack_axis")
+        self._conv.launch(x, y, self._lines(dt), adjoint, self._kind)
 
 
 class Transpose(LocalOperator):
@@ -571,9 +588,7 @@ class Kirchhoff(_KernelOperator):
                 f"Kirchhoff: y={'None' if y is None else 'given'} needs srcs and recs of shape ({nd}, n) with rows "
                 f"{'(x, z)' if y is None else '(y, x, z)'} (y=None: 2-D, shape (2, n); y given: 3-D, shape "
                 f"(3, n)); got srcs {srcs.shape}, recs {recs.shape}")
-        wav = wav.detach().cpu().numpy() if isinstance(wav, torch.Tensor) else np.asarray(wav)
-        if np.iscomplexobj(wav) or wav.ndim != 1:
-            raise NotImplementedError("Kirchhoff: only a real 1-D wavelet is supported")
+        self._wav = _StationaryTaps(_real_filters(wav)[1], wavcenter)   # a real 1-D wavelet, or NotImplementedError
         self.mode = mode
         self.ny = 1 if y is None else np.asarray(y).size
         self.nx, self.nz, self.nt = x.size, z.size, t.size
@@ -600,7 +615,6 @@ class Kirchhoff(_KernelOperator):
             else:
                 self._eikonal(y, x, z, srcs, recs, vel, table_bytes)
             self._nc, self.chunked = self.ni, False
-        self.cop = Convolve1D((self.ns * self.nr, self.nt), wav, offset=int(wavcenter), axis=1, dtype=self.dtype)
         self._ws = {self._tdtype: torch.empty(self.shape[0], dtype=self._tdtype, device="cuda")}
 
     @staticmethod
@@ -724,12 +738,13 @@ class Kirchhoff(_KernelOperator):
         ws = self._ws.get(dt)
         if ws is None:                          # data of the other precision: one more workspace, kept
             ws = self._ws[dt] = torch.empty(self.shape[0], dtype=dt, device="cuda")
+        traces = (self.ns * self.nr, self.nt, 1, dt)      # the wavelet runs along time
         if adjoint:
-            self.cop._launch(x, ws, dt, 1)
+            self._wav.launch(x, ws, traces, 1)
             self._kirch(ws, y, dt, 1)
         else:
             self._kirch(x, ws, dt, 0)
-            self.cop._launch(ws, y, dt, 0)
+            self._wav.launch(ws, y, traces, 0)
 
 
 class LSM:
