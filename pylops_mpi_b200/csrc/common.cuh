@@ -5,6 +5,7 @@
 #include <math.h>
 #include <stdint.h>
 #include <stddef.h>
+#include <type_traits>
 #include "../../include/b200lops.h"
 
 #define B2_CUDA(call)                                  \
@@ -51,6 +52,62 @@ static inline size_t b2_dtype_size(int dt) {
 }
 
 static inline bool b2_aligned16(const void* p) { return (((uintptr_t)p) & 15u) == 0; }
+
+// ---- element types and dtype dispatch ----
+// A complex element: two R, aligned as R (the float2 / double2 of b2_pair_t are the aligned pair for one 8- / 16-byte
+// access).  Complex data can also be handed to a real kernel as 2 n interleaved b2_real_t.
+template <typename R>
+struct b2_cx { R re, im; };
+template <typename R>
+using b2_pair_t = typename std::conditional<sizeof(R) == 4, float2, double2>::type;
+
+template <typename T>
+struct b2_real { using type = T; };
+template <typename R>
+struct b2_real<b2_cx<R>> { using type = R; };
+template <typename T>
+using b2_real_t = typename b2_real<T>::type;
+template <typename T>
+constexpr bool b2_is_cx_v = false;
+template <typename R>
+constexpr bool b2_is_cx_v<b2_cx<R>> = true;
+
+template <typename R>
+__device__ __forceinline__ b2_cx<R> b2_cx_conj(b2_cx<R> a) { return {a.re, -a.im}; }
+template <typename R>
+__device__ __forceinline__ b2_cx<R> b2_cx_add(b2_cx<R> a, b2_cx<R> b) { return {a.re + b.re, a.im + b.im}; }
+// acc += a x as two explicit fma chains (the products' rounding is fixed: the dense products rely on it)
+template <typename R>
+__device__ __forceinline__ void b2_cx_fma(b2_cx<R>& acc, b2_cx<R> a, b2_cx<R> x) {
+  acc.re = fma(a.re, x.re, fma(-a.im, x.im, acc.re));
+  acc.im = fma(a.re, x.im, fma(a.im, x.re, acc.im));
+}
+// a b as the plain expression, which the compiler may contract (it rounds differently from b2_cx_fma)
+template <typename R>
+__device__ __forceinline__ b2_cx<R> b2_cx_mul(b2_cx<R> a, b2_cx<R> b) {
+  return {a.re * b.re - a.im * b.im, a.re * b.im + a.im * b.re};
+}
+
+// f(T()) with T the element type of dtype: float, double, b2_cx<float> or b2_cx<double>; B2_ERR_DTYPE for any other
+template <typename F>
+int b2_dispatch(int dtype, F f) {
+  switch (dtype) {
+    case B2_F32: return f(float());
+    case B2_F64: return f(double());
+    case B2_C64: return f(b2_cx<float>());
+    case B2_C128: return f(b2_cx<double>());
+    default: return B2_ERR_DTYPE;
+  }
+}
+// the same for the real-only kernels (no complex instantiation is compiled into them)
+template <typename F>
+int b2_dispatch_real(int dtype, F f) {
+  switch (dtype) {
+    case B2_F32: return f(float());
+    case B2_F64: return f(double());
+    default: return B2_ERR_DTYPE;
+  }
+}
 
 // ---- launch scaffold ----
 // launch(first, count) over [0, total) in groups of at most per_launch, where one grid cannot hold them all (gridDim.y

@@ -66,25 +66,16 @@ lincomb_scalar_kernel(T* out, const T* x, const T* y, double a_scale, double b_s
 }
 
 // ---- complex path (complex coefficients and/or conj) ----------------------
-template <typename R>
-struct Cx {
-  R re, im;
-};
-template <typename R>
-__device__ __forceinline__ Cx<R> cmul(Cx<R> a, Cx<R> b) {
-  return {a.re * b.re - a.im * b.im, a.re * b.im + a.im * b.re};
-}
-
 template <typename R, bool HAS_Y, bool CONJ>
 __global__ void __launch_bounds__(EW_THREADS)
-lincomb_cx_kernel(Cx<R>* out, const Cx<R>* x, const Cx<R>* y, Cx<R> a, Cx<R> b, size_t n) {
+lincomb_cx_kernel(b2_cx<R>* out, const b2_cx<R>* x, const b2_cx<R>* y, b2_cx<R> a, b2_cx<R> b, size_t n) {
   const size_t stride = (size_t)gridDim.x * EW_THREADS;
   for (size_t i = (size_t)blockIdx.x * EW_THREADS + threadIdx.x; i < n; i += stride) {
-    Cx<R> xv = x[i];
+    b2_cx<R> xv = x[i];
     if (CONJ) xv.im = -xv.im;
-    Cx<R> o = cmul(a, xv);
+    b2_cx<R> o = b2_cx_mul(a, xv);
     if (HAS_Y) {
-      Cx<R> t = cmul(b, y[i]);
+      b2_cx<R> t = b2_cx_mul(b, y[i]);
       o.re += t.re;
       o.im += t.im;
     }
@@ -101,12 +92,12 @@ mul_real_kernel(T* out, const T* x, const T* y, size_t n) {
 }
 template <typename R, bool CONJ>
 __global__ void __launch_bounds__(EW_THREADS)
-mul_cx_kernel(Cx<R>* out, const Cx<R>* x, const Cx<R>* y, size_t n) {
+mul_cx_kernel(b2_cx<R>* out, const b2_cx<R>* x, const b2_cx<R>* y, size_t n) {
   const size_t stride = (size_t)gridDim.x * EW_THREADS;
   for (size_t i = (size_t)blockIdx.x * EW_THREADS + threadIdx.x; i < n; i += stride) {
-    Cx<R> xv = x[i];
+    b2_cx<R> xv = x[i];
     if (CONJ) xv.im = -xv.im;
-    out[i] = cmul(xv, y[i]);
+    out[i] = b2_cx_mul(xv, y[i]);
   }
 }
 
@@ -152,10 +143,10 @@ int lincomb_cx(b2_ctx* ctx, void* out, const void* x, const void* y, const doubl
                const double b[2], size_t n, int conj_x, cudaStream_t st) {
   if (n == 0) return B2_OK;
   int grid = ew_grid(ctx, n);
-  Cx<R> ca{(R)a[0], (R)a[1]}, cb{(R)(b ? b[0] : 0.0), (R)(b ? b[1] : 0.0)};
-  auto o = (Cx<R>*)out;
-  auto xx = (const Cx<R>*)x;
-  auto yy = (const Cx<R>*)y;
+  b2_cx<R> ca{(R)a[0], (R)a[1]}, cb{(R)(b ? b[0] : 0.0), (R)(b ? b[1] : 0.0)};
+  auto o = (b2_cx<R>*)out;
+  auto xx = (const b2_cx<R>*)x;
+  auto yy = (const b2_cx<R>*)y;
   if (y) {
     if (conj_x) lincomb_cx_kernel<R, true, true><<<grid, EW_THREADS, 0, st>>>(o, xx, yy, ca, cb, n);
     else lincomb_cx_kernel<R, true, false><<<grid, EW_THREADS, 0, st>>>(o, xx, yy, ca, cb, n);
@@ -177,22 +168,16 @@ extern "C" int b2_lincomb(b2_ctx* ctx, void* out, const double a[2], const void*
   const double bz[2] = {0.0, 0.0};
   if (!b) b = bz;
   const bool real_coef = (a[1] == 0.0) && (!y || b[1] == 0.0);
-  switch (dtype) {
-    case B2_F32:
-      return lincomb_real<float>(ctx, (float*)out, (const float*)x, (const float*)y, a[0], b[0], nullptr, nullptr, n, st);
-    case B2_F64:
-      return lincomb_real<double>(ctx, (double*)out, (const double*)x, (const double*)y, a[0], b[0], nullptr, nullptr, n, st);
-    case B2_C64:
-      if (real_coef && !conj_x)
-        return lincomb_real<float>(ctx, (float*)out, (const float*)x, (const float*)y, a[0], b[0], nullptr, nullptr, 2 * n, st);
-      return lincomb_cx<float>(ctx, out, x, y, a, b, n, conj_x, st);
-    case B2_C128:
-      if (real_coef && !conj_x)
-        return lincomb_real<double>(ctx, (double*)out, (const double*)x, (const double*)y, a[0], b[0], nullptr, nullptr, 2 * n, st);
-      return lincomb_cx<double>(ctx, out, x, y, a, b, n, conj_x, st);
-    default:
-      return B2_ERR_DTYPE;
-  }
+  return b2_dispatch(dtype, [&](auto t) {
+    using T = decltype(t);
+    using R = b2_real_t<T>;
+    // complex data with real coefficients and no conj: the real kernel on 2 n reals
+    if constexpr (b2_is_cx_v<T>) {
+      if (!real_coef || conj_x) return lincomb_cx<R>(ctx, out, x, y, a, b, n, conj_x, st);
+    }
+    return lincomb_real<R>(ctx, (R*)out, (const R*)x, (const R*)y, a[0], b[0], nullptr, nullptr,
+                           b2_is_cx_v<T> ? 2 * n : n, st);
+  });
 }
 
 extern "C" int b2_lincomb_dev(b2_ctx* ctx, void* out, const double* a_dev, double a_scale,
@@ -200,18 +185,12 @@ extern "C" int b2_lincomb_dev(b2_ctx* ctx, void* out, const double* a_dev, doubl
                               size_t n, int dtype, void* stream) {
   if (!ctx || !out || !x) return B2_ERR_ARG;
   cudaStream_t st = (cudaStream_t)stream;
-  switch (dtype) {
-    case B2_F32:
-      return lincomb_real<float>(ctx, (float*)out, (const float*)x, (const float*)y, a_scale, b_scale, a_dev, b_dev, n, st);
-    case B2_F64:
-      return lincomb_real<double>(ctx, (double*)out, (const double*)x, (const double*)y, a_scale, b_scale, a_dev, b_dev, n, st);
-    case B2_C64:
-      return lincomb_real<float>(ctx, (float*)out, (const float*)x, (const float*)y, a_scale, b_scale, a_dev, b_dev, 2 * n, st);
-    case B2_C128:
-      return lincomb_real<double>(ctx, (double*)out, (const double*)x, (const double*)y, a_scale, b_scale, a_dev, b_dev, 2 * n, st);
-    default:
-      return B2_ERR_DTYPE;
-  }
+  // real coefficients: complex data runs as 2 n reals
+  return b2_dispatch(dtype, [&](auto t) {
+    using R = b2_real_t<decltype(t)>;
+    return lincomb_real<R>(ctx, (R*)out, (const R*)x, (const R*)y, a_scale, b_scale, a_dev, b_dev,
+                           b2_is_cx_v<decltype(t)> ? 2 * n : n, st);
+  });
 }
 
 extern "C" int b2_mul(b2_ctx* ctx, void* out, const void* x, const void* y, size_t n, int dtype,
@@ -220,21 +199,18 @@ extern "C" int b2_mul(b2_ctx* ctx, void* out, const void* x, const void* y, size
   if (n == 0) return B2_OK;
   cudaStream_t st = (cudaStream_t)stream;
   int grid = ew_grid(ctx, n);
-  switch (dtype) {
-    case B2_F32: mul_real_kernel<float><<<grid, EW_THREADS, 0, st>>>((float*)out, (const float*)x, (const float*)y, n); break;
-    case B2_F64: mul_real_kernel<double><<<grid, EW_THREADS, 0, st>>>((double*)out, (const double*)x, (const double*)y, n); break;
-    case B2_C64:
-      if (conj_x) mul_cx_kernel<float, true><<<grid, EW_THREADS, 0, st>>>((Cx<float>*)out, (const Cx<float>*)x, (const Cx<float>*)y, n);
-      else mul_cx_kernel<float, false><<<grid, EW_THREADS, 0, st>>>((Cx<float>*)out, (const Cx<float>*)x, (const Cx<float>*)y, n);
-      break;
-    case B2_C128:
-      if (conj_x) mul_cx_kernel<double, true><<<grid, EW_THREADS, 0, st>>>((Cx<double>*)out, (const Cx<double>*)x, (const Cx<double>*)y, n);
-      else mul_cx_kernel<double, false><<<grid, EW_THREADS, 0, st>>>((Cx<double>*)out, (const Cx<double>*)x, (const Cx<double>*)y, n);
-      break;
-    default: return B2_ERR_DTYPE;
-  }
-  B2_LAUNCH_CHECK();
-  return B2_OK;
+  return b2_dispatch(dtype, [&](auto t) -> int {
+    using T = decltype(t);
+    if constexpr (b2_is_cx_v<T>) {
+      using R = b2_real_t<T>;
+      if (conj_x) mul_cx_kernel<R, true><<<grid, EW_THREADS, 0, st>>>((T*)out, (const T*)x, (const T*)y, n);
+      else mul_cx_kernel<R, false><<<grid, EW_THREADS, 0, st>>>((T*)out, (const T*)x, (const T*)y, n);
+    } else {
+      mul_real_kernel<T><<<grid, EW_THREADS, 0, st>>>((T*)out, (const T*)x, (const T*)y, n);
+    }
+    B2_LAUNCH_CHECK();
+    return B2_OK;
+  });
 }
 
 extern "C" int b2_fill(b2_ctx* ctx, void* out, const double v[2], size_t n, int dtype,
@@ -243,15 +219,17 @@ extern "C" int b2_fill(b2_ctx* ctx, void* out, const double v[2], size_t n, int 
   if (n == 0) return B2_OK;
   cudaStream_t st = (cudaStream_t)stream;
   int grid = ew_grid(ctx, n);
-  switch (dtype) {
-    case B2_F32: fill_kernel<float><<<grid, EW_THREADS, 0, st>>>((float*)out, (float)v[0], n); break;
-    case B2_F64: fill_kernel<double><<<grid, EW_THREADS, 0, st>>>((double*)out, v[0], n); break;
-    case B2_C64: fill_kernel<float2><<<grid, EW_THREADS, 0, st>>>((float2*)out, make_float2((float)v[0], (float)v[1]), n); break;
-    case B2_C128: fill_kernel<double2><<<grid, EW_THREADS, 0, st>>>((double2*)out, make_double2(v[0], v[1]), n); break;
-    default: return B2_ERR_DTYPE;
-  }
-  B2_LAUNCH_CHECK();
-  return B2_OK;
+  return b2_dispatch(dtype, [&](auto t) -> int {
+    using T = decltype(t);
+    if constexpr (b2_is_cx_v<T>) {   // one 8- / 16-byte store per complex element
+      using P = b2_pair_t<b2_real_t<T>>;
+      fill_kernel<P><<<grid, EW_THREADS, 0, st>>>((P*)out, P{(b2_real_t<T>)v[0], (b2_real_t<T>)v[1]}, n);
+    } else {
+      fill_kernel<T><<<grid, EW_THREADS, 0, st>>>((T*)out, (T)v[0], n);
+    }
+    B2_LAUNCH_CHECK();
+    return B2_OK;
+  });
 }
 
 

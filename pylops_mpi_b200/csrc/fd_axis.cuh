@@ -10,14 +10,14 @@ constexpr int DS_NONE = 0, DS_FWD = 1, DS_ADJ = 2;
 template <int DS>
 struct DsTag { static constexpr int value = DS; };
 
-// f(T(), DsTag<DS>()) for the real dtype (B2_F32 / B2_F64, checked by the caller) and the stage of a plain
-// (fused == false) or derivative-fused launch
+// f(T(), DsTag<DS>()) for the real dtype (B2_ERR_DTYPE for any other) and the stage of a plain (fused == false) or
+// derivative-fused launch
 template <typename F>
 int ds_dispatch(int dtype, bool fused, int adjoint, F f) {
   const auto stage = [&](auto t) {
     return !fused ? f(t, DsTag<DS_NONE>()) : adjoint ? f(t, DsTag<DS_ADJ>()) : f(t, DsTag<DS_FWD>());
   };
-  return dtype == B2_F32 ? stage(float()) : stage(double());
+  return b2_dispatch_real(dtype, stage);
 }
 
 // (D x)[j] from x[j-1], x[j], x[j+1] on a line of n samples: 0.5 (x[j+1] - x[j-1]) on [1, n-2] (centered) or

@@ -13,39 +13,18 @@
 
 namespace {
 
-struct c32 { float re, im; };
-struct c64 { double re, im; };
-
-template <typename T> struct Num;
-template <> struct Num<float> {
-  __device__ static __forceinline__ float zero() { return 0.f; }
-  __device__ static __forceinline__ void fma_(float& c, float a, float b) { c = fmaf(a, b, c); }
-  __device__ static __forceinline__ float conj(float a) { return a; }
-  __device__ static __forceinline__ float add(float a, float b) { return a + b; }
+template <typename T> struct Num {   // float / double
+  __device__ static __forceinline__ T zero() { return T(0); }
+  __device__ static __forceinline__ void fma_(T& c, T a, T b) { c = fma(a, b, c); }
+  __device__ static __forceinline__ T conj(T a) { return a; }
+  __device__ static __forceinline__ T add(T a, T b) { return a + b; }
 };
-template <> struct Num<double> {
-  __device__ static __forceinline__ double zero() { return 0.0; }
-  __device__ static __forceinline__ void fma_(double& c, double a, double b) { c = fma(a, b, c); }
-  __device__ static __forceinline__ double conj(double a) { return a; }
-  __device__ static __forceinline__ double add(double a, double b) { return a + b; }
-};
-template <> struct Num<c32> {
-  __device__ static __forceinline__ c32 zero() { return {0.f, 0.f}; }
-  __device__ static __forceinline__ void fma_(c32& c, c32 a, c32 b) {
-    c.re = fmaf(a.re, b.re, fmaf(-a.im, b.im, c.re));
-    c.im = fmaf(a.re, b.im, fmaf(a.im, b.re, c.im));
-  }
-  __device__ static __forceinline__ c32 conj(c32 a) { return {a.re, -a.im}; }
-  __device__ static __forceinline__ c32 add(c32 a, c32 b) { return {a.re + b.re, a.im + b.im}; }
-};
-template <> struct Num<c64> {
-  __device__ static __forceinline__ c64 zero() { return {0.0, 0.0}; }
-  __device__ static __forceinline__ void fma_(c64& c, c64 a, c64 b) {
-    c.re = fma(a.re, b.re, fma(-a.im, b.im, c.re));
-    c.im = fma(a.re, b.im, fma(a.im, b.re, c.im));
-  }
-  __device__ static __forceinline__ c64 conj(c64 a) { return {a.re, -a.im}; }
-  __device__ static __forceinline__ c64 add(c64 a, c64 b) { return {a.re + b.re, a.im + b.im}; }
+template <typename R> struct Num<b2_cx<R>> {
+  using C = b2_cx<R>;
+  __device__ static __forceinline__ C zero() { return {R(0), R(0)}; }
+  __device__ static __forceinline__ void fma_(C& c, C a, C b) { b2_cx_fma(c, a, b); }
+  __device__ static __forceinline__ C conj(C a) { return b2_cx_conj(a); }
+  __device__ static __forceinline__ C add(C a, C b) { return b2_cx_add(a, b); }
 };
 
 constexpr int BM = 64, BN = 64, BK = 16, TM = 4, TN = 4;
@@ -130,19 +109,22 @@ gemm_simt_kernel(const T* __restrict__ A, size_t lda, size_t sA, const T* __rest
   }
 }
 
-template <typename T>
+// FUSED: the epilogue also stores to the peers (b2_batched_gemm_allgather).  That entry point does not check the grid
+// here: an empty or too tall grid is left to the launch, which returns CUDA's error code
+template <typename T, bool FUSED = false>
 int launch_gemm(const void* A, size_t lda, size_t sA, const void* B, size_t ldb, size_t sB,
                 void* C, size_t ldc, size_t sC, size_t m, size_t n, size_t k, size_t batch,
-                int op_a, bool accumulate, cudaStream_t st) {
-  if (m == 0 || n == 0 || batch == 0) return B2_OK;
-  if (batch > 65535) return B2_ERR_ARG;
+                int op_a, bool accumulate, cudaStream_t st, const PeerDst& peers = PeerDst{}) {
   dim3 grid((unsigned)((n + BN - 1) / BN), (unsigned)((m + BM - 1) / BM), (unsigned)batch);
-  if (grid.y > 65535u) return B2_ERR_ARG;
+  if (!FUSED) {
+    if (m == 0 || n == 0 || batch == 0) return B2_OK;
+    if (batch > 65535 || grid.y > 65535u) return B2_ERR_ARG;
+  }
   const bool conj = (op_a == B2_OP_H);
   if (op_a == B2_OP_N)
-    gemm_simt_kernel<T, false><<<grid, 256, 0, st>>>((const T*)A, lda, sA, (const T*)B, ldb, sB, (T*)C, ldc, sC, m, n, k, false, accumulate);
+    gemm_simt_kernel<T, false, FUSED><<<grid, 256, 0, st>>>((const T*)A, lda, sA, (const T*)B, ldb, sB, (T*)C, ldc, sC, m, n, k, false, accumulate, peers);
   else
-    gemm_simt_kernel<T, true><<<grid, 256, 0, st>>>((const T*)A, lda, sA, (const T*)B, ldb, sB, (T*)C, ldc, sC, m, n, k, conj, accumulate);
+    gemm_simt_kernel<T, true, FUSED><<<grid, 256, 0, st>>>((const T*)A, lda, sA, (const T*)B, ldb, sB, (T*)C, ldc, sC, m, n, k, conj, accumulate, peers);
   B2_LAUNCH_CHECK();
   return B2_OK;
 }
@@ -150,34 +132,12 @@ int launch_gemm(const void* A, size_t lda, size_t sA, const void* B, size_t ldb,
 int dispatch(const void* A, size_t lda, size_t sA, const void* B, size_t ldb, size_t sB, void* C,
              size_t ldc, size_t sC, size_t m, size_t n, size_t k, size_t batch, int op_a,
              bool accumulate, int dtype, cudaStream_t st) {
-  switch (dtype) {
-    case B2_F32: return launch_gemm<float>(A, lda, sA, B, ldb, sB, C, ldc, sC, m, n, k, batch, op_a, accumulate, st);
-    case B2_F64: return launch_gemm<double>(A, lda, sA, B, ldb, sB, C, ldc, sC, m, n, k, batch, op_a, accumulate, st);
-    case B2_C64: return launch_gemm<c32>(A, lda, sA, B, ldb, sB, C, ldc, sC, m, n, k, batch, op_a, accumulate, st);
-    case B2_C128: return launch_gemm<c64>(A, lda, sA, B, ldb, sB, C, ldc, sC, m, n, k, batch, op_a, accumulate, st);
-    default: return B2_ERR_DTYPE;
-  }
+  return b2_dispatch(dtype, [&](auto t) {
+    return launch_gemm<decltype(t)>(A, lda, sA, B, ldb, sB, C, ldc, sC, m, n, k, batch, op_a, accumulate, st);
+  });
 }
 
 }  // namespace
-
-template <typename T>
-static int launch_fused(const void* G, const void* x, void* y, void* const* peers, int npeers, size_t nsl, size_t nx,
-                 size_t ny, size_t nz, int adjoint, cudaStream_t st) {
-  const size_t m = adjoint ? ny : nx, k = adjoint ? nx : ny;
-  PeerDst pd;
-  pd.n = npeers;
-  for (int d = 0; d < 8; ++d) pd.p[d] = d < npeers ? peers[d] : nullptr;
-  dim3 grid((unsigned)((nz + BN - 1) / BN), (unsigned)((m + BM - 1) / BM), (unsigned)nsl);
-  if (adjoint)
-    gemm_simt_kernel<T, true, true><<<grid, 256, 0, st>>>((const T*)G, ny, nx * ny, (const T*)x, nz, k * nz, (T*)y, nz,
-                                                          m * nz, m, nz, k, true, false, pd);
-  else
-    gemm_simt_kernel<T, false, true><<<grid, 256, 0, st>>>((const T*)G, ny, nx * ny, (const T*)x, nz, k * nz, (T*)y, nz,
-                                                           m * nz, m, nz, k, false, false, pd);
-  B2_LAUNCH_CHECK();
-  return B2_OK;
-}
 
 // y[s] = op(G[s]) x[s] written to the local output AND to the same offsets of `npeers` peer buffers
 // (fused product + all-gather over NVLink peer memory).  peers_host[d] must already point at the
@@ -189,14 +149,14 @@ extern "C" int b2_batched_gemm_allgather(b2_ctx* ctx, const void* G, const void*
   if (nsl == 0) return B2_OK;
   if (!G || !x || !y || (npeers && !peers_host)) return B2_ERR_ARG;
   if (nsl > 65535) return B2_ERR_ARG;
-  cudaStream_t st = (cudaStream_t)stream;
-  switch (dtype) {
-    case B2_F32: return launch_fused<float>(G, x, y, peers_host, npeers, nsl, nx, ny, nz, adjoint, st);
-    case B2_F64: return launch_fused<double>(G, x, y, peers_host, npeers, nsl, nx, ny, nz, adjoint, st);
-    case B2_C64: return launch_fused<c32>(G, x, y, peers_host, npeers, nsl, nx, ny, nz, adjoint, st);
-    case B2_C128: return launch_fused<c64>(G, x, y, peers_host, npeers, nsl, nx, ny, nz, adjoint, st);
-    default: return B2_ERR_DTYPE;
-  }
+  const size_t m = adjoint ? ny : nx, k = adjoint ? nx : ny;
+  PeerDst pd;
+  pd.n = npeers;
+  for (int d = 0; d < 8; ++d) pd.p[d] = d < npeers ? peers_host[d] : nullptr;
+  return b2_dispatch(dtype, [&](auto t) {
+    return launch_gemm<decltype(t), true>(G, ny, nx * ny, x, nz, k * nz, y, nz, m * nz, m, nz, k, nsl,
+                                          adjoint ? B2_OP_H : B2_OP_N, false, (cudaStream_t)stream, pd);
+  });
 }
 
 // symmetric (peer-mappable) buffers: plain cudaMalloc + CUDA IPC handles exchanged by the caller

@@ -15,41 +15,19 @@
 namespace {
 
 // ---- element traits ---------------------------------------------------------
-struct cf32 { float re, im; };
-struct cf64 { double re, im; };
-
-template <typename TA> struct ElemTraits;
-template <> struct ElemTraits<float> {
-  using X = float; using Acc = float; static constexpr int V = 4;
-  __device__ static __forceinline__ Acc zero() { return 0.f; }
-  __device__ static __forceinline__ void fma_(Acc& acc, float a, float x, bool) { acc = fmaf(a, x, acc); }
+template <typename TA> struct ElemTraits {   // float / double
+  using X = TA; using Acc = TA; static constexpr int V = 16 / sizeof(TA);
+  __device__ static __forceinline__ Acc zero() { return TA(0); }
+  __device__ static __forceinline__ void fma_(Acc& acc, TA a, TA x, bool) { acc = fma(a, x, acc); }
   __device__ static __forceinline__ Acc add(Acc a, Acc b) { return a + b; }
 };
-template <> struct ElemTraits<double> {
-  using X = double; using Acc = double; static constexpr int V = 2;
-  __device__ static __forceinline__ Acc zero() { return 0.0; }
-  __device__ static __forceinline__ void fma_(Acc& acc, double a, double x, bool) { acc = fma(a, x, acc); }
-  __device__ static __forceinline__ Acc add(Acc a, Acc b) { return a + b; }
-};
-template <> struct ElemTraits<cf32> {
-  using X = cf32; using Acc = cf32; static constexpr int V = 2;
-  __device__ static __forceinline__ Acc zero() { return {0.f, 0.f}; }
-  __device__ static __forceinline__ void fma_(Acc& acc, cf32 a, cf32 x, bool conj) {
-    float ai = conj ? -a.im : a.im;
-    acc.re = fmaf(a.re, x.re, fmaf(-ai, x.im, acc.re));
-    acc.im = fmaf(a.re, x.im, fmaf(ai, x.re, acc.im));
+template <typename R> struct ElemTraits<b2_cx<R>> {
+  using X = b2_cx<R>; using Acc = b2_cx<R>; static constexpr int V = 16 / sizeof(b2_cx<R>);
+  __device__ static __forceinline__ Acc zero() { return {R(0), R(0)}; }
+  __device__ static __forceinline__ void fma_(Acc& acc, X a, X x, bool conj) {
+    b2_cx_fma(acc, conj ? b2_cx_conj(a) : a, x);
   }
-  __device__ static __forceinline__ Acc add(Acc a, Acc b) { return {a.re + b.re, a.im + b.im}; }
-};
-template <> struct ElemTraits<cf64> {
-  using X = cf64; using Acc = cf64; static constexpr int V = 1;
-  __device__ static __forceinline__ Acc zero() { return {0.0, 0.0}; }
-  __device__ static __forceinline__ void fma_(Acc& acc, cf64 a, cf64 x, bool conj) {
-    double ai = conj ? -a.im : a.im;
-    acc.re = fma(a.re, x.re, fma(-ai, x.im, acc.re));
-    acc.im = fma(a.re, x.im, fma(ai, x.re, acc.im));
-  }
-  __device__ static __forceinline__ Acc add(Acc a, Acc b) { return {a.re + b.re, a.im + b.im}; }
+  __device__ static __forceinline__ Acc add(Acc a, Acc b) { return b2_cx_add(a, b); }
 };
 template <> struct ElemTraits<__nv_bfloat16> {
   using X = float; using Acc = float; static constexpr int V = 8;
@@ -60,13 +38,8 @@ template <> struct ElemTraits<__nv_bfloat16> {
   __device__ static __forceinline__ Acc add(Acc a, Acc b) { return a + b; }
 };
 
-template <typename A> __device__ __forceinline__ A shfl_xor_t(A v, int o);
-template <> __device__ __forceinline__ float shfl_xor_t(float v, int o) { return __shfl_xor_sync(0xffffffffu, v, o); }
-template <> __device__ __forceinline__ double shfl_xor_t(double v, int o) { return __shfl_xor_sync(0xffffffffu, v, o); }
-template <> __device__ __forceinline__ cf32 shfl_xor_t(cf32 v, int o) {
-  return {__shfl_xor_sync(0xffffffffu, v.re, o), __shfl_xor_sync(0xffffffffu, v.im, o)};
-}
-template <> __device__ __forceinline__ cf64 shfl_xor_t(cf64 v, int o) {
+template <typename A> __device__ __forceinline__ A shfl_xor_t(A v, int o) { return __shfl_xor_sync(0xffffffffu, v, o); }
+template <typename R> __device__ __forceinline__ b2_cx<R> shfl_xor_t(b2_cx<R> v, int o) {
   return {__shfl_xor_sync(0xffffffffu, v.re, o), __shfl_xor_sync(0xffffffffu, v.im, o)};
 }
 
@@ -82,25 +55,15 @@ __device__ __forceinline__ AVec<TA> load_a(const TA* p) {
   return o;
 }
 
-// cached scalar loads for every element type
-__device__ __forceinline__ float ldg_t(const float* p) { return __ldg(p); }
-__device__ __forceinline__ double ldg_t(const double* p) { return __ldg(p); }
-__device__ __forceinline__ cf32 ldg_t(const cf32* p) {
-  float2 t = __ldg(reinterpret_cast<const float2*>(p));
+// cached scalar loads for every element type (a complex element in one 8- / 16-byte load)
+template <typename T> __device__ __forceinline__ T ldg_t(const T* p) { return __ldg(p); }
+template <typename R> __device__ __forceinline__ b2_cx<R> ldg_t(const b2_cx<R>* p) {
+  const b2_pair_t<R> t = __ldg(reinterpret_cast<const b2_pair_t<R>*>(p));
   return {t.x, t.y};
 }
-__device__ __forceinline__ cf64 ldg_t(const cf64* p) {
-  double2 t = __ldg(reinterpret_cast<const double2*>(p));
-  return {t.x, t.y};
-}
-__device__ __forceinline__ float ldcg_t(const float* p) { return __ldcg(p); }
-__device__ __forceinline__ double ldcg_t(const double* p) { return __ldcg(p); }
-__device__ __forceinline__ cf32 ldcg_t(const cf32* p) {
-  float2 t = __ldcg(reinterpret_cast<const float2*>(p));
-  return {t.x, t.y};
-}
-__device__ __forceinline__ cf64 ldcg_t(const cf64* p) {
-  double2 t = __ldcg(reinterpret_cast<const double2*>(p));
+template <typename T> __device__ __forceinline__ T ldcg_t(const T* p) { return __ldcg(p); }
+template <typename R> __device__ __forceinline__ b2_cx<R> ldcg_t(const b2_cx<R>* p) {
+  const b2_pair_t<R> t = __ldcg(reinterpret_cast<const b2_pair_t<R>*>(p));
   return {t.x, t.y};
 }
 
@@ -420,11 +383,5 @@ extern "C" int b2_gemv(b2_ctx* ctx, const void* A, size_t lda, size_t m, size_t 
     return launch_gemv<__nv_bfloat16>(ctx, A, lda, m, n, x, y, op, st);
   }
   if (dtype_a != dtype_xy) return B2_ERR_DTYPE;
-  switch (dtype_a) {
-    case B2_F32: return launch_gemv<float>(ctx, A, lda, m, n, x, y, op, st);
-    case B2_F64: return launch_gemv<double>(ctx, A, lda, m, n, x, y, op, st);
-    case B2_C64: return launch_gemv<cf32>(ctx, A, lda, m, n, x, y, op, st);
-    case B2_C128: return launch_gemv<cf64>(ctx, A, lda, m, n, x, y, op, st);
-    default: return B2_ERR_DTYPE;
-  }
+  return b2_dispatch(dtype_a, [&](auto t) { return launch_gemv<decltype(t)>(ctx, A, lda, m, n, x, y, op, st); });
 }

@@ -223,17 +223,16 @@ int check_args(b2_ctx* ctx, const void* x, void* y, const double* ts, const doub
   return B2_OK;
 }
 
-// image points [i0, i0 + nc): the image side (x forward, y adjoint) starts at i0, the tables hold the chunk only
+// image points [i0, i0 + nc): the image side (x forward, y adjoint) starts at i0, the tables hold the chunk only;
+// B2_ERR_DTYPE for a dtype other than F32 / F64, after every other check of the entry points
 int apply(const void* x, void* y, const double* ts, const double* tr, size_t i0, size_t nc, size_t ns, size_t nr,
           size_t nt, double dt, int adjoint, bool accumulate, int dtype, cudaStream_t st) {
-  if (dtype == B2_F32) {
-    const float* xf = static_cast<const float*>(x) + (adjoint ? 0 : i0);
-    float* yf = static_cast<float*>(y) + (adjoint ? i0 : 0);
-    return launch<float>(xf, yf, ts, tr, nc, (int)ns, (int)nr, nt, dt, adjoint, accumulate, st);
-  }
-  const double* xd = static_cast<const double*>(x) + (adjoint ? 0 : i0);
-  double* yd = static_cast<double*>(y) + (adjoint ? i0 : 0);
-  return launch<double>(xd, yd, ts, tr, nc, (int)ns, (int)nr, nt, dt, adjoint, accumulate, st);
+  return b2_dispatch_real(dtype, [&](auto t) {
+    using T = decltype(t);
+    const T* xt = static_cast<const T*>(x) + (adjoint ? 0 : i0);
+    T* yt = static_cast<T*>(y) + (adjoint ? i0 : 0);
+    return launch<T>(xt, yt, ts, tr, nc, (int)ns, (int)nr, nt, dt, adjoint, accumulate, st);
+  });
 }
 
 }  // namespace
@@ -243,7 +242,6 @@ extern "C" int b2_kirchhoff(b2_ctx* ctx, const void* x, void* y, const double* t
                             void* stream) {
   const int rc = check_args(ctx, x, y, trav_srcs, trav_recs, ni, ns, nr, nt, dt);
   if (rc != B2_OK) return rc;
-  if (dtype != B2_F32 && dtype != B2_F64) return B2_ERR_DTYPE;
   return apply(x, y, trav_srcs, trav_recs, 0, ni, ns, nr, nt, dt, adjoint, false, dtype, (cudaStream_t)stream);
 }
 
@@ -254,7 +252,6 @@ extern "C" int b2_kirchhoff_chunk(b2_ctx* ctx, const void* x, void* y, const dou
   if (rc != B2_OK) return rc;
   if (nc == 0 || i0 % 32 != 0 || i0 >= ni || nc > ni - i0) return B2_ERR_ARG;
   if (accumulate != 0 && (accumulate != 1 || adjoint)) return B2_ERR_ARG;
-  if (dtype != B2_F32 && dtype != B2_F64) return B2_ERR_DTYPE;
   return apply(x, y, trav_srcs, trav_recs, i0, nc, ns, nr, nt, dt, adjoint, accumulate != 0, dtype,
                (cudaStream_t)stream);
 }

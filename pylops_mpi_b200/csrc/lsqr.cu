@@ -321,10 +321,8 @@ extern "C" int b2_lsqr_update(b2_ctx* ctx, void* x, void* w, const void* v, void
   if (n && (!x || !w || !v || x == w || x == v || w == v || (var && (var == x || var == w || var == v))))
     return B2_ERR_ARG;
   const size_t n_real = cx ? 2 * n : n;
-  switch (dtype) {
-    case B2_F32: return launch_update_var<float, false>(ctx, x, w, v, var, n_real, coef_dev, stop_dev, dd_dev, st);
-    case B2_F64: return launch_update_var<double, false>(ctx, x, w, v, var, n_real, coef_dev, stop_dev, dd_dev, st);
-    case B2_C64: return launch_update_var<float, true>(ctx, x, w, v, var, n_real, coef_dev, stop_dev, dd_dev, st);
-    default: return launch_update_var<double, true>(ctx, x, w, v, var, n_real, coef_dev, stop_dev, dd_dev, st);
-  }
+  return b2_dispatch(dtype, [&](auto t) {
+    return launch_update_var<b2_real_t<decltype(t)>, b2_is_cx_v<decltype(t)>>(ctx, x, w, v, var, n_real, coef_dev,
+                                                                              stop_dev, dd_dev, st);
+  });
 }

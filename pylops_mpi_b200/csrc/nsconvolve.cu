@@ -275,7 +275,6 @@ int ns_axis(b2_ctx* ctx, const void* x, void* y, size_t n_outer, size_t n_axis, 
   if (n_outer == 0 || n_axis == 0 || n_inner == 0) return B2_ERR_ARG;
   if (nfilt < 1 || nh < 1 || hc < 0 || hc >= nh || dh < 1) return B2_ERR_ARG;
   if (fused && kind != B2_FD_CENTERED && kind != B2_FD_FORWARD) return B2_ERR_ARG;
-  if (dtype != B2_F32 && dtype != B2_F64) return B2_ERR_DTYPE;
   return ds_dispatch(dtype, fused, adjoint, [&](auto t, auto ds) {
     return launch_ns<decltype(t), decltype(ds)::value>(x, y, hs, n_outer, n_axis, n_inner, nfilt, nh, hc, oh, dh,
                                                        adjoint ? 1 : 0, kind, (cudaStream_t)stream);

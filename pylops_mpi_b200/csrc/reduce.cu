@@ -181,13 +181,10 @@ int launch_reduce(b2_ctx* ctx, F f, const void* x, const void* y, size_t n_real,
 template <typename F>
 int dispatch_reduce(b2_ctx* ctx, F f, const void* x, const void* y, size_t n, int dtype,
                     double* out, cudaStream_t st) {
-  switch (dtype) {
-    case B2_F32: return launch_reduce<float, false, F>(ctx, f, x, y, n, out, st);
-    case B2_F64: return launch_reduce<double, false, F>(ctx, f, x, y, n, out, st);
-    case B2_C64: return launch_reduce<float, true, F>(ctx, f, x, y, 2 * n, out, st);
-    case B2_C128: return launch_reduce<double, true, F>(ctx, f, x, y, 2 * n, out, st);
-    default: return B2_ERR_DTYPE;
-  }
+  return b2_dispatch(dtype, [&](auto t) {
+    constexpr bool CX = b2_is_cx_v<decltype(t)>;
+    return launch_reduce<b2_real_t<decltype(t)>, CX, F>(ctx, f, x, y, CX ? 2 * n : n, out, st);
+  });
 }
 
 __global__ void zero_out_kernel(double* out, int k, double v) {
@@ -289,22 +286,14 @@ extern "C" int b2_dot_multi(b2_ctx* ctx, int k, const void* const* xs, const voi
     p.x[i] = xs[i];
     p.y[i] = ys[i];
   }
-  // output layout: k (re, im) pairs; real dtypes write re only -> zero first
-  const bool cx = (dtype == B2_C64 || dtype == B2_C128);
-  if (!cx) {
-    // real: kernel writes out[0..k); repack to (re,im) pairs is done by the caller reading
-    // out[j] for j<k.  Keep the layout simple: real dtypes -> k doubles.
-    switch (dtype) {
-      case B2_F32: return launch_multi<float, false, false>(ctx, k, p, n, out_dev, st);
-      case B2_F64: return launch_multi<double, false, false>(ctx, k, p, n, out_dev, st);
+  return b2_dispatch(dtype, [&](auto t) {
+    using R = b2_real_t<decltype(t)>;
+    constexpr bool CX = b2_is_cx_v<decltype(t)>;
+    if constexpr (CX) {
+      if (conj_x) return launch_multi<R, true, true>(ctx, k, p, 2 * n, out_dev, st);
     }
-    return B2_ERR_DTYPE;
-  }
-  if (dtype == B2_C64)
-    return conj_x ? launch_multi<float, true, true>(ctx, k, p, 2 * n, out_dev, st)
-                  : launch_multi<float, true, false>(ctx, k, p, 2 * n, out_dev, st);
-  return conj_x ? launch_multi<double, true, true>(ctx, k, p, 2 * n, out_dev, st)
-                : launch_multi<double, true, false>(ctx, k, p, 2 * n, out_dev, st);
+    return launch_multi<R, CX, false>(ctx, k, p, CX ? 2 * n : n, out_dev, st);
+  });
 }
 
 // ---- device-resident scalar arithmetic for solver recurrences ------------------------

@@ -241,11 +241,7 @@ extern "C" int b2_sparse_update(b2_ctx* ctx, const void* base, const void* g, do
   p.half_cut = (pow(54.0, 1.0 / 3.0) / 4.0) * pow(thresh, 2.0 / 3.0);  // pylops' 54 ** (1/3), not cbrt(54)
   p.n_real = cx ? 2 * n : n;
   cudaStream_t st = (cudaStream_t)stream;
-  switch (dtype) {
-    case B2_F32: return launch<float, false>(ctx, p, sums_dev, st);
-    case B2_F64: return launch<double, false>(ctx, p, sums_dev, st);
-    case B2_C64: return launch<float, true>(ctx, p, sums_dev, st);
-    case B2_C128: return launch<double, true>(ctx, p, sums_dev, st);
-    default: return B2_ERR_DTYPE;
-  }
+  return b2_dispatch(dtype, [&](auto t) {
+    return launch<b2_real_t<decltype(t)>, b2_is_cx_v<decltype(t)>>(ctx, p, sums_dev, st);
+  });
 }

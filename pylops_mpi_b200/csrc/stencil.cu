@@ -417,11 +417,7 @@ int launch_stencil(b2_ctx* ctx, const void* x, void* y, const void* lo, const vo
 // dtype F32 / F64 (complex data: the real dtype and twice the columns)
 int launch_stencil(b2_ctx* ctx, const void* x, void* y, const void* lo, const void* hi, const StencilParams& p,
                    int dtype, cudaStream_t st) {
-  switch (dtype) {
-    case B2_F32: return launch_stencil<float>(ctx, x, y, lo, hi, p, st);
-    case B2_F64: return launch_stencil<double>(ctx, x, y, lo, hi, p, st);
-    default: return B2_ERR_DTYPE;
-  }
+  return b2_dispatch_real(dtype, [&](auto t) { return launch_stencil<decltype(t)>(ctx, x, y, lo, hi, p, st); });
 }
 
 }  // namespace
@@ -624,8 +620,7 @@ extern "C" int b2_derivative_peer(b2_ctx* ctx, b2_halo* h, const void* x, void* 
   hp.send_lo = h->box[0] ? need_hi : 0;    // rank-1 needs my first need_hi rows as ITS hi halo
   hp.send_hi = h->box[2] ? need_lo : 0;    // rank+1 needs my last need_lo rows as ITS lo halo
   cudaStream_t st = (cudaStream_t)stream;
-  return dtype == B2_F32 ? launch_vec<float, true>(x, y, nullptr, nullptr, p, hp, st)
-                         : launch_vec<double, true>(x, y, nullptr, nullptr, p, hp, st);
+  return b2_dispatch_real(dtype, [&](auto t) { return launch_vec<decltype(t), true>(x, y, nullptr, nullptr, p, hp, st); });
 }
 
 // ---- rank-local derivative along the MIDDLE axis of a C-ordered [n_outer][n_axis][n_inner] block ------
