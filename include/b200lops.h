@@ -46,8 +46,7 @@ enum { B2_OK = 0, B2_ERR_DTYPE = 2001, B2_ERR_ARG = 2002, B2_ERR_HALO = 2003,
  * stream-ordered with respect to each other: use one b2_ctx per stream that issues reductions concurrently. */
 typedef struct b2_ctx b2_ctx;
 typedef struct b2_comm b2_comm;          /* one NCCL communicator (world, mask group, grid row / col) */
-typedef struct b2_peer b2_peer;          /* peer-memory mailbox group for one-shot SCALAR all-reduces */
-typedef struct b2_peer_vec b2_peer_vec;  /* peer-memory mailboxes for one-shot VECTOR all-reduces */
+typedef struct b2_mailbox b2_mailbox;    /* peer-memory mailboxes: one-shot collectives and the fused halo exchange */
 
 int b2_version(void);
 const char* b2_strerror(int code);
@@ -274,17 +273,12 @@ int b2_eikonal_tables(b2_ctx* ctx, const double* vel, size_t ny, size_t nx, size
  * (one more iterate and the slowness); 0 for a zero or too large size */
 size_t b2_eikonal_work_bytes(size_t ny, size_t nx, size_t nz, size_t n);
 /* Peer-memory halo exchange fused INTO the stencil kernel (replaces the add_ghost_cells Send/Recv pairs of
- * DistributedArray.py:876-953 as used by FirstDerivative.py:221-247, 276-319 and SecondDerivative.py): every rank
- * owns a box of b2_halo_bytes(cap) bytes in IPC-mapped memory (b2_symm_alloc + b2_ipc_*); boxes_host[r] is rank r's
- * box as mapped in this process.  b2_derivative_peer is ONE launch per apply: the first CTAs push the boundary rows
- * into the neighbours' boxes over NVLink and publish a flag, the CTAs of the first / last row chunk run last and
- * wait for it.  Collective: same call sequence on every rank of the handle, all on one stream; each rank must
- * own >= 2 rows; 2 * ncols * sizeof(dtype) must fit in cap_bytes.  deriv = 1 | 2 (first | second derivative). */
-typedef struct b2_halo b2_halo;
-size_t b2_halo_bytes(size_t cap_bytes);
-int b2_halo_create(int rank, int size, void* const* boxes_host, size_t cap_bytes, b2_halo** out);
-int b2_halo_destroy(b2_halo* h);
-int b2_derivative_peer(b2_ctx* ctx, b2_halo* h, const void* x, void* y, size_t nrows_local, size_t ncols,
+ * DistributedArray.py:876-953 as used by FirstDerivative.py:221-247, 276-319 and SecondDerivative.py), on the halo
+ * region of the mailboxes of b2_mailbox_create.  ONE launch per apply: the first CTAs push the boundary rows into the
+ * neighbours' boxes over NVLink and publish a flag, the CTAs of the first / last row chunk run last and wait for it.
+ * Collective: same call sequence on every rank of the handle, all on one stream; each rank must own >= 2 rows;
+ * 2 * ncols * sizeof(dtype) must fit in halo_cap (B2_ERR_WORKSPACE).  deriv = 1 | 2 (first | second derivative). */
+int b2_derivative_peer(b2_ctx* ctx, b2_mailbox* h, const void* x, void* y, size_t nrows_local, size_t ncols,
                        size_t row0, size_t nrows_global, int deriv, int kind, int order, int edge, double sampling,
                        int adjoint, int dtype, void* stream);
 /* Same operator on HOST buffers (pageable or pinned).  x_host / y_host address the
@@ -365,27 +359,31 @@ int b2_ipc_get_handle(void* p, void* handle64_host);
 int b2_ipc_open_handle(const void* handle64_host, void** out);
 int b2_ipc_close_handle(void* p);
 
-/* One-shot all-reduce of k <= 8 float64 scalars over NVLink peer memory (no NCCL): the collective half
- * of DistributedArray.dot / norm (DistributedArray.py:684-686, 714-757) and of the CGLS step scalars.
- * slots_host[r] = rank r's mailbox (b2_symm_alloc of b2_peer_slots_bytes(), IPC-mapped here). */
-size_t b2_peer_slots_bytes(void);
-int b2_peer_create(int rank, int size, void* const* slots_host, b2_peer** out);
-int b2_peer_destroy(b2_peer* peer);
-int b2_peer_allreduce(b2_peer* peer, double* vals_dev, int k, int op, void* stream);
+/* Peer-memory mailboxes over NVLink (no NCCL): every rank of a group of 1..8 owns one box of
+ * b2_mailbox_bytes(halo_cap) bytes (b2_symm_alloc), and boxes_host[r] is rank r's box as IPC-mapped in this process
+ * (own pointer for r == rank).  The box has one region per use: the scalar all-reduce, the vector all-reduce /
+ * all-gather, and the halo exchange of b2_derivative_peer, whose slots hold halo_cap bytes (a multiple of 16) per
+ * parity and side.  Create zeroes this rank's region headers: every rank creates its handle before any rank's first
+ * call on it.  Calls of each use keep a sequence number in device memory, so they can be captured in a CUDA graph;
+ * the calls on one handle are collective and issued on one stream.  B2_ERR_ARG: a null pointer, size outside 1..8,
+ * rank outside [0, size), halo_cap zero or not a multiple of 16. */
+size_t b2_mailbox_bytes(size_t halo_cap);
+int b2_mailbox_create(int rank, int size, void* const* boxes_host, size_t halo_cap, b2_mailbox** out);
+int b2_mailbox_destroy(b2_mailbox* h);
 
-/* One-shot SUM all-reduce of a small vector (<= b2_peer_vec_max_bytes()) over peer memory: the array
- * Allreduce of MPIVStack._rmatvec (VStack.py:146-148) / MatrixMult.py:420-426 in the latency regime.
- * boxes_host[r] = rank r's mailbox (b2_symm_alloc of b2_peer_vec_bytes(), IPC-mapped here). */
-size_t b2_peer_vec_bytes(void);
+/* One-shot all-reduce of k <= 8 float64 scalars: the collective half of DistributedArray.dot / norm
+ * (DistributedArray.py:684-686, 714-757) and of the CGLS step scalars. */
+int b2_peer_allreduce(b2_mailbox* h, double* vals_dev, int k, int op, void* stream);
+
+/* One-shot SUM all-reduce of a small vector (<= b2_peer_vec_max_bytes()): the array Allreduce of
+ * MPIVStack._rmatvec (VStack.py:146-148) / MatrixMult.py:420-426 in the latency regime. */
 size_t b2_peer_vec_max_bytes(void);
-int b2_peer_vec_create(int rank, int size, void* const* boxes_host, b2_peer_vec** out);
-int b2_peer_vec_destroy(b2_peer_vec* h);
-int b2_peer_vec_allreduce(b2_peer_vec* h, void* buf_dev, size_t n, int dtype, void* stream);
+int b2_peer_vec_allreduce(b2_mailbox* h, void* buf_dev, size_t n, int dtype, void* stream);
 
-/* One-shot Allgather(v) over the same mailboxes (every chunk <= b2_peer_vec_max_bytes()): recv = concatenation of the
- * ranks' counts_host[r] elements.  The latency-regime replacement of the pad-to-max NCCL gather of
- * utils/_nccl.py:363-403 (e.g. the 128 KB model vector of MPIMatrixMult's single-column apply). */
-int b2_peer_vec_allgatherv(b2_peer_vec* h, const void* send, void* recv, const size_t* counts_host, int dtype,
+/* One-shot Allgather(v) (every chunk <= b2_peer_vec_max_bytes()): recv = concatenation of the ranks' counts_host[r]
+ * elements.  The latency-regime replacement of the pad-to-max NCCL gather of utils/_nccl.py:363-403 (e.g. the
+ * 128 KB model vector of MPIMatrixMult's single-column apply). */
+int b2_peer_vec_allgatherv(b2_mailbox* h, const void* send, void* recv, const size_t* counts_host, int dtype,
                            void* stream);
 
 /* ---- NCCL collectives (utils/_nccl.py:98-403, utils/_mpi.py:21-344,

@@ -35,9 +35,9 @@ def allreduce_(comm: Comm, buf: torch.Tensor, op: str = SUM) -> torch.Tensor:
     _flat(buf)
     if buf.dtype is torch.float64 and buf.numel() <= 8:
         # scalars (dot / norm / solver step lengths): one-shot all-reduce over NVLink peer memory
-        peer = comm.peer
-        if peer is not None:
-            _lib.check(_lib.lib.b2_peer_allreduce(peer, buf.data_ptr(), buf.numel(), _OPS[op], _lib.stream()),
+        mailbox = comm.mailbox
+        if mailbox is not None:
+            _lib.check(_lib.lib.b2_peer_allreduce(mailbox, buf.data_ptr(), buf.numel(), _OPS[op], _lib.stream()),
                        "b2_peer_allreduce")
             return buf
     if op in (SUM, None) and buf.dtype in (torch.float32, torch.float64) and \
@@ -46,12 +46,12 @@ def allreduce_(comm: Comm, buf: torch.Tensor, op: str = SUM) -> torch.Tensor:
         # The transport is chosen from RANK-INVARIANT data only (dtype, element count, op): a rank-local
         # property such as pointer alignment could send ranks down different paths (and the lazy, collective
         # mailbox setup) and hang the job; a mis-aligned view is staged through an aligned scratch instead.
-        # The mailbox handles keep a host-side sequence number: all calls on one communicator must be issued
+        # The mailbox keeps its sequence numbers in device memory: all calls on one communicator must be issued
         # on ONE stream (the current torch stream of the solver loop).
-        pv = comm.peer_vec
-        if pv is not None:
+        mailbox = comm.mailbox
+        if mailbox is not None:
             work = buf if buf.data_ptr() % 16 == 0 else buf.clone()
-            _lib.check(_lib.lib.b2_peer_vec_allreduce(pv, work.data_ptr(), work.numel(), _lib.code(work.dtype),
+            _lib.check(_lib.lib.b2_peer_vec_allreduce(mailbox, work.data_ptr(), work.numel(), _lib.code(work.dtype),
                                                       _lib.stream()), "b2_peer_vec_allreduce")
             if work is not buf:
                 buf.copy_(work)
@@ -84,10 +84,11 @@ def allgatherv(comm: Comm, send: torch.Tensor, counts: Sequence[int],
     arr, cmax = hit
     if cmax * send.element_size() <= _PEER_VEC_MAX:
         # latency regime: one-shot all-gather over peer memory (rank-invariant choice: counts and dtype only)
-        pv = comm.peer_vec
-        if pv is not None:
-            _lib.check(_lib.lib.b2_peer_vec_allgatherv(pv, send.data_ptr() if send.numel() else None, out.data_ptr(), arr,
-                                                       _lib.code(send.dtype), _lib.stream()), "b2_peer_vec_allgatherv")
+        mailbox = comm.mailbox
+        if mailbox is not None:
+            _lib.check(_lib.lib.b2_peer_vec_allgatherv(mailbox, send.data_ptr() if send.numel() else None,
+                                                       out.data_ptr(), arr, _lib.code(send.dtype), _lib.stream()),
+                       "b2_peer_vec_allgatherv")
             return out
     _lib.check(_lib.lib.b2_allgatherv(comm.nccl, send.data_ptr(), out.data_ptr(), arr,
                                       _lib.code(send.dtype), _lib.stream()), "b2_allgatherv")

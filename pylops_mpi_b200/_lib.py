@@ -98,9 +98,6 @@ def _load():
         "b2_kirchhoff_tables": ([vp, vp, vp, vp, sz, sz, sz, vp, sz, d, sz, sz, vp, vp], i),
         "b2_eikonal_tables": ([vp, vp, sz, sz, sz, d, d, d, vp, sz, sz, vp, vp, vp, vp], i),
         "b2_eikonal_work_bytes": ([sz, sz, sz, sz], sz),
-        "b2_halo_bytes": ([sz], sz),
-        "b2_halo_create": ([i, i, C.POINTER(vp), sz, C.POINTER(vp)], i),
-        "b2_halo_destroy": ([vp], i),
         "b2_derivative_peer": ([vp, vp, vp, vp, sz, sz, sz, sz, i, i, i, i, d, i, i, vp], i),
         "b2_first_derivative_host": ([vp, vp, vp, sz, sz, sz, sz, i, i, i, d, i, i], i),
         "b2_gemv": ([vp, vp, sz, sz, sz, vp, vp, i, i, i, vp], i),
@@ -119,14 +116,11 @@ def _load():
         "b2_ipc_get_handle": ([vp, vp], i),
         "b2_ipc_open_handle": ([vp, C.POINTER(vp)], i),
         "b2_ipc_close_handle": ([vp], i),
-        "b2_peer_slots_bytes": ([], sz),
-        "b2_peer_create": ([i, i, C.POINTER(vp), C.POINTER(vp)], i),
-        "b2_peer_destroy": ([vp], i),
+        "b2_mailbox_bytes": ([sz], sz),
+        "b2_mailbox_create": ([i, i, C.POINTER(vp), sz, C.POINTER(vp)], i),
+        "b2_mailbox_destroy": ([vp], i),
         "b2_peer_allreduce": ([vp, vp, i, i, vp], i),
-        "b2_peer_vec_bytes": ([], sz),
         "b2_peer_vec_max_bytes": ([], sz),
-        "b2_peer_vec_create": ([i, i, C.POINTER(vp), C.POINTER(vp)], i),
-        "b2_peer_vec_destroy": ([vp], i),
         "b2_peer_vec_allreduce": ([vp, vp, sz, i, vp], i),
         "b2_peer_vec_allgatherv": ([vp, vp, vp, C.POINTER(sz), i, vp], i),
         "b2_get_unique_id": ([vp], i),

@@ -135,12 +135,12 @@ class MPIFirstDerivative(MPILinearOperator):
         # fused path: halo rows are pushed / awaited INSIDE the stencil kernel over NVLink peer memory (ONE launch,
         # no NCCL, no side stream)
         if peer_ok:
-            halo = x.base_comm.halo
-            if halo is not None:
+            mailbox = x.base_comm.mailbox
+            if mailbox is not None:
                 if xr.data_ptr() % 16:        # never branch on a rank-local property: stage a mis-aligned view
                     xr = xr.clone()
-                _lib.check(_lib.lib.b2_derivative_peer(ctx, halo, xr.data_ptr(), yr.data_ptr(), nloc, ncols, row0,
-                                                       self.dims[0], self._deriv, self._kind_code, self.order,
+                _lib.check(_lib.lib.b2_derivative_peer(ctx, mailbox, xr.data_ptr(), yr.data_ptr(), nloc, ncols,
+                                                       row0, self.dims[0], self._deriv, self._kind_code, self.order,
                                                        int(self.edge), float(self.sampling), int(adjoint), code,
                                                        _lib.stream()), "b2_derivative_peer")
                 return y

@@ -319,7 +319,7 @@ class _MPISummaMatrixMult(DistributedMixIn, MPILinearOperator):
         self._kA = self._w * self._pa
         if self._bm % 32 or self._w % 8 or self._bn % 8:
             raise NotImplementedError("stationary=True needs M/Pc % 32 == 0 and 8-aligned tile extents")
-        if comm.Get_size() > 1 and comm.peer is None:
+        if comm.Get_size() > 1 and comm.mailbox is None:
             raise NotImplementedError("stationary=True needs CUDA IPC peer access between the ranks")
         self._A_full = (torch.cat(self._A_panels, dim=1) if self._pa > 1 else self._A_panels[0]).contiguous()
         Mp = self._bm * self._Pc

@@ -35,6 +35,8 @@ class Comm:
         self._group = group                     # torch.distributed group (None when size == 1)
         self._ranks = list(ranks) if ranks is not None else list(range(size))  # global ranks
         self._nccl = None                       # b2_comm handle (lazy)
+        self._mailbox = None                    # b2_mailbox handle (lazy)
+        self._mailbox_failed = False
         self._split_cache = {}
 
     # ---- mpi4py surface ------------------------------------------------------
@@ -157,32 +159,6 @@ class Comm:
             return 0, ptr.value, None
         return 1, ptr.value, ptrs
 
-    def _ipc_mailboxes(self, attr: str, nbytes_fn, create_fn):
-        """collective lazy setup of an IPC-mapped mailbox group (one symmetric buffer per rank, every
-        rank maps every peer's); returns the library handle or None when CUDA IPC is unavailable"""
-        if self._size == 1 or self._size > 8 or os.environ.get("B2_PEER_ALLREDUCE", "1") == "0":
-            return None
-        if getattr(self, attr, None) is None and not getattr(self, attr + "_failed", False):
-            from . import _lib
-            nbytes = getattr(_lib.lib, nbytes_fn)() if isinstance(nbytes_fn, str) else nbytes_fn()
-            ok, _, ptrs = self._symm_map(nbytes)
-            hnd = None
-            if ok:
-                try:
-                    boxes = (C.c_void_p * self._size)(*ptrs)
-                    hnd = C.c_void_p()
-                    if isinstance(create_fn, str):
-                        _lib.check(getattr(_lib.lib, create_fn)(self._rank, self._size, boxes, C.byref(hnd)), create_fn)
-                    else:
-                        create_fn(boxes, hnd)
-                except Exception:
-                    ok = 0
-            if min(self.allgather(ok)) == 1:      # every rank zeroed its mailbox and mapped its peers
-                setattr(self, attr, hnd)
-            else:
-                setattr(self, attr + "_failed", True)
-        return getattr(self, attr, None)
-
     def symm_alloc(self, nbytes: int):
         """COLLECTIVE: every rank allocates ``nbytes`` of IPC-mappable device memory and maps every peer's
         buffer; returns ``(my_ptr, ptrs)`` with ``ptrs[r]`` = rank r's buffer as addressable from this process
@@ -195,33 +171,35 @@ class Comm:
                                  f"failed on at least one rank")
         return ptr, ptrs
 
-    @property
-    def peer(self):
-        """b2_peer handle: mailboxes for one-shot SCALAR all-reduces over NVLink peer memory"""
-        return self._ipc_mailboxes("_peer", "b2_peer_slots_bytes", "b2_peer_create")
+    HALO_CAP = 4 << 20      # bytes per (parity, side) slot of the halo region of a mailbox
 
     @property
-    def peer_vec(self):
-        """b2_peer_vec handle: mailboxes for one-shot small-VECTOR all-reduces over peer memory"""
-        return self._ipc_mailboxes("_peer_vec", "b2_peer_vec_bytes", "b2_peer_vec_create")
-
-    HALO_CAP = int(os.environ.get("B2_HALO_CAP_BYTES", 4 << 20))   # bytes per (parity, side) slot of a halo box
-
-    @property
-    def halo(self):
-        """b2_halo handle: per-rank boxes for the halo rows the stencil kernels exchange over NVLink peer
-        memory INSIDE the kernel (one launch per apply, no NCCL); None when CUDA IPC is unavailable"""
-        hit = self.__dict__.get("_halo")
-        if hit is not None:           # hot enqueue path: no environment lookups once the boxes exist
+    def mailbox(self):
+        """b2_mailbox handle: this rank's box of IPC-mapped device memory and its mapping of every peer's box, for
+        the one-shot scalar and vector all-reduces, the all-gather and the halo exchange inside the stencil kernels
+        over NVLink peer memory.  Created collectively on first use; None for one rank, for more than 8 ranks, or
+        when the allocation or the CUDA IPC mapping fails on any rank"""
+        hit = self._mailbox
+        if hit is not None:           # hot enqueue path: no lookups once the mailbox exists
             return hit
-        if os.environ.get("B2_PEER_HALO", "1") == "0":
+        if self._size == 1 or self._size > 8 or self._mailbox_failed:
             return None
         from . import _lib
-        cap = self.HALO_CAP
+        ok, _, ptrs = self._symm_map(_lib.lib.b2_mailbox_bytes(self.HALO_CAP))
+        hnd = C.c_void_p()
+        if ok:
+            try:
+                _lib.check(_lib.lib.b2_mailbox_create(self._rank, self._size, (C.c_void_p * self._size)(*ptrs),
+                                                      self.HALO_CAP, C.byref(hnd)), "b2_mailbox_create")
+            except Exception:
+                ok = 0
+        if min(self.allgather(ok)) == 1:      # every rank zeroed its box headers and mapped its peers
+            self._mailbox = hnd
+        else:
+            self._mailbox_failed = True
+        return self._mailbox
 
-        def create(boxes, hnd):
-            _lib.check(_lib.lib.b2_halo_create(self._rank, self._size, boxes, cap, C.byref(hnd)), "b2_halo_create")
-        return self._ipc_mailboxes("_halo", lambda: _lib.lib.b2_halo_bytes(cap), create)
+    halo = peer_vec = mailbox   # earlier names of the mailbox, which bench.py reads
 
     def split_by_mask(self, mask: Sequence[int]) -> "Comm":
         """cached ``Split(color=mask[rank], key=rank)`` (DistributedArray.py:74-100)"""

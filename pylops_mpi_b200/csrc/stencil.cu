@@ -20,6 +20,7 @@
 // 64-row chunks (first design) reached 0.85 of the copy peak, 4-row chunks 1.04.
 // Algorithmic bytes: 2*sizeof(T) per element.
 #include "common.cuh"
+#include "peer.cuh"
 
 namespace {
 
@@ -43,20 +44,16 @@ struct StencilParams {
 };
 
 // ---- halo rows over NVLink PEER MEMORY inside the stencil kernel (round 2) -----------------------------------
-// Every rank owns a mailbox ("box") in IPC-mapped memory: flags + 2 parities x 2 sides of halo rows.  The first
-// column-tile CTAs of the kernel push this rank's boundary rows straight into the neighbours' boxes (16-byte P2P
+// The halo region of every rank's mailbox (peer.cuh) holds flags + 2 parities x 2 sides of halo rows.  The first
+// column-tile CTAs of the kernel push this rank's boundary rows straight into the neighbours' regions (16-byte P2P
 // stores) and publish a system-scope flag; only the CTAs that own the first / last row chunk wait for the
 // neighbour's flag, and they are scheduled LAST, so the exchange hides behind the interior rows: ONE launch per
 // apply, no NCCL call, no side stream (the reference does 2-4 add_ghost_cells exchanges per apply,
-// FirstDerivative.py:221-247, 276-319).  Sequence number and tickets live in device memory (graph-capturable).
-constexpr size_t HALO_HDR = 256;
-struct HaloBox {
-  unsigned long long flag[2][2];   // [parity][side]: side 0 = rows from rank-1, side 1 = rows from rank+1
-};
+// FirstDerivative.py:221-247, 276-319).
 struct HaloPeer {
-  char* mine;        // this rank's box (local mapping)
-  char* prev;        // rank-1's box (peer mapping) or nullptr
-  char* next;        // rank+1's box or nullptr
+  char* mine;        // this rank's halo region (local mapping)
+  char* prev;        // rank-1's halo region (peer mapping) or nullptr
+  char* next;        // rank+1's halo region or nullptr
   size_t cap;        // bytes per (parity, side) slot
   unsigned long long* seq;   // device: number of completed exchanges
   unsigned int* tickets;     // device: [0] push ticket, [1] edge ticket, [2] push-done marker
@@ -64,14 +61,6 @@ struct HaloPeer {
 };
 __device__ __forceinline__ char* halo_slot(char* box, size_t cap, int par, int side) {
   return box + HALO_HDR + ((size_t)par * 2 + side) * cap;
-}
-__device__ __forceinline__ void st_release_sys_u64(unsigned long long* p, unsigned long long v) {
-  asm volatile("st.release.sys.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
-}
-__device__ __forceinline__ unsigned long long ld_acquire_sys_u64(const unsigned long long* p) {
-  unsigned long long v;
-  asm volatile("ld.acquire.sys.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
-  return v;
 }
 
 // forward taps of global row i (offsets -2..2), before the 1/sampling scale
@@ -189,8 +178,8 @@ stencil_vec_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restri
       rc = (e == 0) ? 0 : n_rc - n_edge + e;
       edge_cta = true;
     }
-    seq = *reinterpret_cast<volatile unsigned long long*>(hp.seq) + 1ull;
-    const int par = (int)(seq & 1ull);
+    seq = peer_next_seq(hp.seq);
+    const int par = peer_parity(seq);
     if (j == 0) {
       // push my boundary rows into the neighbours' boxes (this CTA's column tile)
       if (cv < ncv) {
@@ -210,8 +199,8 @@ stencil_vec_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restri
         const unsigned int t = atomicAdd(&hp.tickets[0], 1u);
         if (t == (unsigned int)n_ct - 1u) {      // every column tile of this rank is on its way: publish
           __threadfence_system();
-          if (hp.prev) st_release_sys_u64(&reinterpret_cast<HaloBox*>(hp.prev)->flag[par][1], seq);
-          if (hp.next) st_release_sys_u64(&reinterpret_cast<HaloBox*>(hp.next)->flag[par][0], seq);
+          if (hp.prev) st_release_sys(&reinterpret_cast<HaloBox*>(hp.prev)->flag[par][1], seq);
+          if (hp.next) st_release_sys(&reinterpret_cast<HaloBox*>(hp.next)->flag[par][0], seq);
           *reinterpret_cast<volatile unsigned int*>(&hp.tickets[2]) = 1u;
         }
       }
@@ -222,14 +211,14 @@ stencil_vec_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restri
   const long long r0 = rc * ST_ROWS;
   const long long r1 = (r0 + ST_ROWS < p.nloc) ? r0 + ST_ROWS : p.nloc;
   if constexpr (PEER) {
-    const int par = (int)(seq & 1ull);
+    const int par = peer_parity(seq);
     const bool needs_lo = hp.prev && p.n_lo > 0 && r0 - R < 0;
     const bool needs_hi = hp.next && p.n_hi > 0 && r1 - 1 + R >= p.nloc;
     if (needs_lo || needs_hi) {
       if (threadIdx.x == 0) {
         const HaloBox* me = reinterpret_cast<const HaloBox*>(hp.mine);
-        if (needs_lo) while (ld_acquire_sys_u64(&me->flag[par][0]) < seq) { }
-        if (needs_hi) while (ld_acquire_sys_u64(&me->flag[par][1]) < seq) { }
+        if (needs_lo) while (ld_acquire_sys(&me->flag[par][0]) < seq) { }
+        if (needs_hi) while (ld_acquire_sys(&me->flag[par][1]) < seq) { }
       }
       __syncthreads();
     }
@@ -316,10 +305,10 @@ stencil_vec_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restri
       if (threadIdx.x == 0) {
         const unsigned int t = atomicAdd(&hp.tickets[1], 1u);
         if (t == (unsigned int)(n_edge * n_ct) - 1u) {
-          const int par = (int)(seq & 1ull);
+          const int par = peer_parity(seq);
           const HaloBox* me = reinterpret_cast<const HaloBox*>(hp.mine);
-          if (hp.prev) while (ld_acquire_sys_u64(&me->flag[par][0]) < seq) { }
-          if (hp.next) while (ld_acquire_sys_u64(&me->flag[par][1]) < seq) { }
+          if (hp.prev) while (ld_acquire_sys(&me->flag[par][0]) < seq) { }
+          if (hp.next) while (ld_acquire_sys(&me->flag[par][1]) < seq) { }
           while (*reinterpret_cast<volatile unsigned int*>(&hp.tickets[2]) == 0u) { }
           hp.tickets[0] = 0u;
           hp.tickets[1] = 0u;
@@ -542,58 +531,10 @@ extern "C" int b2_second_derivative(b2_ctx* ctx, const void* x, void* y, const v
                   FdOp{2, kind, 0, edge, adjoint}, sampling, dtype, stream);
 }
 
-// ---- peer-memory halo handle ------------------------------------------------------------------------------------
-struct b2_halo {
-  int rank, size;
-  char* box[3];               // [0] rank-1's box (peer mapping or NULL), [1] mine, [2] rank+1's
-  size_t cap;
-  unsigned long long* seq;    // device
-  unsigned int* tickets;      // device, 4 uints
-};
-
-extern "C" size_t b2_halo_bytes(size_t cap_bytes) { return HALO_HDR + 4 * cap_bytes; }
-
-// boxes_host[r]: rank r's box as mapped in THIS process (own pointer for r == rank; only rank +/- 1 are used).
-// Zeroes this rank's flags: callers barrier on the host between creation and the first apply.
-extern "C" int b2_halo_create(int rank, int size, void* const* boxes_host, size_t cap_bytes, b2_halo** out) {
-  if (!out || !boxes_host || size < 1 || rank < 0 || rank >= size || cap_bytes == 0 || (cap_bytes % 16)) return B2_ERR_ARG;
-  b2_halo* h = new b2_halo();
-  h->rank = rank;
-  h->size = size;
-  h->cap = cap_bytes;
-  h->box[0] = rank > 0 ? (char*)boxes_host[rank - 1] : nullptr;
-  h->box[1] = (char*)boxes_host[rank];
-  h->box[2] = rank < size - 1 ? (char*)boxes_host[rank + 1] : nullptr;
-  h->seq = nullptr;
-  h->tickets = nullptr;
-  cudaError_t e = cudaMalloc((void**)&h->seq, sizeof(unsigned long long));
-  if (e == cudaSuccess) e = cudaMalloc((void**)&h->tickets, 4 * sizeof(unsigned int));
-  if (e == cudaSuccess) e = cudaMemset(h->seq, 0, sizeof(unsigned long long));
-  if (e == cudaSuccess) e = cudaMemset(h->tickets, 0, 4 * sizeof(unsigned int));
-  if (e == cudaSuccess) e = cudaMemset(h->box[1], 0, HALO_HDR);
-  if (e == cudaSuccess) e = cudaDeviceSynchronize();
-  if (e != cudaSuccess) {
-    if (h->seq) cudaFree(h->seq);
-    if (h->tickets) cudaFree(h->tickets);
-    delete h;
-    return (int)e;
-  }
-  *out = h;
-  return B2_OK;
-}
-
-extern "C" int b2_halo_destroy(b2_halo* h) {
-  if (!h) return B2_OK;
-  if (h->seq) cudaFree(h->seq);
-  if (h->tickets) cudaFree(h->tickets);
-  delete h;
-  return B2_OK;
-}
-
 // One-launch distributed stencil: deriv = 1 (MPIFirstDerivative) or 2 (MPISecondDerivative); the halo rows
-// travel through the peer boxes inside the kernel.  Collective over the ranks of the handle (same call
-// sequence on every rank, one stream); every rank must own at least max(need_lo, need_hi) rows.
-extern "C" int b2_derivative_peer(b2_ctx* ctx, b2_halo* h, const void* x, void* y, size_t nrows_local, size_t ncols,
+// travel through the halo regions of the mailboxes inside the kernel.  Collective over the ranks of the handle
+// (same call sequence on every rank, one stream); every rank must own at least max(need_lo, need_hi) rows.
+extern "C" int b2_derivative_peer(b2_ctx* ctx, b2_mailbox* h, const void* x, void* y, size_t nrows_local, size_t ncols,
                                   size_t row0, size_t nrows_global, int deriv, int kind, int order, int edge,
                                   double sampling, int adjoint, int dtype, void* stream) {
   if (!ctx || !h || !x || !y || (deriv != 1 && deriv != 2)) return B2_ERR_ARG;
@@ -605,20 +546,21 @@ extern "C" int b2_derivative_peer(b2_ctx* ctx, b2_halo* h, const void* x, void* 
   const size_t esz = b2_dtype_size(dtype), V = 16 / esz;
   if ((long long)nrows_local < (need_lo > need_hi ? need_lo : need_hi)) return B2_ERR_HALO;
   if (ncols % V || ncols / V < 8 || !b2_aligned16(x) || !b2_aligned16(y)) return B2_ERR_ALIGN;
-  if ((size_t)(need_lo > need_hi ? need_lo : need_hi) * ncols * esz > h->cap) return B2_ERR_WORKSPACE;
-  const int n_lo = h->box[0] ? need_lo : 0, n_hi = h->box[2] ? need_hi : 0;
+  if ((size_t)(need_lo > need_hi ? need_lo : need_hi) * ncols * esz > h->halo_cap) return B2_ERR_WORKSPACE;
+  const bool has_prev = h->rank > 0, has_next = h->rank < h->size - 1;
   StencilParams p;
-  rc = b2_fd_build_params(&p, n_lo, n_hi, nrows_local, ncols, row0, nrows_global, op, sampling);
+  rc = b2_fd_build_params(&p, has_prev ? need_lo : 0, has_next ? need_hi : 0, nrows_local, ncols, row0,
+                          nrows_global, op, sampling);
   if (rc) return rc;
   HaloPeer hp;
-  hp.mine = h->box[1];
-  hp.prev = h->box[0];
-  hp.next = h->box[2];
-  hp.cap = h->cap;
-  hp.seq = h->seq;
-  hp.tickets = h->tickets;
-  hp.send_lo = h->box[0] ? need_hi : 0;    // rank-1 needs my first need_hi rows as ITS hi halo
-  hp.send_hi = h->box[2] ? need_lo : 0;    // rank+1 needs my last need_lo rows as ITS lo halo
+  hp.mine = h->box[h->rank] + MB_HALO_OFF;
+  hp.prev = has_prev ? h->box[h->rank - 1] + MB_HALO_OFF : nullptr;
+  hp.next = has_next ? h->box[h->rank + 1] + MB_HALO_OFF : nullptr;
+  hp.cap = h->halo_cap;
+  hp.seq = &h->counters->seq[MB_SEQ_HALO];
+  hp.tickets = h->counters->tickets;
+  hp.send_lo = has_prev ? need_hi : 0;    // rank-1 needs my first need_hi rows as ITS hi halo
+  hp.send_hi = has_next ? need_lo : 0;    // rank+1 needs my last need_lo rows as ITS lo halo
   cudaStream_t st = (cudaStream_t)stream;
   return b2_dispatch_real(dtype, [&](auto t) { return launch_vec<decltype(t), true>(x, y, nullptr, nullptr, p, hp, st); });
 }

@@ -52,9 +52,9 @@ class MPIFredholm1(MPILinearOperator):
         self.usematmul = usematmul
         # fused=True: product + all-gather in ONE kernel over NVLink peer memory (IPC-mapped output
         # arenas); fused=False: product kernel, then one NCCL Allgatherv in place
-        # fused=None (default): on when CUDA IPC peer mapping works between the ranks (probed by comm.peer)
+        # fused=None (default): on when CUDA IPC peer mapping works between the ranks (probed by comm.mailbox)
         if fused is None:
-            fused = base_comm.Get_size() > 1 and base_comm.peer is not None
+            fused = base_comm.Get_size() > 1 and base_comm.mailbox is not None
         self._fused = bool(fused) and base_comm.Get_size() > 1 and not self._scatter_data
         if self._fused:
             esz = torch.empty(0, dtype=self._tdtype).element_size()

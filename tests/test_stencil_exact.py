@@ -381,10 +381,10 @@ def test_entry_point_argument_errors(L):
         if rc != want:
             bad.append(("b2_derivative_axis", change, rc, want))
     cap = 32 * 8
-    box = torch.zeros(L.lib.b2_halo_bytes(cap), dtype=torch.uint8, device="cuda")
+    box = torch.zeros(L.lib.b2_mailbox_bytes(cap), dtype=torch.uint8, device="cuda")
     boxes = (C.c_void_p * 1)(box.data_ptr())
     h = C.c_void_p()
-    L.check(L.lib.b2_halo_create(0, 1, boxes, cap, C.byref(h)), "b2_halo_create")
+    L.check(L.lib.b2_mailbox_create(0, 1, boxes, cap, C.byref(h)), "b2_mailbox_create")
     try:
         for change, want in PEER_ARGS:
             a = args(PEER, change, ["ctx", "h", "x", "y", "nloc", "ncols", "row0", "nglob", "deriv", "kind", "order",
@@ -394,7 +394,7 @@ def test_entry_point_argument_errors(L):
             if rc != want:
                 bad.append(("b2_derivative_peer", change, rc, want))
     finally:
-        L.check(L.lib.b2_halo_destroy(h), "b2_halo_destroy")
+        L.check(L.lib.b2_mailbox_destroy(h), "b2_mailbox_destroy")
     xh, yh = np.ones((8, 32)), np.zeros((8, 32))
     ptr.update(x=xh.ctypes.data, y=yh.ctypes.data)
     for change, want in HOST_ARGS:
