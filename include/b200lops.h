@@ -43,7 +43,11 @@ enum { B2_OK = 0, B2_ERR_DTYPE = 2001, B2_ERR_ARG = 2002, B2_ERR_HALO = 2003,
 
 /* per-device context: SM count + the reduction workspace (per-CTA partials, ticket counter) shared by b2_dot /
  * b2_norm_partial / b2_dot_multi / b2_sparse_update / the transposed b2_gemv.  Calls that use the workspace must be
- * stream-ordered with respect to each other: use one b2_ctx per stream that issues reductions concurrently. */
+ * stream-ordered with respect to each other: use one b2_ctx per stream that issues reductions concurrently.
+ * Every workspace address stays valid until b2_ctx_destroy, so a CUDA graph may capture calls that use it: the
+ * transposed b2_gemv's chunk-partial scratch only grows, keeps each buffer it outgrows until b2_ctx_destroy and never
+ * synchronises; when it would have to grow while the stream is capturing, b2_gemv returns B2_ERR_WORKSPACE and
+ * enqueues nothing (run the call once eagerly before capturing it).  Destroy the graphs before the context. */
 typedef struct b2_ctx b2_ctx;
 typedef struct b2_comm b2_comm;          /* one NCCL communicator (world, mask group, grid row / col) */
 typedef struct b2_mailbox b2_mailbox;    /* peer-memory mailboxes: one-shot collectives and the fused halo exchange */
@@ -296,7 +300,8 @@ int b2_first_derivative_host(b2_ctx* ctx, const void* x_host, void* y_host, size
  *      MPIVStack, BlockDiag.py:127-129,139-141; VStack.py:129-131,144-145; and
  *      the M==1 tile product of MPIMatrixMult, MatrixMult.py:366-370,670) ----
  * y[m or n] = op(A[m x n, row-major, leading dim lda]) x ; dtype_a in
- * {F32,F64,C64,C128,BF16}; x,y have dtype_xy (BF16 A pairs with F32 x/y). */
+ * {F32,F64,C64,C128,BF16}; x,y have dtype_xy (BF16 A pairs with F32 x/y).  Any m and n; op T / H with more than
+ * 128 rows uses the context's chunk-partial scratch (B2_ERR_WORKSPACE rule above). */
 int b2_gemv(b2_ctx* ctx, const void* A, size_t lda, size_t m, size_t n, const void* x, void* y,
             int op, int dtype_a, int dtype_xy, void* stream);
 
@@ -321,7 +326,7 @@ int b2_gemm_bf16_seg(b2_ctx* ctx, const void* A, size_t lda, const void* B, size
 int b2_sum_slots(b2_ctx* ctx, const float* slots, size_t slot_stride, int nslots, size_t ld_in, float* out,
                  size_t rows, size_t cols, void* stream);
 /* generic SIMT tile product for the dtypes tensor cores do not serve
- * (f32/f64/c64/c128 parity cases of tests/test_matrixmult.py) */
+ * (f32/f64/c64/c128 parity cases of tests/test_matrixmult.py); any m, n, k, leading dimensions >= the row lengths */
 int b2_gemm(b2_ctx* ctx, const void* A, size_t lda, const void* B, size_t ldb, void* C, size_t ldc,
             size_t m, size_t n, size_t k, int op_a, int accumulate, int dtype, void* stream);
 

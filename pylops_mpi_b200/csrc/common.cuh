@@ -20,14 +20,18 @@
     if (e__ != cudaSuccess) return (int)e__;           \
   } while (0)
 
+constexpr int B2_GEMV_RETIRED_MAX = 48;   // the gemv scratch doubles as it grows: 48 retired buffers are never reached
+
 struct b2_ctx {
   int device;
   int sm_count;
   // reduction workspace: partial sums + ticket counters (device memory)
   double* red_partials;     // B2_RED_MAX_BLOCKS * B2_RED_MAX_OUT doubles
   unsigned int* tickets;    // B2_TICKETS uints, zero between launches
-  float* gemv_partials;     // scratch for transposed gemv (bytes = gemv_partials_bytes)
+  float* gemv_partials;     // scratch for transposed gemv (bytes = gemv_partials_bytes); grows, never shrinks
   size_t gemv_partials_bytes;
+  float* gemv_retired[B2_GEMV_RETIRED_MAX];  // buffers gemv_partials outgrew, freed by b2_ctx_destroy
+  int gemv_retired_n;
   // host-buffer pipeline (b2_first_derivative_host)
   void* pipe_buf[3][2];     // [slot][in/out]
   size_t pipe_bytes;

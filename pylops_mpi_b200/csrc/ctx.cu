@@ -53,6 +53,7 @@ extern "C" int b2_ctx_destroy(b2_ctx* c) {
   if (c->red_partials) cudaFree(c->red_partials);
   if (c->tickets) cudaFree(c->tickets);
   if (c->gemv_partials) cudaFree(c->gemv_partials);
+  for (int i = 0; i < c->gemv_retired_n; ++i) cudaFree(c->gemv_retired[i]);
   for (int s = 0; s < 3; ++s) {
     for (int k = 0; k < 2; ++k)
       if (c->pipe_buf[s][k]) cudaFree(c->pipe_buf[s][k]);

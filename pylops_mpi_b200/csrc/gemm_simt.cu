@@ -110,23 +110,30 @@ gemm_simt_kernel(const T* __restrict__ A, size_t lda, size_t sA, const T* __rest
 }
 
 // FUSED: the epilogue also stores to the peers (b2_batched_gemm_allgather).  That entry point does not check the grid
-// here: an empty or too tall grid is left to the launch, which returns CUDA's error code
+// here: an empty or too tall grid is left to the launch, which returns CUDA's error code.  Otherwise more than
+// B2_GRID_Y_MAX row tiles are issued in groups of output rows, one launch each: a group starts at row r0 of C and of
+// op(A), i.e. row r0 of A for op N and column r0 for op T / H
 template <typename T, bool FUSED = false>
 int launch_gemm(const void* A, size_t lda, size_t sA, const void* B, size_t ldb, size_t sB,
                 void* C, size_t ldc, size_t sC, size_t m, size_t n, size_t k, size_t batch,
                 int op_a, bool accumulate, cudaStream_t st, const PeerDst& peers = PeerDst{}) {
-  dim3 grid((unsigned)((n + BN - 1) / BN), (unsigned)((m + BM - 1) / BM), (unsigned)batch);
-  if (!FUSED) {
-    if (m == 0 || n == 0 || batch == 0) return B2_OK;
-    if (batch > 65535 || grid.y > 65535u) return B2_ERR_ARG;
-  }
   const bool conj = (op_a == B2_OP_H);
-  if (op_a == B2_OP_N)
-    gemm_simt_kernel<T, false, FUSED><<<grid, 256, 0, st>>>((const T*)A, lda, sA, (const T*)B, ldb, sB, (T*)C, ldc, sC, m, n, k, false, accumulate, peers);
-  else
-    gemm_simt_kernel<T, true, FUSED><<<grid, 256, 0, st>>>((const T*)A, lda, sA, (const T*)B, ldb, sB, (T*)C, ldc, sC, m, n, k, conj, accumulate, peers);
-  B2_LAUNCH_CHECK();
-  return B2_OK;
+  auto launch = [&](size_t r0, size_t rows) {
+    const dim3 grid((unsigned)((n + BN - 1) / BN), (unsigned)((rows + BM - 1) / BM), (unsigned)batch);
+    T* c = (T*)C + r0 * ldc;
+    if (op_a == B2_OP_N)
+      gemm_simt_kernel<T, false, FUSED><<<grid, 256, 0, st>>>((const T*)A + r0 * lda, lda, sA, (const T*)B, ldb, sB, c, ldc, sC, rows, n, k, false, accumulate, peers);
+    else
+      gemm_simt_kernel<T, true, FUSED><<<grid, 256, 0, st>>>((const T*)A + r0, lda, sA, (const T*)B, ldb, sB, c, ldc, sC, rows, n, k, conj, accumulate, peers);
+  };
+  if (FUSED) {
+    launch(0, m);
+    B2_LAUNCH_CHECK();
+    return B2_OK;
+  }
+  if (m == 0 || n == 0 || batch == 0) return B2_OK;
+  if (batch > 65535) return B2_ERR_ARG;
+  return b2_launch_groups(m, B2_GRID_Y_MAX * BM, launch);
 }
 
 int dispatch(const void* A, size_t lda, size_t sA, const void* B, size_t ldb, size_t sB, void* C,

@@ -10,6 +10,7 @@
 //  * op = T/H: one lane per 16-byte column vector, warps stride over the rows of a
 //            row chunk, CTA-level smem fold, chunk partials folded in chunk order
 //            by the last CTA of each column tile (deterministic, no atomics on y).
+#include <limits.h>
 #include "common.cuh"
 
 namespace {
@@ -210,62 +211,71 @@ gemv_n_split_kernel(const TA* __restrict__ A, size_t lda, size_t m, size_t n,
 
 // -------------------------------------------------------------------------
 // op = T / H : y_j = sum_i op(A_ij) x_i
-// grid = (column tiles, row chunks); CTA = 8 warps; lane <-> 16-byte column vector
+// grid = (column tiles, row chunks of `rows` rows); CTA = 8 warps; lane <-> 16-byte column vector
 // -------------------------------------------------------------------------
 constexpr int GT_WARPS = 8;
-constexpr int GT_ROWS = 128;   // rows per chunk
+constexpr size_t GT_ROWS = 128;   // rows per chunk while m fits in B2_GRID_Y_MAX chunks; a multiple of it beyond
 
-template <typename TA, bool VEC>
+// TALL: chunks of `rows` rows, a multiple of GT_ROWS (m > B2_GRID_Y_MAX * GT_ROWS); otherwise chunks of GT_ROWS rows
+template <typename TA, bool VEC, bool TALL>
 __global__ void __launch_bounds__(GT_WARPS * 32)
 gemv_t_kernel(const TA* __restrict__ A, size_t lda, size_t m, size_t n,
               const typename ElemTraits<TA>::X* __restrict__ x,
               typename ElemTraits<TA>::X* __restrict__ y,
               typename ElemTraits<TA>::Acc* __restrict__ partials,
-              unsigned int* __restrict__ tickets, bool conj) {
+              unsigned int* __restrict__ tickets, size_t rows, bool conj) {
   using Tr = ElemTraits<TA>;
   using Acc = typename Tr::Acc;
   constexpr int V = VEC ? Tr::V : 1;
   constexpr int TILE = 32 * V;   // columns per CTA
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const size_t col0 = (size_t)blockIdx.x * TILE + (size_t)lane * V;
-  const size_t r0 = (size_t)blockIdx.y * GT_ROWS;
-  const size_t r1 = (r0 + GT_ROWS < m) ? r0 + GT_ROWS : m;
   Acc acc[V];
 #pragma unroll
   for (int e = 0; e < V; ++e) acc[e] = Tr::zero();
-  if (VEC) {
-    if (col0 + V <= n) {
-      size_t i = r0 + warp;
-      // 4 rows in flight per warp
-      for (; i + 3 * GT_WARPS < r1; i += 4 * GT_WARPS) {
-        AVec<TA> av[4];
-        typename Tr::X xv[4];
+  // rows [r0, r1) of the chunk, r1 - r0 <= GT_ROWS: each lane adds its rows in ascending order
+  auto add_rows = [&](const size_t r0, const size_t r1) {
+    if (VEC) {
+      if (col0 + V <= n) {
+        size_t i = r0 + warp;
+        // 4 rows in flight per warp
+        for (; i + 3 * GT_WARPS < r1; i += 4 * GT_WARPS) {
+          AVec<TA> av[4];
+          typename Tr::X xv[4];
 #pragma unroll
-        for (int u = 0; u < 4; ++u) av[u] = load_a(A + (i + u * GT_WARPS) * lda + col0);
+          for (int u = 0; u < 4; ++u) av[u] = load_a(A + (i + u * GT_WARPS) * lda + col0);
 #pragma unroll
-        for (int u = 0; u < 4; ++u) xv[u] = ldg_t(x + i + u * GT_WARPS);
+          for (int u = 0; u < 4; ++u) xv[u] = ldg_t(x + i + u * GT_WARPS);
 #pragma unroll
-        for (int u = 0; u < 4; ++u)
+          for (int u = 0; u < 4; ++u)
 #pragma unroll
-          for (int e = 0; e < V; ++e) Tr::fma_(acc[e], av[u].v[e], xv[u], conj);
-      }
-      for (; i < r1; i += GT_WARPS) {
-        AVec<TA> av = load_a(A + i * lda + col0);
-        typename Tr::X xv = ldg_t(x + i);
+            for (int e = 0; e < V; ++e) Tr::fma_(acc[e], av[u].v[e], xv[u], conj);
+        }
+        for (; i < r1; i += GT_WARPS) {
+          AVec<TA> av = load_a(A + i * lda + col0);
+          typename Tr::X xv = ldg_t(x + i);
 #pragma unroll
-        for (int e = 0; e < V; ++e) Tr::fma_(acc[e], av.v[e], xv, conj);
+          for (int e = 0; e < V; ++e) Tr::fma_(acc[e], av.v[e], xv, conj);
+        }
+      } else {
+        for (size_t i = r0 + warp; i < r1; i += GT_WARPS) {
+          typename Tr::X xv = x[i];
+#pragma unroll
+          for (int e = 0; e < V; ++e)
+            if (col0 + e < n) Tr::fma_(acc[e], A[i * lda + col0 + e], xv, conj);
+        }
       }
     } else {
-      for (size_t i = r0 + warp; i < r1; i += GT_WARPS) {
-        typename Tr::X xv = x[i];
-#pragma unroll
-        for (int e = 0; e < V; ++e)
-          if (col0 + e < n) Tr::fma_(acc[e], A[i * lda + col0 + e], xv, conj);
-      }
+      if (col0 < n)
+        for (size_t i = r0 + warp; i < r1; i += GT_WARPS) Tr::fma_(acc[0], A[i * lda + col0], x[i], conj);
     }
-  } else {
-    if (col0 < n)
-      for (size_t i = r0 + warp; i < r1; i += GT_WARPS) Tr::fma_(acc[0], A[i * lda + col0], x[i], conj);
+  };
+  if (!TALL) {
+    const size_t c0 = (size_t)blockIdx.y * GT_ROWS;
+    add_rows(c0, (c0 + GT_ROWS < m) ? c0 + GT_ROWS : m);
+  } else {   // the taller chunk in slices of GT_ROWS rows
+    const size_t c0 = (size_t)blockIdx.y * rows, c1 = (c0 + rows < m) ? c0 + rows : m;
+    for (size_t r0 = c0; r0 < c1; r0 += GT_ROWS) add_rows(r0, (r0 + GT_ROWS < c1) ? r0 + GT_ROWS : c1);
   }
   // fold the 8 warps through shared memory (fixed order)
   __shared__ Acc smem[GT_WARPS][32 * (VEC ? Tr::V : 1)];
@@ -307,6 +317,24 @@ gemv_t_kernel(const TA* __restrict__ A, size_t lda, size_t m, size_t n,
 }
 
 
+// The chunk partials of the transposed gemv only grow (to at least twice their size), and a buffer they outgrow stays
+// allocated until b2_ctx_destroy: an address a CUDA graph captured stays valid, and work still in flight on the old
+// buffer needs no synchronisation.  Nothing is allocated while the stream is capturing: B2_ERR_WORKSPACE.
+int reserve_gemv_partials(b2_ctx* ctx, size_t need, cudaStream_t st) {
+  if (need <= ctx->gemv_partials_bytes) return B2_OK;
+  cudaStreamCaptureStatus capturing;
+  B2_CUDA(cudaStreamIsCapturing(st, &capturing));
+  if (capturing != cudaStreamCaptureStatusNone) return B2_ERR_WORKSPACE;
+  if (ctx->gemv_partials && ctx->gemv_retired_n == B2_GEMV_RETIRED_MAX) return B2_ERR_WORKSPACE;
+  const size_t bytes = need > 2 * ctx->gemv_partials_bytes ? need : 2 * ctx->gemv_partials_bytes;
+  float* p = nullptr;
+  B2_CUDA(cudaMalloc((void**)&p, bytes));
+  if (ctx->gemv_partials) ctx->gemv_retired[ctx->gemv_retired_n++] = ctx->gemv_partials;
+  ctx->gemv_partials = p;
+  ctx->gemv_partials_bytes = bytes;
+  return B2_OK;
+}
+
 template <typename TA>
 int launch_gemv(b2_ctx* ctx, const void* A, size_t lda, size_t m, size_t n, const void* x,
                 void* y, int op, cudaStream_t st) {
@@ -334,32 +362,29 @@ int launch_gemv(b2_ctx* ctx, const void* A, size_t lda, size_t m, size_t n, cons
   }
   if (n == 0) return B2_OK;
   const bool conj = (op == B2_OP_H);
-  const int tile = 32 * (vec ? V : 1);
+  const size_t tile = 32 * (vec ? V : 1);
   const size_t ntiles = (n + tile - 1) / tile;
-  size_t nchunks = (m + GT_ROWS - 1) / GT_ROWS;
-  if (nchunks < 1) nchunks = 1;
-  if (ntiles > (size_t)B2_TICKETS) return B2_ERR_WORKSPACE;
-  if (nchunks > 65535) return B2_ERR_ARG;
-  const size_t need = nchunks * n * sizeof(Acc);
-  if (nchunks > 1 && need > ctx->gemv_partials_bytes) {
-    // grow scratch (stream-ordered would be nicer; this happens once per shape class)
-    B2_CUDA(cudaStreamSynchronize(st));
-    if (ctx->gemv_partials) B2_CUDA(cudaFree(ctx->gemv_partials));
-    ctx->gemv_partials = nullptr;
-    ctx->gemv_partials_bytes = 0;
-    B2_CUDA(cudaMalloc((void**)&ctx->gemv_partials, need));
-    ctx->gemv_partials_bytes = need;
+  // m >= 1 here.  Chunks of GT_ROWS rows, taller ones once m needs more than B2_GRID_Y_MAX of them
+  const size_t rows = GT_ROWS * ((m + GT_ROWS * B2_GRID_Y_MAX - 1) / (GT_ROWS * B2_GRID_Y_MAX));
+  const size_t nchunks = (m + rows - 1) / rows;
+  // with several chunks the column tiles take tickets (ctx->tickets[64 ..]; slot 0 is the reduction ticket) and
+  // are issued in groups of at most that many tiles, one launch per group, each group reusing the tickets and the
+  // chunk partials of the previous one (stream order); one chunk needs neither
+  const size_t per_launch = nchunks > 1 ? (size_t)(B2_TICKETS - 64) : (size_t)INT_MAX;
+  if (nchunks > 1) {
+    const size_t group_cols = n < per_launch * tile ? n : per_launch * tile;
+    const int rc = reserve_gemv_partials(ctx, nchunks * group_cols * sizeof(Acc), st);
+    if (rc) return rc;
   }
-  dim3 grid((unsigned)ntiles, (unsigned)nchunks);
-  // tickets for gemv live after the first 64 slots (slot 0 is the reduction ticket)
   unsigned int* tk = ctx->tickets + 64;
-  if (ntiles + 64 > (size_t)B2_TICKETS) return B2_ERR_WORKSPACE;
-  if (vec)
-    gemv_t_kernel<TA, true><<<grid, GT_WARPS * 32, 0, st>>>((const TA*)A, lda, m, n, (const X*)x, (X*)y, (Acc*)ctx->gemv_partials, tk, conj);
-  else
-    gemv_t_kernel<TA, false><<<grid, GT_WARPS * 32, 0, st>>>((const TA*)A, lda, m, n, (const X*)x, (X*)y, (Acc*)ctx->gemv_partials, tk, conj);
-  B2_LAUNCH_CHECK();
-  return B2_OK;
+  return b2_launch_groups(ntiles, per_launch, [&](size_t t0, size_t nt) {
+    const size_t c0 = t0 * tile, nc = n - c0 < nt * tile ? n - c0 : nt * tile;
+    const dim3 grid((unsigned)nt, (unsigned)nchunks);
+    const auto kernel = vec ? (rows == GT_ROWS ? gemv_t_kernel<TA, true, false> : gemv_t_kernel<TA, true, true>)
+                            : (rows == GT_ROWS ? gemv_t_kernel<TA, false, false> : gemv_t_kernel<TA, false, true>);
+    kernel<<<grid, GT_WARPS * 32, 0, st>>>((const TA*)A + c0, lda, m, nc, (const X*)x, (X*)y + c0,
+                                           (Acc*)ctx->gemv_partials, tk, rows, conj);
+  });
 }
 
 }  // namespace
