@@ -12,6 +12,7 @@ MatrixMult.py:742-763 into a plain column broadcast.
 """
 from __future__ import annotations
 
+import ctypes as C
 import math
 from typing import Tuple
 
@@ -97,7 +98,6 @@ def _xdtype(adt: torch.dtype) -> torch.dtype:
 
 def _cast_bf16(X: torch.Tensor) -> torch.Tensor:
     """float32 (k x ncol, contiguous) -> bfloat16 through the library's cast kernel (no eager torch pass)"""
-    import ctypes as C
     if X.dtype is not torch.float32 or not X.is_contiguous():
         return X.to(torch.bfloat16)
     out = torch.empty(X.shape, dtype=torch.bfloat16, device=X.device)
@@ -292,10 +292,16 @@ class _MPISummaMatrixMult(DistributedMixIn, MPILinearOperator):
         MPILinearOperator.__init__(self, shape=shape, dtype=_lib.numpy_dtype(_xdtype(A.dtype)),
                                    base_comm=base_comm)
         self._side = None
+        # local shapes of the output tiles of every rank, forward [0] and adjoint [1]
+        self._y_shapes = (self._tile_shapes(self._bn, self.N), self._tile_shapes(self._w * self._px, self.K))
         if self._replicate:
             self._build_replicas()
         if self._stationary:
             self._setup_stationary()
+        # the function, not a bound method: a reference cycle would keep the tiles alive after the operator is dropped
+        self._product = (_MPISummaMatrixMult._product_stationary if self._stationary else
+                         _MPISummaMatrixMult._product_replicated if self._replicate else
+                         _MPISummaMatrixMult._product_summa)
 
     # ---- stationary-A mode: A never moves; X / Y panels are all-gathered, partial products reduce-scattered -------
     def _setup_stationary(self):
@@ -309,7 +315,6 @@ class _MPISummaMatrixMult(DistributedMixIn, MPILinearOperator):
           adjoint  the same with A^H: gather Y along the grid row, one product per A panel, staging at rank (r, c).
         Two flag barriers per apply (peer-memory mailbox kernels); ~4x fewer NVLink bytes than broadcasting A at
         M = 4096 and no replication of A (cf. ``replicate=True``)."""
-        import ctypes as C
         comm = self.base_comm
         A0 = self._A_panels[0]
         if A0.dtype is not torch.bfloat16:
@@ -337,21 +342,13 @@ class _MPISummaMatrixMult(DistributedMixIn, MPILinearOperator):
         have completed"""
         allreduce_(self.base_comm, self._st_flag, SUM)
 
-    def _apply_stationary(self, x: DistributedArray, adjoint: bool) -> DistributedArray:
-        import ctypes as C
+    def _product_stationary(self, x_block: torch.Tensor, Y: torch.Tensor, adjoint: bool):
         lib, ctx, st = _lib.lib, _lib.ctx(), _lib.stream()
         Pr, Pc, pa, px, w = self._Pr, self._Pc, self._pa, self._px, self._w
         bn, bm, Mp, kA = self._bn, self._bm, self._st_Mp, self._kA
         bkX = w * px
         i, j = self._row_id, self._col_id
         rank_of = lambda r, c: r * Pc + c          # noqa: E731
-        rows_in, full_in = (bn, self.N) if adjoint else (bkX, self.K)
-        rows_out, full_out = (bkX, self.K) if adjoint else (bn, self.N)
-        y = DistributedArray(global_shape=(full_out * self.M), mask=x.mask,
-                             local_shapes=self._tile_sizes(rows_out, full_out), partition=Partition.SCATTER,
-                             dtype=torch.float32, base_comm=x.base_comm, _trusted=True)
-        x_block, _, local_m = self._padded_block(x, rows_in, full_in, torch.float32)
-        local_out = self._extent(rows_out, full_out, i, Pr)
 
         def cast_to(src, rows, dst_ptrs):
             arr = (C.c_void_p * len(dst_ptrs))(*dst_ptrs)
@@ -387,12 +384,7 @@ class _MPISummaMatrixMult(DistributedMixIn, MPILinearOperator):
                 gemm_seg(self._A_full.data_ptr() + la * w * 2, kA, YG[0], segs, w, bn, _lib.OP_H)
             self._st_barrier()
             slots, nslots, rows_blk = SA[0], Pr, bkX
-        direct = (local_out == rows_blk and local_m == bm)
-        out = y.local_array if direct else torch.empty(rows_blk * bm, dtype=torch.float32, device=x_block.device)
-        _lib.check(lib.b2_sum_slots(ctx, slots, rows_blk * bm, nslots, bm, out.data_ptr(), rows_blk, bm, st), "b2_sum_slots")
-        if not direct:
-            y.local_array.copy_(out.view(rows_blk, bm)[:local_out, :local_m].reshape(-1))
-        return y
+        _lib.check(lib.b2_sum_slots(ctx, slots, rows_blk * bm, nslots, bm, Y.data_ptr(), rows_blk, bm, st), "b2_sum_slots")
 
     # ---- replicated-panel mode (spend HBM, not NVLink) --------------------------------
     def _build_replicas(self):
@@ -439,28 +431,14 @@ class _MPISummaMatrixMult(DistributedMixIn, MPILinearOperator):
         flat = allgatherv(self._col_comm, blk.reshape(-1), [blk.numel()] * self._Pr)
         return flat.view(self._Pr * blk.shape[0], blk.shape[1])
 
-    def _apply_replicated(self, x: DistributedArray, adjoint: bool) -> DistributedArray:
-        xdt = _xdtype(self._A_row.dtype)
-        bkX = self._w * self._px
-        rows_in, full_in = (self._bn, self.N) if adjoint else (bkX, self.K)
-        rows_out, full_out = (bkX, self.K) if adjoint else (self._bn, self.N)
-        y = DistributedArray._internal((full_out * self.M,), self._tile_shapes(rows_out, full_out), x.base_comm, xdt,
-                                       mask=x.mask)
-        x_block, _, local_m = self._padded_block(x, rows_in, full_in, xdt)
+    def _product_replicated(self, x_block: torch.Tensor, Y: torch.Tensor, adjoint: bool):
         if self._A_row.dtype is torch.bfloat16 and self._bm > 1:
             x_block = _cast_bf16(x_block)                 # halves the allgather payload
         Xcol = self._gather_col(x_block)
-        local_out = self._extent(rows_out, full_out, self._row_id, self._Pr)
-        direct = (local_out == rows_out and local_m == self._bm)
-        Y_local = y.local_array.view(rows_out, self._bm) if direct else \
-            torch.empty((rows_out, self._bm), dtype=xdt, device=x_block.device)
         if adjoint:
-            tile_product(self._A_col, Xcol, Y_local, _lib.OP_H, False)
+            tile_product(self._A_col, Xcol, Y, _lib.OP_H, False)
         else:
-            tile_product(self._A_row, Xcol, Y_local, _lib.OP_N, False)
-        if not direct:
-            y.local_array.copy_(Y_local[:local_out, :local_m].reshape(-1))
-        return y
+            tile_product(self._A_row, Xcol, Y, _lib.OP_N, False)
 
     # ---- grid bookkeeping ------------------------------------------------------------------------
     def _extent(self, blk: int, full: int, idx: int, nblk: int) -> int:
@@ -500,24 +478,11 @@ class _MPISummaMatrixMult(DistributedMixIn, MPILinearOperator):
                 recv(self.base_comm, t, src)
         return mine
 
-    def _tile_sizes(self, rows_blk: int, rows_full: int):
-        cache = self.__dict__.setdefault("_tile_sizes_cache", {})
-        hit = cache.get((rows_blk, rows_full))
-        if hit is not None:
-            return hit
-        sizes = cache[(rows_blk, rows_full)] = []
-        for r in range(self.size):
-            ri, ci = divmod(r, self._Pc)
-            sizes.append(self._extent(rows_blk, rows_full, ri, self._Pr) * self._extent(self._bm, self.M, ci, self._Pc))
-        return sizes
-
     def _tile_shapes(self, rows_blk: int, rows_full: int):
-        """``_tile_sizes`` as a list of 1-tuples (the normalised form ``DistributedArray._internal`` takes)"""
-        cache = self.__dict__.setdefault("_tile_shapes_cache", {})
-        hit = cache.get((rows_blk, rows_full))
-        if hit is None:
-            hit = cache[(rows_blk, rows_full)] = [(int(n),) for n in self._tile_sizes(rows_blk, rows_full)]
-        return hit
+        """unpadded local shape of every rank's (rows_blk x bm) tile, as the 1-tuples ``DistributedArray._internal``
+        takes"""
+        return [(self._extent(rows_blk, rows_full, r // self._Pc, self._Pr) *
+                 self._extent(self._bm, self.M, r % self._Pc, self._Pc),) for r in range(self.size)]
 
     def _padded_block(self, x: DistributedArray, rows_blk: int, rows_full: int, xdt):
         local_r = self._extent(rows_blk, rows_full, self._row_id, self._Pr)
@@ -562,88 +527,81 @@ class _MPISummaMatrixMult(DistributedMixIn, MPILinearOperator):
                 done_compute[pl % 2] = ce
             pending = nxt
 
-    # ---- forward: Y_ij = sum_l A_i,l X_l,j  (MatrixMult.py:612-674) --------------------------------------
+    # ---- pipelined SUMMA ----------------------------------------------------------------------------------
+    def _product_summa(self, x_block: torch.Tensor, Y: torch.Tensor, adjoint: bool):
+        w, pa, px = self._w, self._pa, self._px
+        a_tmp = [torch.empty_like(self._A_panels[0]) for _ in range(2)] if self.size > 1 else None
+        if not adjoint:
+            # forward: Y_ij = sum_l A_i,l X_l,j  (MatrixMult.py:612-674)
+            x_tmp = [torch.empty((w, self._bm), dtype=x_block.dtype, device=x_block.device) for _ in range(2)] \
+                if self.size > 1 else None
+
+            def fetch(l):
+                a_root, la = l // pa, l % pa
+                x_root, lx = l // px, l % px
+                xp = x_block[lx * w:(lx + 1) * w]
+                if self.size == 1:
+                    return self._A_panels[la], xp
+                a_k = self._A_panels[la] if self._col_id == a_root else a_tmp[l % 2]
+                x_k = xp if self._row_id == x_root else x_tmp[l % 2]
+                bcast_(self._row_comm, a_k, root=a_root)
+                bcast_(self._col_comm, x_k, root=x_root)
+                return a_k, x_k
+
+            def compute(l, bufs):
+                tile_product(bufs[0], bufs[1], Y, _lib.OP_N, accumulate=(l > 0))
+        else:
+            # adjoint: Xadj_ij = sum_r sum_{l in tile i} (A_r,l)^H Y_r,j  (MatrixMult.py:676-767)
+            x_tmp = [torch.empty_like(x_block) for _ in range(2)] if self.size > 1 else None
+            state = {"r": -1, "buf": None}
+
+            def fetch(p):
+                a_root = p // pa
+                r = p // px
+                if self.size == 1:
+                    return self._At_panels[p % pa], x_block
+                a_k = self._At_panels[p % pa] if self._col_id == a_root else a_tmp[p % 2]
+                bcast_(self._row_comm, a_k, root=a_root)
+                if r != state["r"]:               # Y_r,j is shared by the px panels of round-group r
+                    y_k = x_block if self._row_id == r else x_tmp[r % 2]
+                    bcast_(self._col_comm, y_k, root=r)
+                    state["r"], state["buf"] = r, y_k
+                return a_k, state["buf"]
+
+            def compute(p, bufs):
+                # Y needs no zero fill: round group 0 (p < px) stores every row slice lx without accumulating
+                lx = p % px
+                tile_product(bufs[0], bufs[1], Y[lx * w:(lx + 1) * w], _lib.OP_H, accumulate=(p // px > 0))
+
+        self._pipeline(self._L, fetch, compute)
+
+    # ---- one apply frame for the three products ---------------------------------------------------------------
+    def _apply(self, x: DistributedArray, adjoint: bool) -> DistributedArray:
+        """the mode's product writes the padded (rows_out x bm) output tile ``Y``: a view of ``y`` when this rank's
+        tile is not ragged, else scratch whose unpadded part is copied out once"""
+        if x.partition != Partition.SCATTER:
+            raise ValueError(f"x should have partition={Partition.SCATTER}. Got {x.partition} instead." if adjoint else
+                             f"x should have partition={Partition.SCATTER} Got {x.partition} instead...")
+        bkX = self._w * self._px
+        rows_in, full_in, rows_out, full_out = (self._bn, self.N, bkX, self.K) if adjoint else \
+            (bkX, self.K, self._bn, self.N)
+        xdt = _xdtype(self.A.dtype)
+        y = DistributedArray._internal((full_out * self.M,), self._y_shapes[adjoint], x.base_comm, xdt, mask=x.mask)
+        x_block, _, local_m = self._padded_block(x, rows_in, full_in, xdt)
+        local_out = self._extent(rows_out, full_out, self._row_id, self._Pr)
+        direct = local_out == rows_out and local_m == self._bm
+        Y = y.local_array.view(rows_out, self._bm) if direct else \
+            torch.empty((rows_out, self._bm), dtype=xdt, device=x_block.device)
+        self._product(self, x_block, Y, adjoint)
+        if not direct:
+            y.local_array.copy_(Y[:local_out, :local_m].reshape(-1))
+        return y
+
     def _matvec(self, x: DistributedArray) -> DistributedArray:
-        if x.partition != Partition.SCATTER:
-            raise ValueError(f"x should have partition={Partition.SCATTER} Got {x.partition} instead...")
-        if self._stationary:
-            return self._apply_stationary(x, False)
-        if self._replicate:
-            return self._apply_replicated(x, False)
-        xdt = _xdtype(self._A_panels[0].dtype)
-        bkX = self._w * self._px
-        y = DistributedArray(global_shape=(self.N * self.M), mask=x.mask,
-                             local_shapes=self._tile_sizes(self._bn, self.N), partition=Partition.SCATTER,
-                             dtype=xdt, base_comm=x.base_comm, _trusted=True)
-        x_block, local_k, local_m = self._padded_block(x, bkX, self.K, xdt)
-        local_n = self._extent(self._bn, self.N, self._row_id, self._Pr)
-        Y_local = torch.empty((self._bn, self._bm), dtype=xdt, device=x_block.device)
-        a_tmp = [torch.empty_like(self._A_panels[0]) for _ in range(2)] if self.size > 1 else None
-        x_tmp = [torch.empty((self._w, self._bm), dtype=xdt, device=x_block.device) for _ in range(2)] \
-            if self.size > 1 else None
-        w, pa, px = self._w, self._pa, self._px
+        return self._apply(x, False)
 
-        def fetch(l):
-            a_root, la = l // pa, l % pa
-            x_root, lx = l // px, l % px
-            xp = x_block[lx * w:(lx + 1) * w]
-            if self.size == 1:
-                return self._A_panels[la], xp
-            a_k = self._A_panels[la] if self._col_id == a_root else a_tmp[l % 2]
-            x_k = xp if self._row_id == x_root else x_tmp[l % 2]
-            bcast_(self._row_comm, a_k, root=a_root)
-            bcast_(self._col_comm, x_k, root=x_root)
-            return a_k, x_k
-
-        def compute(l, bufs):
-            tile_product(bufs[0], bufs[1], Y_local, _lib.OP_N, accumulate=(l > 0))
-
-        self._pipeline(self._L, fetch, compute)
-        y.local_array.copy_(Y_local[:local_n, :local_m].reshape(-1))
-        return y
-
-    # ---- adjoint: Xadj_ij = sum_r sum_{l in tile i} (A_r,l)^H Y_r,j  (MatrixMult.py:676-767) -----------------
     def _rmatvec(self, x: DistributedArray) -> DistributedArray:
-        if x.partition != Partition.SCATTER:
-            raise ValueError(f"x should have partition={Partition.SCATTER}. Got {x.partition} instead.")
-        if self._stationary:
-            return self._apply_stationary(x, True)
-        if self._replicate:
-            return self._apply_replicated(x, True)
-        xdt = _xdtype(self._A_panels[0].dtype)
-        bkX = self._w * self._px
-        y = DistributedArray(global_shape=(self.K * self.M), mask=x.mask,
-                             local_shapes=self._tile_sizes(bkX, self.K), partition=Partition.SCATTER,
-                             dtype=xdt, base_comm=x.base_comm, _trusted=True)
-        x_block, local_n, local_m = self._padded_block(x, self._bn, self.N, xdt)
-        local_k = self._extent(bkX, self.K, self._row_id, self._Pr)
-        Y_local = torch.zeros((bkX, self._bm), dtype=xdt, device=x_block.device)
-        a_tmp = [torch.empty_like(self._A_panels[0]) for _ in range(2)] if self.size > 1 else None
-        x_tmp = [torch.empty_like(x_block) for _ in range(2)] if self.size > 1 else None
-        w, pa, px = self._w, self._pa, self._px
-        state = {"r": -1, "buf": None}
-
-        def fetch(p):
-            a_root = p // pa
-            r = p // px
-            if self.size == 1:
-                return self._At_panels[p % pa], x_block
-            a_k = self._At_panels[p % pa] if self._col_id == a_root else a_tmp[p % 2]
-            bcast_(self._row_comm, a_k, root=a_root)
-            if r != state["r"]:               # Y_r,j is shared by the px panels of round-group r
-                y_k = x_block if self._row_id == r else x_tmp[r % 2]
-                bcast_(self._col_comm, y_k, root=r)
-                state["r"], state["buf"] = r, y_k
-            return a_k, state["buf"]
-
-        def compute(p, bufs):
-            lx = p % px
-            tile_product(bufs[0], bufs[1], Y_local[lx * w:(lx + 1) * w], _lib.OP_H, accumulate=(p // px > 0))
-
-        self._pipeline(self._L, fetch, compute)
-        y.local_array.copy_(Y_local[:local_k, :local_m].reshape(-1))
-        return y
-
+        return self._apply(x, True)
 
 def MPIMatrixMult(A, M: int, saveAt: bool = False, base_comm=COMM_WORLD, kind: str = "summa",
                   dtype="float64", base_comm_nccl=None, grid=None, replicate: bool = False, stationary: bool = False):

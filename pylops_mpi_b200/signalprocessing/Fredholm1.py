@@ -11,7 +11,7 @@ import torch
 
 from .. import _lib
 from ..comm import COMM_WORLD, resolve
-from ..DistributedArray import DistributedArray, Partition
+from ..DistributedArray import _BCAST, DistributedArray, Partition
 from ..LinearOperator import MPILinearOperator
 
 # products per slice (nx * ny * nz) from which float32 / complex64 slices run on the tensor-core plan; smaller slices
@@ -56,8 +56,8 @@ class MPIFredholm1(MPILinearOperator):
         if fused is None:
             fused = base_comm.Get_size() > 1 and base_comm.mailbox is not None
         self._fused = bool(fused) and base_comm.Get_size() > 1 and not self._scatter_data
+        esz = self.G.element_size()
         if self._fused:
-            esz = torch.empty(0, dtype=self._tdtype).element_size()
             self._arena = {}
             for adjoint in (False, True):
                 nelem = nslstot * (self.ny if adjoint else self.nx) * self.nz
@@ -74,6 +74,19 @@ class MPIFredholm1(MPILinearOperator):
             _lib.check(_lib.lib.b2_fredholm_plan_create(_lib.ctx(), self.G.data_ptr(), self.nsl, self.nx, self.ny, self.nz,
                                                         _lib.code(self._tdtype), C.byref(h)), "b2_fredholm_plan_create")
             self._plan = h
+        # by direction (index: adjoint): byte offsets of this rank's slices in the input (the scattered data holds only
+        # them) and in the output, the local shapes of a gathered output, and the element counts / offsets of every
+        # rank's slices in it
+        size, start = base_comm.Get_size(), int(self.islstart[base_comm.Get_rank()])
+        self._x_off = [start * self.ny * self.nz * esz, 0 if self._scatter_data else start * self.nx * self.nz * esz]
+        self._y_shapes = [[(n,)] * size for n in self.shape]
+        self._y_off = [start * n * self.nz * esz for n in (self.nx, self.ny)]
+        self._gatherv = [((C.c_size_t * size)(*[int(k) * n * self.nz for k in self.nsls]),
+                          (C.c_size_t * size)(*[int(o) * n * self.nz for o in self.islstart])) for n in (self.nx, self.ny)]
+        # how an apply delivers its output, chosen once; the function, not a bound method, so that no reference cycle
+        # delays __del__
+        self._output = (MPIFredholm1._out_scattered if self._scatter_data else
+                        MPIFredholm1._out_fused if self._fused else MPIFredholm1._out_gathered)
 
     def __del__(self):
         plan = getattr(self, "_plan", None)
@@ -102,89 +115,69 @@ class MPIFredholm1(MPILinearOperator):
                                                 self.nz, int(adjoint), _lib.code(self._tdtype), _lib.stream()),
                        "b2_batched_gemm")
 
-    def _product_gathered(self, xs: torch.Tensor, y: DistributedArray, adjoint: bool) -> DistributedArray:
+    def _local_slices(self, x: DistributedArray, adjoint: bool):
+        """this rank's slices of ``x`` in the operator dtype: ``(tensor holding them, address of the first)``; the
+        caller keeps the tensor alive until the product is enqueued"""
+        xl = x._cont()
+        if xl.dtype != self._tdtype:
+            xl = xl.to(self._tdtype)
+        return xl, xl.data_ptr() + self._x_off[adjoint]
+
+    def _out_gathered(self, x_ptr: int, x: DistributedArray, adjoint: bool) -> DistributedArray:
         """this rank's slices of op(G) x straight into their place in the BROADCAST ``y``, then ONE NCCL Allgatherv
         in place on the current stream brings in the other ranks' slices"""
-        rank, pout = self.rank, (self.ny if adjoint else self.nx) * self.nz
-        yflat = y.local_array.view(-1)
-        mine = yflat[self.islstart[rank] * pout: self.islend[rank] * pout]
+        shapes = self._y_shapes[adjoint]
+        y = DistributedArray._internal(shapes[0], shapes, x.base_comm, self._tdtype,
+                                       partition=Partition.BROADCAST if x.partition is Partition.SCATTER else x.partition)
+        base = y.local_array.data_ptr()
         if self.nsl:
-            self._product(xs.data_ptr(), mine.data_ptr(), adjoint)
-        if y.size > 1:
-            comm = y.base_comm
-            counts = (C.c_size_t * comm.size)(*[int(n) * pout for n in self.nsls])
-            offs = (C.c_size_t * comm.size)(*[int(o) * pout for o in self.islstart])
-            _lib.check(_lib.lib.b2_allgatherv_at(comm.nccl, mine.data_ptr(), yflat.data_ptr(), counts, offs,
+            self._product(x_ptr, base + self._y_off[adjoint], adjoint)
+        if self.size > 1:
+            counts, offs = self._gatherv[adjoint]
+            _lib.check(_lib.lib.b2_allgatherv_at(x.base_comm.nccl, base + self._y_off[adjoint], base, counts, offs,
                                                  _lib.code(self._tdtype), _lib.stream()), "b2_allgatherv_at")
         return y
 
-    # ---- fused product + all-gather over peer memory ------------------------------------------------
-    def _apply_fused(self, x: DistributedArray, adjoint: bool) -> DistributedArray:
+    def _out_scattered(self, x_ptr: int, x: DistributedArray, adjoint: bool) -> DistributedArray:
+        """scatter_data: the forward output holds only this rank's slices (no gather); the adjoint gathers"""
+        if adjoint:
+            return self._out_gathered(x_ptr, x, True)
+        y = DistributedArray._internal((self.shape[0],), [(int(n) * self.nx * self.nz,) for n in self.nsls],
+                                       x.base_comm, self._tdtype)
+        if self.nsl:
+            self._product(x_ptr, y.local_array.data_ptr(), False)
+        return y
+
+    def _out_fused(self, x_ptr: int, x: DistributedArray, adjoint: bool) -> DistributedArray:
+        """product and all-gather in one kernel over peer memory"""
         from ..Distributed import allreduce_
         rank, comm = self.rank, x.base_comm
-        nin, nout = (self.nx, self.ny) if adjoint else (self.ny, self.nx)
-        xl = x.local_array if x.local_array.dtype == self._tdtype else x.local_array.to(self._tdtype)
-        per, pout = nin * self.nz, nout * self.nz
-        xs = xl.reshape(-1)[self.islstart[rank] * per: self.islend[rank] * per]
         b = self._toggle[adjoint]
         self._toggle[adjoint] = 1 - b
         base, peers, nelem = self._arena[(adjoint, b)]
-        off = int(self.islstart[rank]) * pout * xl.element_size()
-        self._product(xs.data_ptr(), base + off, adjoint, [peers[r] + off for r in range(comm.Get_size()) if r != rank])
+        off = self._y_off[adjoint]
+        self._product(x_ptr, base + off, adjoint, [peers[r] + off for r in range(comm.Get_size()) if r != rank])
         # stream-ordered cross-rank completion: when this tiny Allreduce finishes every rank's product
         # kernel (and its peer stores) has finished
         allreduce_(comm, self._flag, "sum")
-        y = DistributedArray(global_shape=self.shape[1] if adjoint else self.shape[0], base_comm=comm,
-                             partition=x.partition, dtype=self._tdtype)
+        shapes = self._y_shapes[adjoint]
+        y = DistributedArray._internal(shapes[0], shapes, comm, self._tdtype, partition=x.partition)
         # copy out of the (double-buffered) arena: the caller owns an ordinary array, as in the reference
         _lib.check(_lib.lib.b2_lincomb(_lib.ctx(), y.local_array.data_ptr(), _lib.cpair(1.0), base, None, None, nelem,
                                        _lib.code(self._tdtype), 0, _lib.stream()), "b2_lincomb")
         return y
 
-    def _apply_scatter(self, x: DistributedArray, adjoint: bool) -> DistributedArray:
-        rank = self.rank
-        if not adjoint:
-            if x.partition not in [Partition.BROADCAST, Partition.UNSAFE_BROADCAST]:
-                raise ValueError(f"x should have partition={Partition.BROADCAST},{Partition.UNSAFE_BROADCAST}"
-                                 f"Got  {x.partition} instead...")
-            per = self.ny * self.nz
-            xl = x.local_array if x.local_array.dtype == self._tdtype else x.local_array.to(self._tdtype)
-            xs = xl.reshape(-1)[self.islstart[rank] * per: self.islend[rank] * per]
-            y = DistributedArray(global_shape=self.shape[0], base_comm=x.base_comm, partition=Partition.SCATTER,
-                                 local_shapes=[(int(n) * self.nx * self.nz,) for n in self.nsls], dtype=self._tdtype)
-            if self.nsl:
-                self._product(xs.data_ptr(), y.local_array.data_ptr(), False)
-            return y
-        if x.partition is not Partition.SCATTER:
-            raise ValueError(f"x should have partition={Partition.SCATTER} Got {x.partition} instead...")
-        xl = x.local_array if x.local_array.dtype == self._tdtype else x.local_array.to(self._tdtype)
-        if xl.numel() != self.nsl * self.nx * self.nz:
-            raise ValueError("scattered data does not match this rank's slices")
-        y = DistributedArray(global_shape=self.shape[1], base_comm=x.base_comm, partition=Partition.BROADCAST,
-                             dtype=self._tdtype)
-        return self._product_gathered(xl.reshape(-1), y, True)
-
     def _apply(self, x: DistributedArray, adjoint: bool) -> DistributedArray:
-        if self._scatter_data:
-            return self._apply_scatter(x, adjoint)
-        if x.partition not in [Partition.BROADCAST, Partition.UNSAFE_BROADCAST]:
+        if self._scatter_data and adjoint:
+            if x.partition is not Partition.SCATTER:
+                raise ValueError(f"x should have partition={Partition.SCATTER} Got {x.partition} instead...")
+            if x.local_array.numel() != self.nsl * self.nx * self.nz:
+                raise ValueError("scattered data does not match this rank's slices")
+        elif x.partition not in _BCAST:
             raise ValueError(f"x should have partition={Partition.BROADCAST},{Partition.UNSAFE_BROADCAST}"
                              f"Got  {x.partition} instead...")
-        if self._fused:
-            return self._apply_fused(x, adjoint)
-        if x.size == 1 and self._plan is not None and x.local_array.dtype == self._tdtype:
-            # single rank, tensor-core plan: one library call (the 18.6 us apply is otherwise host-bound)
-            n = self.shape[1] if adjoint else self.shape[0]
-            y = DistributedArray._internal((n,), [(n,)], x.base_comm, self._tdtype, partition=x.partition)
-            self._product(x._cont().data_ptr(), y.local_array.data_ptr(), adjoint)
-            return y
-        rank = self.rank
-        per = (self.nx if adjoint else self.ny) * self.nz
-        xl = x.local_array if x.local_array.dtype == self._tdtype else x.local_array.to(self._tdtype)
-        xs = xl.reshape(-1)[self.islstart[rank] * per: self.islend[rank] * per]
-        y = DistributedArray(global_shape=self.shape[1] if adjoint else self.shape[0],
-                             base_comm=x.base_comm, partition=x.partition, dtype=self._tdtype)
-        return self._product_gathered(xs, y, adjoint)
+        xl, x_ptr = self._local_slices(x, adjoint)      # xl holds the slices until the product is enqueued
+        return self._output(self, x_ptr, x, adjoint)
 
     def _matvec(self, x: DistributedArray) -> DistributedArray:
         return self._apply(x, False)
