@@ -225,6 +225,17 @@ int b2_nsconvolve_axis(b2_ctx* ctx, const void* x, void* y, size_t n_outer, size
 int b2_nspoststack_axis(b2_ctx* ctx, const void* x, void* y, size_t n_outer, size_t n_axis, size_t n_inner,
                         const void* hs, int nfilt, int nh, int hc, long long oh, long long dh, int kind, int adjoint,
                         int dtype, void* stream);
+/* rank-local NON-STATIONARY 2-D convolution of a C-ordered [nx][nz][n_inner] image (n_inner 1, or 2 for complex data
+ * as (re, im) pairs of the real dtype): pylops.signalprocessing.NonStationaryConvolve2D.  hs is a device array
+ * [nfx][nfz][nhx][nhz] of real filters (the data's real dtype) at the points (ohx + dhx a, ohz + dhz b), centre
+ * (nhx / 2, nhz / 2); point j uses h_j, bilinear in the bank with float64 per-axis weights (the first / last filter
+ * outside the nodes), each weight product rounded to the dtype.  Forward y[i] = sum_j h_j[hc + i - j] x[j], adjoint =
+ * exact transpose.  One launch, no atomics, no allocation: repeated applies give identical bits.  dtype F32 / F64.
+ * B2_ERR_ARG: a null pointer, x == y, an empty image, n_inner not 1 or 2, nfx / nfz / nhx / nhz < 1, dhx / dhz < 1;
+ * B2_ERR_DTYPE: another dtype; y is untouched on every error */
+int b2_nsconvolve2d(b2_ctx* ctx, const void* x, void* y, size_t nx, size_t nz, size_t n_inner, const void* hs, int nfx,
+                    int nfz, int nhx, int nhz, long long ohx, long long dhx, long long ohz, long long dhz, int adjoint,
+                    int dtype, void* stream);
 /* rank-local Kirchhoff demigration, spreading / stacking stage: pylops.waveeqprocessing.Kirchhoff (mode="analytic",
  * 2-D or 3-D, dynamic=False) before its wavelet convolution (run that as b2_convolve_axis on the [ns*nr][nt] traces).
  * Tables are float64 device arrays in the kernel's layout: trav_srcs [ns][ni], trav_recs [nr][ni] (a trace reads

@@ -390,22 +390,85 @@ class NonStationaryConvolve1D(_AxisOperator):
             raise ValueError(f"hs must be a 2-D array of filters (nfilt, nh); got shape {hs.shape}")
         if hs.shape[1] % 2 == 0:
             raise ValueError("filters hs must have odd length")
-        ih = np.asarray(ih).ravel()
-        if len(ih) != hs.shape[0]:
-            raise ValueError(f"ih has {len(ih)} indices for {hs.shape[0]} filters")
-        if len(np.unique(np.diff(ih))) > 1:
-            raise ValueError("the indices of filters 'ih' must be regularly sampled")
         super().__init__(dims, axis, dtype)
-        if min(ih) < 0 or max(ih) >= self.dims[self.axis]:
-            raise ValueError("the indices of filters 'ih' must be larger than 0 and smaller than `dims`")
-        dh = int(ih[1] - ih[0]) if len(ih) > 1 else 1
-        if dh < 1:
-            raise ValueError("the indices of filters 'ih' must be increasing")
-        self._conv = c = _FilterBank(bank, hs.shape[1] // 2, ih[0], dh)
+        oh, dh = _regular_nodes("ih", ih, hs.shape[0], self.dims[self.axis])
+        self._conv = c = _FilterBank(bank, hs.shape[1] // 2, oh, dh)
         self.nfilt, self.nh, self.hc, self.oh, self.dh = c.nfilt, c.nh, c.hc, c.oh, c.dh
 
     def _launch(self, x, y, dt, adjoint):
         self._conv.launch(x, y, self._lines(dt), adjoint)
+
+
+def _regular_nodes(name, ih, nfilt, n):
+    """``(origin, step)`` of the filter indices ``ih`` along an axis of ``n`` samples holding ``nfilt`` filters, with
+    pylops' ``ValueError``s and ours (count, decreasing); one filter has step 1"""
+    ih = np.asarray(ih).ravel()
+    if len(ih) != nfilt:
+        raise ValueError(f"{name} has {len(ih)} indices for {nfilt} filters")
+    if len(np.unique(np.diff(ih))) > 1:
+        raise ValueError(f"the indices of filters '{name}' must be regularly sampled")
+    if min(ih) < 0 or max(ih) >= n:
+        raise ValueError(f"the indices of filters '{name}' must be larger than 0 and smaller than `dims`")
+    dh = int(ih[1] - ih[0]) if len(ih) > 1 else 1
+    if dh < 1:
+        raise ValueError(f"the indices of filters '{name}' must be increasing")
+    return int(ih[0]), dh
+
+
+class NonStationaryConvolve2D(_KernelOperator):
+    """Rank-local non-stationary 2-D convolution of a C-ordered ``dims = (nx, nz)`` image,
+    pylops.signalprocessing.NonStationaryConvolve2D (pylops 2.x) inside MPIBlockDiag: image-domain least-squares
+    migration, with point-spread functions for filters.  ``hs`` of shape ``(nfx, nfz, nhx, nhz)`` holds real filters
+    of odd sizes at the regularly spaced image points ``(ihx[a], ihz[b])``; point ``j`` uses ``h_j``, bilinear in the
+    four filters around it (per axis, the first / last filter outside the nodes)::
+
+        y[i] = sum_j h_j[nhx // 2 + ix - jx, nhz // 2 + iz - jz] x[j]
+
+    and the adjoint is the exact transpose.  One b2_nsconvolve2d launch per apply (csrc/nsconvolve2d.cu), complex data
+    included.  The operator dtype is ``dtype``; data are promoted and ``out=`` is handled as in
+    :class:`NonStationaryConvolve1D`, and float32 data of a float32 operator use the bank rounded to float32.
+    ``ValueError`` for even filter sizes, irregular or decreasing indices, indices outside ``[0, dims)``,
+    ``len(ihx) != nfx``, ``len(ihz) != nfz``, an ``hs`` that is not 4-D and ``dims`` without two entries; complex
+    filters are not provided.  ``engine`` and ``num_threads_per_blocks`` are accepted and ignored."""
+
+    def __init__(self, dims, hs, ihx, ihz, engine="numpy", num_threads_per_blocks=(32, 32), dtype="float64"):
+        hs = hs.detach().cpu().numpy() if isinstance(hs, torch.Tensor) else np.asarray(hs)
+        if np.iscomplexobj(hs):
+            raise NotImplementedError("complex filters are not supported")
+        dims = tuple(int(d) for d in (dims if np.ndim(dims) else (dims,)))
+        if len(dims) != 2:
+            raise ValueError(f"dims must hold two entries (nx, nz); got {dims}")
+        if hs.ndim != 4:
+            raise ValueError(f"hs must be a 4-D array of filters (nfx, nfz, nhx, nhz); got shape {hs.shape}")
+        if hs.shape[2] % 2 == 0 or hs.shape[3] % 2 == 0:
+            raise ValueError("filters hs must have odd length")
+        self.ohx, self.dhx = _regular_nodes("ihx", ihx, hs.shape[0], dims[0])
+        self.ohz, self.dhz = _regular_nodes("ihz", ihz, hs.shape[1], dims[1])
+        self.dims = self.dimsd = dims
+        n = dims[0] * dims[1]
+        self.shape = (n, n)
+        self._tdtype = _lib.torch_dtype(dtype)
+        self.dtype = _lib.numpy_dtype(self._tdtype)
+        self.engine, self.num_threads_per_blocks = engine, num_threads_per_blocks
+        _lib.ctx()
+        self._bank = _real_filters(hs)[1]
+        self.nfilt = (int(hs.shape[0]), int(hs.shape[1]))
+        self.nh = (int(hs.shape[2]), int(hs.shape[3]))
+        self.hc = (self.nh[0] // 2, self.nh[1] // 2)
+        self.oh = (self.ohx, self.ohz)
+        self.dh = (self.dhx, self.dhz)
+
+    def _compute_dtype(self, xdt):
+        if xdt.is_complex and not self._tdtype.is_complex:
+            return _CPLX_OF[torch.promote_types(self._tdtype, _REAL_OF[xdt])]
+        return self._tdtype
+
+    def _launch(self, x, y, dt, adjoint):
+        real = _REAL_OF.get(dt, dt)
+        _lib.check(_lib.lib.b2_nsconvolve2d(_lib.ctx(), x.data_ptr(), y.data_ptr(), *self.dims,
+                                            2 if dt.is_complex else 1, self._bank[real].data_ptr(), *self.nfilt,
+                                            *self.nh, self.ohx, self.dhx, self.ohz, self.dhz, adjoint,
+                                            _lib.code(real), _lib.stream()), "b2_nsconvolve2d")
 
 
 class PoststackLinearModelling(_AxisOperator):
