@@ -236,6 +236,19 @@ int b2_nspoststack_axis(b2_ctx* ctx, const void* x, void* y, size_t n_outer, siz
 int b2_nsconvolve2d(b2_ctx* ctx, const void* x, void* y, size_t nx, size_t nz, size_t n_inner, const void* hs, int nfx,
                     int nfz, int nhx, int nhz, long long ohx, long long dhx, long long ohz, long long dhz, int adjoint,
                     int dtype, void* stream);
+/* rank-local NON-STATIONARY 3-D convolution of a C-ordered [nx][ny][nz][n_inner] volume (n_inner 1, or 2 for complex
+ * data as (re, im) pairs of the real dtype): pylops.signalprocessing.NonStationaryConvolve3D.  hs is a device array
+ * [nfx][nfy][nfz][nhx][nhy][nhz] of real filters (the data's real dtype) at the points (ohx + dhx a, ohy + dhy b,
+ * ohz + dhz e), centre (nhx / 2, nhy / 2, nhz / 2); point j uses h_j, trilinear in the bank with float64 per-axis
+ * weights (the first / last filter outside the nodes), each weight product (wz wy) wx rounded once to the dtype.
+ * Forward y[i] = sum_j h_j[hc + i - j] x[j], adjoint = exact transpose.  One launch, no atomics, no allocation:
+ * repeated applies give identical bits.  dtype F32 / F64.
+ * B2_ERR_ARG: a null pointer, x == y, an empty axis, n_inner not 1 or 2, nfx / nfy / nfz / nhx / nhy / nhz < 1,
+ * dhx / dhy / dhz < 1, an axis, filter size or node position of 2^29 samples or more (the kernel indexes each axis
+ * in 32 bits), more tiles than one grid holds; B2_ERR_DTYPE: another dtype; y is untouched on every error */
+int b2_nsconvolve3d(b2_ctx* ctx, const void* x, void* y, size_t nx, size_t ny, size_t nz, size_t n_inner, const void* hs,
+                    int nfx, int nfy, int nfz, int nhx, int nhy, int nhz, long long ohx, long long dhx, long long ohy,
+                    long long dhy, long long ohz, long long dhz, int adjoint, int dtype, void* stream);
 /* rank-local Kirchhoff demigration, spreading / stacking stage: pylops.waveeqprocessing.Kirchhoff (mode="analytic",
  * 2-D or 3-D, dynamic=False) before its wavelet convolution (run that as b2_convolve_axis on the [ns*nr][nt] traces).
  * Tables are float64 device arrays in the kernel's layout: trav_srcs [ns][ni], trav_recs [nr][ni] (a trace reads

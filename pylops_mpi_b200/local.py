@@ -471,6 +471,67 @@ class NonStationaryConvolve2D(_KernelOperator):
                                             _lib.code(real), _lib.stream()), "b2_nsconvolve2d")
 
 
+class NonStationaryConvolve3D(_KernelOperator):
+    """Rank-local non-stationary 3-D convolution of a C-ordered volume of shape ``dims`` (three entries),
+    pylops.signalprocessing.NonStationaryConvolve3D (pylops 2.x as remembered: pylops is not installed here to check
+    the signature, defaults or weight clamp) inside MPIBlockDiag: image-domain least-squares migration in 3-D, with
+    point-spread functions for filters.  ``hs`` of shape ``(nfx, nfy, nfz, nhx, nhy, nhz)`` holds real filters of odd
+    sizes at the regularly spaced points ``(ihx[a], ihy[b], ihz[e])``; point ``j`` uses ``h_j``, trilinear in the
+    eight filters around it (per axis, the first / last filter outside the nodes)::
+
+        y[i] = sum_j h_j[nhx // 2 + ix - jx, nhy // 2 + iy - jy, nhz // 2 + iz - jz] x[j]
+
+    and the adjoint is the exact transpose.  ``x``, ``y`` and ``z`` are pylops' labels for the positions 0, 1 and 2 of
+    ``dims``: a 3-D :class:`Kirchhoff` image is ``(ny, nx, nz)``, so the operator for its PSFs is
+    ``NonStationaryConvolve3D((ny, nx, nz), hs, i_first_axis, i_second_axis, iz)``.  One b2_nsconvolve3d launch per
+    apply (csrc/nsconvolve3d.cu), complex data included.  The operator dtype is ``dtype``; data are promoted and
+    ``out=`` is handled as in :class:`NonStationaryConvolve2D`, and float32 data of a float32 operator use the bank
+    rounded to float32.  ``ValueError`` for even filter sizes, irregular or decreasing indices, indices outside
+    ``[0, dims)``, ``len(ihx) != nfx`` (and for y, z), an ``hs`` that is not 6-D and ``dims`` without three entries;
+    complex filters are not provided.  ``engine`` and ``num_threads_per_blocks`` are accepted and ignored."""
+
+    def __init__(self, dims, hs, ihx, ihy, ihz, engine="numpy", num_threads_per_blocks=(2, 16, 16),
+                 dtype="float64"):
+        hs = hs.detach().cpu().numpy() if isinstance(hs, torch.Tensor) else np.asarray(hs)
+        if np.iscomplexobj(hs):
+            raise NotImplementedError("complex filters are not supported")
+        dims = tuple(int(d) for d in (dims if np.ndim(dims) else (dims,)))
+        if len(dims) != 3:
+            raise ValueError(f"dims must hold three entries (nx, ny, nz); got {dims}")
+        if hs.ndim != 6:
+            raise ValueError(f"hs must be a 6-D array of filters (nfx, nfy, nfz, nhx, nhy, nhz); got shape {hs.shape}")
+        if any(n % 2 == 0 for n in hs.shape[3:]):
+            raise ValueError("filters hs must have odd length")
+        nodes = [_regular_nodes(name, ih, nf, n) for name, ih, nf, n in zip(("ihx", "ihy", "ihz"), (ihx, ihy, ihz),
+                                                                               hs.shape[:3], dims)]
+        self.dims = self.dimsd = dims
+        n = dims[0] * dims[1] * dims[2]
+        self.shape = (n, n)
+        self._tdtype = _lib.torch_dtype(dtype)
+        self.dtype = _lib.numpy_dtype(self._tdtype)
+        self.engine, self.num_threads_per_blocks = engine, num_threads_per_blocks
+        _lib.ctx()
+        self._bank = _real_filters(hs)[1]
+        self.nfilt = tuple(int(v) for v in hs.shape[:3])
+        self.nh = tuple(int(v) for v in hs.shape[3:])
+        self.hc = tuple(v // 2 for v in self.nh)
+        self.oh = tuple(o for o, _ in nodes)
+        self.dh = tuple(d for _, d in nodes)
+
+    def _compute_dtype(self, xdt):
+        if xdt.is_complex and not self._tdtype.is_complex:
+            return _CPLX_OF[torch.promote_types(self._tdtype, _REAL_OF[xdt])]
+        return self._tdtype
+
+    def _launch(self, x, y, dt, adjoint):
+        real = _REAL_OF.get(dt, dt)
+        axes = [v for o, d in zip(self.oh, self.dh) for v in (o, d)]
+        _lib.check(_lib.lib.b2_nsconvolve3d(_lib.ctx(), x.data_ptr(), y.data_ptr(), *self.dims,
+                                            2 if dt.is_complex else 1, self._bank[real].data_ptr(), *self.nfilt,
+                                            *self.nh, *axes, adjoint, _lib.code(real), _lib.stream()),
+                   "b2_nsconvolve3d")
+
+
 class PoststackLinearModelling(_AxisOperator):
     """Rank-local post-stack seismic modelling, pylops.avo.poststack.PoststackLinearModelling (pylops 2.x) for a
     real wavelet, as tutorials/poststack.py uses it inside MPIBlockDiag::
