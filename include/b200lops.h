@@ -236,6 +236,23 @@ int b2_nspoststack_axis(b2_ctx* ctx, const void* x, void* y, size_t n_outer, siz
 int b2_nsconvolve2d(b2_ctx* ctx, const void* x, void* y, size_t nx, size_t nz, size_t n_inner, const void* hs, int nfx,
                     int nfz, int nhx, int nhz, long long ohx, long long dhx, long long ohz, long long dhz, int adjoint,
                     int dtype, void* stream);
+/* rank-local NON-STATIONARY FILTER ESTIMATION, adjoint: pylops.signalprocessing.NonStationaryFilters2D^H (and
+ * NonStationaryFilters1D^H with nx = nfx = nhx = 1, ohx = 0, dhx = 1).  For a C-ordered real image d [nx][nz] and the
+ * fixed real image inp [nx][nz], writes the bank hs_out [nfx][nfz][nhx][nhz] of the transpose of b2_nsconvolve2d's
+ * forward in its bank: g_c[k] = sum_(j in S_c) W_c[j] inp[j] d[j + k - hc], with the points, weights, supports and
+ * centres of b2_nsconvolve2d.  Each filter's support is split into a number of parts fixed by the shape; with more
+ * than one part the partial banks go to work (b2_nsfilters2d_work_bytes bytes, 0 with one part) and are folded in
+ * ascending order.  No atomics, no allocation: the bits depend only on the shape and the dtype.  dtype F32 / F64.
+ * B2_ERR_ARG: a null ctx, d, inp or hs_out, hs_out overlapping d or inp, an empty image, an axis over 2^40 samples
+ * or an image over 2^50, nfx / nfz / nhx / nhz < 1, dhx / dhz < 1, more CTAs than one grid holds, a null or short work
+ * (when one is needed) or work overlapping d, inp or hs_out; B2_ERR_DTYPE: another dtype; hs_out is untouched on every error */
+int b2_nsfilters2d_adjoint(b2_ctx* ctx, const void* d, const void* inp, void* hs_out, size_t nx, size_t nz, int nfx,
+                           int nfz, int nhx, int nhz, long long ohx, long long dhx, long long ohz, long long dhz,
+                           void* work, size_t work_bytes, int dtype, void* stream);
+/* *bytes = the workspace b2_nsfilters2d_adjoint needs for this shape and dtype; error codes as that entry's shape
+ * checks, plus B2_ERR_ARG for a null bytes */
+int b2_nsfilters2d_work_bytes(size_t nx, size_t nz, int nfx, int nfz, int nhx, int nhz, long long ohx, long long dhx,
+                              long long ohz, long long dhz, int dtype, size_t* bytes);
 /* rank-local NON-STATIONARY 3-D convolution of a C-ordered [nx][ny][nz][n_inner] volume (n_inner 1, or 2 for complex
  * data as (re, im) pairs of the real dtype): pylops.signalprocessing.NonStationaryConvolve3D.  hs is a device array
  * [nfx][nfy][nfz][nhx][nhy][nhz] of real filters (the data's real dtype) at the points (ohx + dhx a, ohy + dhy b,

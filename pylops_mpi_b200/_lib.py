@@ -95,6 +95,8 @@ def _load():
         "b2_nspoststack_axis": ([vp, vp, vp, sz, sz, sz, vp, i, i, i, ll, ll, i, i, i, vp], i),
         "b2_nsconvolve2d": ([vp, vp, vp, sz, sz, sz, vp, i, i, i, i, ll, ll, ll, ll, i, i, vp], i),
         "b2_nsconvolve3d": ([vp, vp, vp, sz, sz, sz, sz, vp, i, i, i, i, i, i, ll, ll, ll, ll, ll, ll, i, i, vp], i),
+        "b2_nsfilters2d_adjoint": ([vp, vp, vp, vp, sz, sz, i, i, i, i, ll, ll, ll, ll, vp, sz, i, vp], i),
+        "b2_nsfilters2d_work_bytes": ([sz, sz, i, i, i, i, ll, ll, ll, ll, i, C.POINTER(sz)], i),
         "b2_kirchhoff": ([vp, vp, vp, vp, vp, sz, sz, sz, sz, d, i, i, vp], i),
         "b2_kirchhoff_chunk": ([vp, vp, vp, vp, vp, sz, sz, sz, sz, sz, sz, d, i, i, i, vp], i),
         "b2_kirchhoff_tables": ([vp, vp, vp, vp, sz, sz, sz, vp, sz, d, sz, sz, vp, vp], i),

@@ -25,53 +25,15 @@
 // in ascending (x, z) order (forward: of the reversed filter), one fma per term.  No atomics, no allocation: repeated
 // applies give identical bits.  The sums differ from pylops' (interpolate h_j, then convolve) only in rounding; with
 // exactly representable inputs both are exact.
-#include "common.cuh"
+#include "ns2_core.cuh"
 
 namespace {
-
-constexpr int N2_LANES = 32, N2_GROUPS = 8, N2_THREADS = N2_LANES * N2_GROUPS;
-constexpr int N2_RT = 8;                                   // consecutive z outputs per thread
-constexpr int N2_TX = N2_LANES, N2_TZ = N2_GROUPS * N2_RT;   // outputs per CTA: 32 (x) x 64 (z)
-constexpr int N2_KC = 32;                                  // taps per chunk along each axis (a multiple of N2_RT)
-constexpr int N2_WR = N2_TX + N2_KC - 1;                   // window rows (x)
-constexpr int N2_WC = N2_TZ + N2_KC;                       // window columns (z): the register window reads one past
-constexpr int N2_WS = N2_WC + 1;                           // odd row stride: the lanes' rows fall in different banks
-constexpr int N2_WELEMS = (N2_WR * N2_WS + 15) / 16 * 16;  // window elements, padded so the taps stay vector-aligned
-
-struct Axis {
-  long long n, oh, dh;
-  int nf, nh, hc;
-};
 
 struct Ns2Params {
   Axis ax[2];            // x, z
   long long tiles_z;
   long long n_inner;
 };
-
-__device__ __forceinline__ long long floor_div(long long a, long long b) {   // b > 0
-  const long long q = a / b;
-  return (a % b != 0 && a < 0) ? q - 1 : q;
-}
-
-// [lo, hi): the samples of [0, n) with a non-zero weight on filter a
-__device__ __forceinline__ void support(const Axis& A, int a, long long& lo, long long& hi) {
-  lo = a == 0 ? 0 : A.oh + (long long)(a - 1) * A.dh + 1;
-  hi = a == A.nf - 1 ? A.n : A.oh + (long long)(a + 1) * A.dh;
-  lo = max(lo, 0LL);
-  hi = min(hi, A.n);
-}
-
-// the float64 weight of filter a at sample j
-__device__ __forceinline__ double axis_weight(const Axis& A, int a, long long j) {
-  const double v = (double)(j - A.oh) / (double)A.dh;
-  const double fl = floor(v);
-  if (fl < 0.0) return a == 0 ? 1.0 : 0.0;
-  if (fl >= (double)(A.nf - 1)) return a == A.nf - 1 ? 1.0 : 0.0;
-  const int l = (int)fl;
-  if (a == l) return 1.0 - (v - fl);
-  return a == l + 1 ? v - fl : 0.0;
-}
 
 // taps [qlo, qhi) of filter a that can meet its support from a tile of nt outputs at i0 (window row m = sample jb + m)
 __device__ __forceinline__ bool tap_span(const Axis& A, int a, long long i0, long long jb, int nt, bool adj, int& qlo,
@@ -93,33 +55,6 @@ __device__ __forceinline__ bool tap_span(const Axis& A, int a, long long i0, lon
   qlo = (int)q0;
   qhi = (int)q1;
   return q0 < q1;
-}
-
-// out[r] += sum_(qx < nqx, qz < nqz8) hk[qx][qz] w[lane + qx][t0 + r + qz]
-template <typename T>
-__device__ __forceinline__ void correlate(T (&out)[N2_RT], const T* __restrict__ w, const T* __restrict__ hk, int nqx,
-                                          int nqz8, int lane, int t0) {
-  using VA = VecN<T, N2_RT>;
-  for (int qx = 0; qx < nqx; ++qx) {
-    const T* wr = w + (lane + qx) * N2_WS + t0;
-    const T* hr = hk + qx * N2_KC;
-    T lo[N2_RT];
-#pragma unroll
-    for (int r = 0; r < N2_RT; ++r) lo[r] = wr[r];
-    for (int q0 = 0; q0 < nqz8; q0 += N2_RT) {
-      T hi[N2_RT];
-#pragma unroll
-      for (int r = 0; r < N2_RT; ++r) hi[r] = wr[q0 + N2_RT + r];
-      const VA hv = *reinterpret_cast<const VA*>(hr + q0);
-#pragma unroll
-      for (int qq = 0; qq < N2_RT; ++qq) {
-#pragma unroll
-        for (int r = 0; r < N2_RT; ++r) out[r] = fma(hv.v[qq], r + qq < N2_RT ? lo[r + qq] : hi[r + qq - N2_RT], out[r]);
-      }
-#pragma unroll
-      for (int r = 0; r < N2_RT; ++r) lo[r] = hi[r];
-    }
-  }
 }
 
 template <typename T, bool ADJ>

@@ -532,6 +532,135 @@ class NonStationaryConvolve3D(_KernelOperator):
                    "b2_nsconvolve3d")
 
 
+class _NonStationaryFilters(_KernelOperator):
+    """The shared part of :class:`NonStationaryFilters1D` / :class:`NonStationaryFilters2D`: the fixed real input
+    ``inp`` (uploaded once, in both real precisions), the shape ``(nx, nz, nfx, nfz, nhx, nhz, ohx, dhx, ohz, dhz)``
+    of the 2-D adjoint (a 1-D operator has a singleton x axis), its workspace, sized once here so that no apply has
+    to allocate, and the adjoint launch.  The kernels are real: complex data are applied part by part, and an operator
+    of a complex dtype computes in its real dtype and returns complex results, as a complex NumPy operator would."""
+
+    @staticmethod
+    def _host_input(inp, ndim):
+        """``inp`` on the host, checked: real (``NotImplementedError``) and of rank ``ndim`` (``ValueError``)"""
+        inp = inp.detach().cpu().numpy() if isinstance(inp, torch.Tensor) else np.asarray(inp)
+        if np.iscomplexobj(inp):
+            raise NotImplementedError("complex inp is not supported")
+        if inp.ndim != ndim:
+            raise ValueError(f"inp must have {ndim} dimension(s); got shape {inp.shape}")
+        return inp
+
+    def _setup(self, inp, dims, dimsd, geom, dtype):
+        self.dims, self.dimsd = tuple(dims), tuple(dimsd)
+        self.shape = (math.prod(self.dimsd), math.prod(self.dims))
+        tdt = _lib.torch_dtype(dtype)
+        self._tdtype = _REAL_OF.get(tdt, tdt)       # the kernels' dtype: a complex operator applies data by parts
+        self.dtype = _lib.numpy_dtype(tdt)
+        _lib.ctx()
+        self._inp, self._geom = _real_filters(inp)[1], tuple(int(v) for v in geom)
+        nbytes = C.c_size_t(0)
+        _lib.check(_lib.lib.b2_nsfilters2d_work_bytes(*self._geom, _lib.code(torch.float64), C.byref(nbytes)),
+                   "b2_nsfilters2d_work_bytes")
+        self._work = torch.empty(nbytes.value, dtype=torch.uint8, device="cuda") if nbytes.value else None
+
+    def _complex_data(self, x):
+        """real data of a complex operator as complex data, so that the result is complex"""
+        return x.to(_CPLX_OF[x.dtype]) if self.dtype.kind == "c" and x.dtype in _CPLX_OF else x
+
+    def matvec(self, x, out=None):
+        return self._apply(self._complex_data(x), 0, out)
+
+    def rmatvec(self, x, out=None):
+        return self._apply(self._complex_data(x), 1, out)
+
+    _matvec, _rmatvec = matvec, rmatvec
+
+    def _adjoint(self, x, y, dt):
+        work, nbytes = (self._work.data_ptr(), self._work.numel()) if self._work is not None else (None, 0)
+        _lib.check(_lib.lib.b2_nsfilters2d_adjoint(_lib.ctx(), x.data_ptr(), self._inp[dt].data_ptr(), y.data_ptr(),
+                                                   *self._geom, work, nbytes, _lib.code(dt), _lib.stream()),
+                   "b2_nsfilters2d_adjoint")
+
+
+class NonStationaryFilters1D(_NonStationaryFilters):
+    """Rank-local non-stationary 1-D filter estimation, pylops.signalprocessing.NonStationaryFilters1D (pylops 2.x as
+    remembered: pylops is not installed here to check the signature) inside MPIVStack: time-varying wavelet
+    estimation.  The model is the bank ``(nfilt = len(ih), hsize)`` of filters of odd length at the regularly spaced
+    samples ``ih`` of the fixed real 1-D signal ``inp`` of ``n`` samples; the data are ``(n,)``::
+
+        y[i] = sum_j h_j[hsize // 2 + i - j] inp[j]
+
+    with ``h_j`` interpolated from the model bank as :class:`NonStationaryConvolve1D` interpolates its filters, so
+    ``NonStationaryFilters1D(inp, hsize, ih) @ hs == NonStationaryConvolve1D(n, hs, ih) @ inp``.  The forward is one
+    b2_nsconvolve_axis launch with ``inp`` for the data and the model for the bank; the adjoint, the exact transpose,
+    is one b2_nsfilters2d_adjoint call with a singleton x axis (csrc/nsfilters.cu).  A float32 operator uses ``inp``
+    rounded to float32; complex data are applied to their real and imaginary parts.  ``ValueError`` for an even
+    ``hsize``, irregular or decreasing ``ih``, ``ih`` outside ``[0, n)`` and an ``inp`` that is not 1-D; a complex
+    ``inp`` raises ``NotImplementedError``."""
+
+    def __init__(self, inp, hsize, ih, dtype="float64", name="C"):
+        inp = self._host_input(inp, 1)
+        self.hsize, self.name = int(hsize), name
+        if self.hsize % 2 == 0:
+            raise ValueError("filters hs must have odd length")
+        self.n, self.nfilt = int(inp.shape[0]), len(np.ravel(ih))
+        self.oh, self.dh = _regular_nodes("ih", ih, self.nfilt, self.n)
+        self.hc = self.hsize // 2
+        self._setup(inp, (self.nfilt, self.hsize), (self.n,),
+                    (1, self.n, 1, self.nfilt, 1, self.hsize, 0, 1, self.oh, self.dh), dtype)
+
+    def _launch(self, x, y, dt, adjoint):
+        if adjoint:
+            self._adjoint(x, y, dt)
+            return
+        _lib.check(_lib.lib.b2_nsconvolve_axis(_lib.ctx(), self._inp[dt].data_ptr(), y.data_ptr(), 1, self.n, 1,
+                                               x.data_ptr(), self.nfilt, self.hsize, self.hc, self.oh, self.dh, 0,
+                                               _lib.code(dt), _lib.stream()), "b2_nsconvolve_axis")
+
+
+class NonStationaryFilters2D(_NonStationaryFilters):
+    """Rank-local non-stationary 2-D filter estimation, pylops.signalprocessing.NonStationaryFilters2D (pylops 2.x as
+    remembered: pylops is not installed here to check the signature) inside MPIVStack: estimating a bank of
+    point-spread or deblurring filters.  The model is the bank ``(nfx, nfz, nhx, nhz)`` (``hshape = (nhx, nhz)``,
+    odd) at the regularly spaced points ``(ihx[a], ihz[b])`` of the fixed real image ``inp`` of shape ``(nx, nz)``;
+    the data are ``(nx, nz)``::
+
+        y[i] = sum_j h_j[nhx // 2 + ix - jx, nhz // 2 + iz - jz] inp[j]
+
+    with ``h_j`` bilinear in the model bank as in :class:`NonStationaryConvolve2D`, so
+    ``NonStationaryFilters2D(inp, hshape, ihx, ihz) @ hs == NonStationaryConvolve2D(inp.shape, hs, ihx, ihz) @ inp``.
+    The forward is one b2_nsconvolve2d launch with ``inp`` for the image and the model for the bank; the adjoint,
+    the exact transpose, is b2_nsfilters2d_adjoint (csrc/nsfilters.cu).  A float32 operator uses ``inp`` rounded to
+    float32; complex data are applied to their real and imaginary parts.  ``ValueError`` for even ``hshape`` entries,
+    irregular or decreasing indices, indices outside ``[0, inp.shape)`` and an ``inp`` that is not 2-D; a complex
+    ``inp`` raises ``NotImplementedError``.  ``engine`` and ``num_threads_per_blocks`` are accepted and ignored."""
+
+    def __init__(self, inp, hshape, ihx, ihz, engine="numpy", num_threads_per_blocks=(32, 32), dtype="float64",
+                 name="C"):
+        inp = self._host_input(inp, 2)
+        self.hshape = self.nh = tuple(int(h) for h in hshape)
+        if len(self.nh) != 2:
+            raise ValueError(f"hshape must hold two entries (nhx, nhz); got {hshape}")
+        if self.nh[0] % 2 == 0 or self.nh[1] % 2 == 0:
+            raise ValueError("filters hs must have odd length")
+        nx, nz = (int(v) for v in inp.shape)
+        self.nfilt = (len(np.ravel(ihx)), len(np.ravel(ihz)))
+        self.ohx, self.dhx = _regular_nodes("ihx", ihx, self.nfilt[0], nx)
+        self.ohz, self.dhz = _regular_nodes("ihz", ihz, self.nfilt[1], nz)
+        self.hc = (self.nh[0] // 2, self.nh[1] // 2)
+        self.oh, self.dh = (self.ohx, self.ohz), (self.dhx, self.dhz)
+        self.engine, self.num_threads_per_blocks, self.name = engine, num_threads_per_blocks, name
+        self._setup(inp, self.nfilt + self.nh, (nx, nz),
+                    (nx, nz, *self.nfilt, *self.nh, self.ohx, self.dhx, self.ohz, self.dhz), dtype)
+
+    def _launch(self, x, y, dt, adjoint):
+        if adjoint:
+            self._adjoint(x, y, dt)
+            return
+        _lib.check(_lib.lib.b2_nsconvolve2d(_lib.ctx(), self._inp[dt].data_ptr(), y.data_ptr(), *self.dimsd, 1,
+                                            x.data_ptr(), *self.nfilt, *self.nh, self.ohx, self.dhx, self.ohz,
+                                            self.dhz, 0, _lib.code(dt), _lib.stream()), "b2_nsconvolve2d")
+
+
 class PoststackLinearModelling(_AxisOperator):
     """Rank-local post-stack seismic modelling, pylops.avo.poststack.PoststackLinearModelling (pylops 2.x) for a
     real wavelet, as tutorials/poststack.py uses it inside MPIBlockDiag::
