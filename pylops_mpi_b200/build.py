@@ -56,7 +56,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
                 and os.path.getmtime(obj) > os.path.getmtime(os.path.join(CSRC, "tc_ptx.cuh"))
                 and os.path.getmtime(obj) > os.path.getmtime(os.path.join(CSRC, "fd_axis.cuh"))
                 and os.path.getmtime(obj) > os.path.getmtime(os.path.join(CSRC, "peer.cuh"))
-                and os.path.getmtime(obj) > os.path.getmtime(os.path.join(CSRC, "ns2_core.cuh"))
+                and os.path.getmtime(obj) > os.path.getmtime(os.path.join(CSRC, "ns_core.cuh"))
                 and os.path.getmtime(obj) > os.path.getmtime(os.path.join(INCLUDE, "b200lops.h"))):
             continue
         cmd = [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",

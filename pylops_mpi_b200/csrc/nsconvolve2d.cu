@@ -25,40 +25,18 @@
 // in ascending (x, z) order (forward: of the reversed filter), one fma per term.  No atomics, no allocation: repeated
 // applies give identical bits.  The sums differ from pylops' (interpolate h_j, then convolve) only in rounding; with
 // exactly representable inputs both are exact.
-#include "ns2_core.cuh"
+#include "ns_core.cuh"
 
 namespace {
 
 struct Ns2Params {
-  Axis ax[2];            // x, z
+  AxisT<long long> ax[2];   // x, z
   long long tiles_z;
   long long n_inner;
 };
 
-// taps [qlo, qhi) of filter a that can meet its support from a tile of nt outputs at i0 (window row m = sample jb + m)
-__device__ __forceinline__ bool tap_span(const Axis& A, int a, long long i0, long long jb, int nt, bool adj, int& qlo,
-                                         int& qhi) {
-  long long lo, hi;
-  support(A, a, lo, hi);
-  long long q0, q1;
-  if (!adj) {                     // outputs t in [0, nt) read the rows t + q; the non-zero rows are the support's
-    q0 = lo - jb - nt + 1;
-    q1 = hi - jb;
-  } else {                        // the outputs in the support read the rows t + q; the non-zero rows are [0, n)'s
-    const long long tlo = max(lo - i0, 0LL), thi = min(hi - i0, (long long)nt);
-    if (tlo >= thi) return false;
-    q0 = -jb - thi + 1;
-    q1 = A.n - jb - tlo;
-  }
-  q0 = max(q0, 0LL);
-  q1 = min(q1, (long long)A.nh);
-  qlo = (int)q0;
-  qhi = (int)q1;
-  return q0 < q1;
-}
-
 template <typename T, bool ADJ>
-__global__ void __launch_bounds__(N2_THREADS, 2)
+__global__ void __launch_bounds__(NS_THREADS, 2)
 ns2_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restrict__ hs, const Ns2Params p) {
   extern __shared__ __align__(64) unsigned char ns2_smem[];
   T* w = reinterpret_cast<T*>(ns2_smem);                          // [WR][WS] window
@@ -66,29 +44,24 @@ ns2_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restrict__ hs,
   double* wgx = reinterpret_cast<double*>(hk + N2_KC * N2_KC);     // [WR] x weights of the window rows (forward)
   double* wgz = wgx + N2_WR;                                       // [WC] z weights of the window columns (forward)
 
-  const Axis& X = p.ax[0];
-  const Axis& Z = p.ax[1];
+  const auto& X = p.ax[0];
+  const auto& Z = p.ax[1];
   const long long ci = blockIdx.y;
-  const long long i0x = (long long)(blockIdx.x / p.tiles_z) * N2_TX, i0z = (long long)(blockIdx.x % p.tiles_z) * N2_TZ;
-  const int tid = threadIdx.x, lane = tid % N2_LANES, t0 = tid / N2_LANES * N2_RT;
+  const long long i0x = (long long)(blockIdx.x / p.tiles_z) * N2_TX, i0z = (long long)(blockIdx.x % p.tiles_z) * NS_TZ;
+  const int tid = threadIdx.x, lane = tid % NS_LANES, t0 = tid / NS_LANES * NS_RT;
   // window origin (sample of row / column 0) and the filters whose support can reach the tile
   const long long jbx = ADJ ? i0x - X.hc : i0x + X.hc - X.nh + 1;
   const long long jbz = ADJ ? i0z - Z.hc : i0z + Z.hc - Z.nh + 1;
   int af[2], al[2];
   {
     const long long lo[2] = {ADJ ? i0x : jbx, ADJ ? i0z : jbz};
-    const long long hi[2] = {ADJ ? i0x + N2_TX : jbx + N2_TX + X.nh - 1, ADJ ? i0z + N2_TZ : jbz + N2_TZ + Z.nh - 1};
+    const long long hi[2] = {ADJ ? i0x + N2_TX : jbx + N2_TX + X.nh - 1, ADJ ? i0z + NS_TZ : jbz + NS_TZ + Z.nh - 1};
 #pragma unroll
-    for (int d = 0; d < 2; ++d) {
-      const Axis& A = p.ax[d];
-      const long long l = max(lo[d], 0LL), h = min(hi[d], A.n);
-      af[d] = (int)min(max(floor_div(l - A.oh, A.dh), 0LL), (long long)A.nf - 1);
-      al[d] = (int)min(max(floor_div(h - 1 - A.oh + A.dh - 1, A.dh), 0LL), (long long)A.nf - 1);
-    }
+    for (int d = 0; d < 2; ++d) filter_span(p.ax[d], lo[d], hi[d], af[d], al[d]);
   }
-  T acc[N2_RT];
+  T acc[NS_RT];
 #pragma unroll
-  for (int r = 0; r < N2_RT; ++r) acc[r] = T(0);
+  for (int r = 0; r < NS_RT; ++r) acc[r] = T(0);
 
   for (int a = af[0]; a <= al[0]; ++a) {
     int qxlo, qxhi;
@@ -97,22 +70,22 @@ ns2_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restrict__ hs,
     support(X, a, sxlo, sxhi);
     for (int b = af[1]; b <= al[1]; ++b) {
       int qzlo, qzhi;
-      if (!tap_span(Z, b, i0z, jbz, N2_TZ, ADJ, qzlo, qzhi)) continue;
+      if (!tap_span(Z, b, i0z, jbz, NS_TZ, ADJ, qzlo, qzhi)) continue;
       long long szlo, szhi;
       support(Z, b, szlo, szhi);
       const T* hc = hs + ((size_t)a * Z.nf + b) * (size_t)X.nh * Z.nh;
-      T v[N2_RT];
+      T v[NS_RT];
 #pragma unroll
-      for (int r = 0; r < N2_RT; ++r) v[r] = T(0);
+      for (int r = 0; r < NS_RT; ++r) v[r] = T(0);
       for (int cx = qxlo; cx < qxhi; cx += N2_KC) {
         const int nqx = min(N2_KC, qxhi - cx);
         const int nwr = N2_TX + nqx - 1;                            // window rows the chunk reads
         for (int cz = qzlo; cz < qzhi; cz += N2_KC) {
-          const int nqz = min(N2_KC, qzhi - cz), nqz8 = (nqz + N2_RT - 1) / N2_RT * N2_RT;
-          const int nwc = N2_TZ + nqz - 1;                          // window columns with a non-zero tap
+          const int nqz = min(N2_KC, qzhi - cz), nqz8 = (nqz + NS_RT - 1) / NS_RT * NS_RT;
+          const int nwc = NS_TZ + nqz - 1;                          // window columns with a non-zero tap
           __syncthreads();                                          // the previous chunk's readers are done
           if constexpr (!ADJ) {
-            for (int m = tid; m < N2_WR + N2_WC; m += N2_THREADS) {
+            for (int m = tid; m < N2_WR + N2_WC; m += NS_THREADS) {
               if (m < N2_WR) {
                 const long long j = jbx + cx + m;
                 wgx[m] = (j >= sxlo && j < sxhi) ? axis_weight(X, a, j) : 0.0;
@@ -123,7 +96,7 @@ ns2_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restrict__ hs,
             }
             __syncthreads();
           }
-          for (int e = tid; e < nwr * N2_WC; e += N2_THREADS) {
+          for (int e = tid; e < nwr * N2_WC; e += NS_THREADS) {
             const int r = e / N2_WC, c = e - r * N2_WC;
             const long long jx = jbx + cx + r, jz = jbz + cz + c;
             T val = T(0);
@@ -139,7 +112,7 @@ ns2_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restrict__ hs,
             }
             w[r * N2_WS + c] = val;
           }
-          for (int e = tid; e < nqx * N2_KC; e += N2_THREADS) {
+          for (int e = tid; e < nqx * N2_KC; e += NS_THREADS) {
             const int qx = e / N2_KC, qz = e - qx * N2_KC;
             T tap = T(0);
             if (qz < nqz) {
@@ -158,7 +131,7 @@ ns2_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restrict__ hs,
         if (jx >= sxlo && jx < sxhi) {
           const double wx = axis_weight(X, a, jx);
 #pragma unroll
-          for (int r = 0; r < N2_RT; ++r) {
+          for (int r = 0; r < NS_RT; ++r) {
             const long long jz = i0z + t0 + r;
             if (jz >= szlo && jz < szhi) acc[r] = fma(T(axis_weight(Z, b, jz) * wx), v[r], acc[r]);
           }
@@ -169,7 +142,7 @@ ns2_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restrict__ hs,
   const long long ix = i0x + lane;
   if (ix >= X.n) return;
 #pragma unroll
-  for (int r = 0; r < N2_RT; ++r) {
+  for (int r = 0; r < NS_RT; ++r) {
     const long long iz = i0z + t0 + r;
     if (iz < Z.n) __stcs(y + ((size_t)ix * Z.n + iz) * p.n_inner + ci, acc[r]);
   }
@@ -180,7 +153,7 @@ int launch_ns2(const void* x, void* y, const void* hs, const Ns2Params& p, long 
   const size_t smem = (size_t)(N2_WELEMS + N2_KC * N2_KC) * sizeof(T) + (size_t)(N2_WR + N2_WC) * sizeof(double);
   const int rc = b2_allow_smem<ns2_kernel<T, ADJ>>(smem);
   if (rc != B2_OK) return rc;
-  ns2_kernel<T, ADJ><<<dim3((unsigned)(tiles_x * p.tiles_z), (unsigned)p.n_inner), N2_THREADS, smem, st>>>(
+  ns2_kernel<T, ADJ><<<dim3((unsigned)(tiles_x * p.tiles_z), (unsigned)p.n_inner), NS_THREADS, smem, st>>>(
       static_cast<const T*>(x), static_cast<T*>(y), static_cast<const T*>(hs), p);
   B2_LAUNCH_CHECK();
   return B2_OK;
@@ -191,14 +164,11 @@ int launch_ns2(const void* x, void* y, const void* hs, const Ns2Params& p, long 
 extern "C" int b2_nsconvolve2d(b2_ctx* ctx, const void* x, void* y, size_t nx, size_t nz, size_t n_inner,
                                const void* hs, int nfx, int nfz, int nhx, int nhz, long long ohx, long long dhx,
                                long long ohz, long long dhz, int adjoint, int dtype, void* stream) {
-  if (!ctx || !x || !y || !hs || x == y) return B2_ERR_ARG;
-  if (nx == 0 || nz == 0 || (n_inner != 1 && n_inner != 2)) return B2_ERR_ARG;
-  if (nfx < 1 || nfz < 1 || nhx < 1 || nhz < 1 || dhx < 1 || dhz < 1) return B2_ERR_ARG;
+  if (!ctx || !x || !y || !hs || x == y || (n_inner != 1 && n_inner != 2)) return B2_ERR_ARG;
   Ns2Params p;
-  p.ax[0] = Axis{(long long)nx, ohx, dhx, nfx, nhx, nhx / 2};
-  p.ax[1] = Axis{(long long)nz, ohz, dhz, nfz, nhz, nhz / 2};
+  if (!make_axis(nx, nfx, nhx, ohx, dhx, p.ax[0]) || !make_axis(nz, nfz, nhz, ohz, dhz, p.ax[1])) return B2_ERR_ARG;
   p.n_inner = (long long)n_inner;
-  p.tiles_z = (long long)((nz + N2_TZ - 1) / N2_TZ);
+  p.tiles_z = (long long)((nz + NS_TZ - 1) / NS_TZ);
   const long long tiles_x = (long long)((nx + N2_TX - 1) / N2_TX);
   if (tiles_x > 0x7fffffffLL / p.tiles_z) return B2_ERR_ARG;      // one 1-D grid holds every tile
   return b2_dispatch_real(dtype, [&](auto t) {

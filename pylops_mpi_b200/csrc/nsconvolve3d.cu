@@ -18,9 +18,9 @@
 // meet the support.  The 3-D correlation is a sum over x tap planes of 2-D correlations: the CTA stages one (y, z)
 // input plane at a time in shared memory (double-buffered, one barrier per plane), and each staged plane feeds every
 // one of the TX output planes it reaches (tap plane = input plane - output plane), so a window value loaded into
-// registers serves up to TX tap planes.  Within a plane the tile is nsconvolve2d.cu's: lanes of a warp run along y
-// (one output row each, every tap a broadcast), a thread's RT = 8 consecutive z outputs slide a register window along
-// z, and the window row stride is odd.  Taps go in chunks of KCX x KCY x KCZ: any filter size fits the fixed shared
+// registers serves up to TX tap planes (correlate_plane, ns_core.cuh).  Within a plane the tile is nsconvolve2d.cu's
+// with its own chunk size: lanes of a warp run along y (one output row each, every tap a broadcast), a thread's RT = 8
+// consecutive z outputs slide a register window along z, and the window row stride is odd.  Taps go in chunks of KCX x KCY x KCZ: any filter size fits the fixed shared
 // memory, filters larger than the volume included.
 //   forward  the window holds u_c = W_c . x (zero off S_c) and the taps are reversed: acc[t] += h_c[K-1-q] u_c[t + q]
 //   adjoint  the window holds y, v[t] += h_c[q] y[t + q] over the whole filter, then acc[t] = fma(W_c[t], v[t], acc[t])
@@ -28,17 +28,15 @@
 // chunk in ascending (x, y, z) order (forward: of the reversed filter), one fma per term.  No atomics, no allocation:
 // repeated applies give identical bits.  The sums differ from pylops' (interpolate h_j, then convolve) only in
 // rounding; with exactly representable inputs both are exact.
-#include "common.cuh"
+#include "ns_core.cuh"
 
 namespace {
 
-constexpr int N3_LANES = 32, N3_GROUPS = 8, N3_THREADS = N3_LANES * N3_GROUPS;
-constexpr int N3_RT = 8;                                   // consecutive z outputs per thread
-constexpr int N3_TY = N3_LANES, N3_TZ = N3_GROUPS * N3_RT;   // outputs per plane of a CTA: 32 (y) x 64 (z)
+constexpr int N3_TY = NS_LANES;                            // outputs per plane of a CTA: 32 (y) x 64 (z)
 constexpr int N3_KCX = 16;                                 // tap planes per chunk (x)
-constexpr int N3_KC = 16;                                  // taps per chunk along y and z (a multiple of N3_RT)
+constexpr int N3_KC = 16;                                  // taps per chunk along y and z (a multiple of NS_RT)
 constexpr int N3_WR = N3_TY + N3_KC - 1;                   // window rows (y)
-constexpr int N3_WC = N3_TZ + N3_KC;                       // window columns (z): the register window reads one past
+constexpr int N3_WC = NS_TZ + N3_KC;                       // window columns (z): the register window reads one past
 constexpr int N3_WS = N3_WC + 1;                           // odd row stride: the lanes' rows fall in different banks
 constexpr int N3_WELEMS = (N3_WR * N3_WS + 15) / 16 * 16;  // one window plane, padded so the taps stay vector-aligned
 
@@ -47,102 +45,15 @@ constexpr int N3_WELEMS = (N3_WR * N3_WS + 15) / 16 * 16;  // one window plane, 
 template <typename T, bool ADJ>
 constexpr int N3_TX = sizeof(T) == 4 ? (ADJ ? 2 : 4) : 1;
 
-// Axis, floor_div, support, axis_weight and tap_span are nsconvolve2d.cu's in 32-bit coordinates: in 64 bits the
-// third axis's state does not fit the registers (every variant spilled), and sharing them would change the 2-D code
-struct Axis {
-  int n, oh, dh;
-  int nf, nh, hc;
-};
-
+// coordinates are 32-bit: in 64 bits the third axis's state does not fit the registers (every variant spilled)
 struct Ns3Params {
-  Axis ax[3];            // x, y, z
+  AxisT<int> ax[3];      // x, y, z
   int tiles_y, tiles_z;
   int n_inner;
 };
 
-__device__ __forceinline__ int floor_div(int a, int b) {   // b > 0
-  const int q = a / b;
-  return (a % b != 0 && a < 0) ? q - 1 : q;
-}
-
-// [lo, hi): the samples of [0, n) with a non-zero weight on filter a
-__device__ __forceinline__ void support(const Axis& A, int a, int& lo, int& hi) {
-  lo = a == 0 ? 0 : A.oh + (a - 1) * A.dh + 1;
-  hi = a == A.nf - 1 ? A.n : A.oh + (a + 1) * A.dh;
-  lo = max(lo, 0);
-  hi = min(hi, A.n);
-}
-
-// the float64 weight of filter a at sample j
-__device__ __forceinline__ double axis_weight(const Axis& A, int a, int j) {
-  const double v = (double)(j - A.oh) / (double)A.dh;
-  const double fl = floor(v);
-  if (fl < 0.0) return a == 0 ? 1.0 : 0.0;
-  if (fl >= (double)(A.nf - 1)) return a == A.nf - 1 ? 1.0 : 0.0;
-  const int l = (int)fl;
-  if (a == l) return 1.0 - (v - fl);
-  return a == l + 1 ? v - fl : 0.0;
-}
-
-// taps [qlo, qhi) of filter a that can meet its support from a tile of nt outputs at i0 (window index m = sample
-// jb + m)
-__device__ __forceinline__ bool tap_span(const Axis& A, int a, int i0, int jb, int nt, bool adj, int& qlo,
-                                         int& qhi) {
-  int lo, hi;
-  support(A, a, lo, hi);
-  int q0, q1;
-  if (!adj) {                     // outputs t in [0, nt) read t + q; the non-zero inputs are the support's
-    q0 = lo - jb - nt + 1;
-    q1 = hi - jb;
-  } else {                        // the outputs in the support read t + q; the non-zero inputs are [0, n)'s
-    const int tlo = max(lo - i0, 0), thi = min(hi - i0, nt);
-    if (tlo >= thi) return false;
-    q0 = -jb - thi + 1;
-    q1 = A.n - jb - tlo;
-  }
-  q0 = max(q0, 0);
-  q1 = min(q1, A.nh);
-  qlo = q0;
-  qhi = q1;
-  return q0 < q1;
-}
-
-// for every output plane t whose tap plane m - t lies in [0, nqx):
-//   out[t][r] += sum_(qy < nqy, qz < nqz8) hk[m - t][qy][qz] w[lane + qy][t0 + r + qz]
-// one window row in registers serves every such t
-template <typename T, int TX>
-__device__ __forceinline__ void correlate_plane(T (&out)[TX][N3_RT], const T* __restrict__ w, const T* __restrict__ hk,
-                                                int m, int nqx, int nqy, int nqz8, int lane, int t0) {
-  using VA = VecN<T, N3_RT>;
-  for (int qy = 0; qy < nqy; ++qy) {
-    const T* wr = w + (lane + qy) * N3_WS + t0;
-    T lo[N3_RT];
-#pragma unroll
-    for (int r = 0; r < N3_RT; ++r) lo[r] = wr[r];
-    for (int q0 = 0; q0 < nqz8; q0 += N3_RT) {
-      T hi[N3_RT];
-#pragma unroll
-      for (int r = 0; r < N3_RT; ++r) hi[r] = wr[q0 + N3_RT + r];
-#pragma unroll
-      for (int t = 0; t < TX; ++t) {
-        const int qx = m - t;
-        if (qx < 0 || qx >= nqx) continue;
-        const VA hv = *reinterpret_cast<const VA*>(hk + (qx * N3_KC + qy) * N3_KC + q0);
-#pragma unroll
-        for (int qq = 0; qq < N3_RT; ++qq) {
-#pragma unroll
-          for (int r = 0; r < N3_RT; ++r)
-            out[t][r] = fma(hv.v[qq], r + qq < N3_RT ? lo[r + qq] : hi[r + qq - N3_RT], out[t][r]);
-        }
-      }
-#pragma unroll
-      for (int r = 0; r < N3_RT; ++r) lo[r] = hi[r];
-    }
-  }
-}
-
 template <typename T, bool ADJ>
-__global__ void __launch_bounds__(N3_THREADS, 2)
+__global__ void __launch_bounds__(NS_THREADS, 2)
 ns3_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restrict__ hs, const Ns3Params p) {
   constexpr int TX = N3_TX<T, ADJ>;
   constexpr int NP = TX + N3_KCX - 1;                               // window planes of a full x chunk
@@ -153,14 +64,14 @@ ns3_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restrict__ hs,
   double* wgy = wgx + NP;                                           // [WR] y weights of the rows (forward)
   double* wgz = wgy + N3_WR;                                        // [WC] z weights of the columns (forward)
 
-  const Axis& X = p.ax[0];
-  const Axis& Y = p.ax[1];
-  const Axis& Z = p.ax[2];
+  const auto& X = p.ax[0];
+  const auto& Y = p.ax[1];
+  const auto& Z = p.ax[2];
   const int ci = blockIdx.y;
   const int tyz = p.tiles_y * p.tiles_z;
   const int bx = blockIdx.x / tyz, byz = blockIdx.x % tyz;
-  const int i0x = bx * TX, i0y = (byz / p.tiles_z) * N3_TY, i0z = (byz % p.tiles_z) * N3_TZ;
-  const int tid = threadIdx.x, lane = tid % N3_LANES, t0 = tid / N3_LANES * N3_RT;
+  const int i0x = bx * TX, i0y = (byz / p.tiles_z) * N3_TY, i0z = (byz % p.tiles_z) * NS_TZ;
+  const int tid = threadIdx.x, lane = tid % NS_LANES, t0 = tid / NS_LANES * NS_RT;
   // window origin (sample of plane / row / column 0) and the filters whose support can reach the tile
   const int jbx = ADJ ? i0x - X.hc : i0x + X.hc - X.nh + 1;
   const int jby = ADJ ? i0y - Y.hc : i0y + Y.hc - Y.nh + 1;
@@ -169,20 +80,15 @@ ns3_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restrict__ hs,
   {
     const int lo[3] = {ADJ ? i0x : jbx, ADJ ? i0y : jby, ADJ ? i0z : jbz};
     const int hi[3] = {ADJ ? i0x + TX : jbx + TX + X.nh - 1, ADJ ? i0y + N3_TY : jby + N3_TY + Y.nh - 1,
-                             ADJ ? i0z + N3_TZ : jbz + N3_TZ + Z.nh - 1};
+                             ADJ ? i0z + NS_TZ : jbz + NS_TZ + Z.nh - 1};
 #pragma unroll
-    for (int d = 0; d < 3; ++d) {
-      const Axis& A = p.ax[d];
-      const int l = max(lo[d], 0), h = min(hi[d], A.n);
-      af[d] = min(max(floor_div(l - A.oh, A.dh), 0), A.nf - 1);
-      al[d] = min(max(floor_div(h - 1 - A.oh + A.dh - 1, A.dh), 0), A.nf - 1);
-    }
+    for (int d = 0; d < 3; ++d) filter_span(p.ax[d], lo[d], hi[d], af[d], al[d]);
   }
-  T acc[TX][N3_RT];
+  T acc[TX][NS_RT];
 #pragma unroll
   for (int t = 0; t < TX; ++t)
 #pragma unroll
-    for (int r = 0; r < N3_RT; ++r) acc[t][r] = T(0);
+    for (int r = 0; r < NS_RT; ++r) acc[t][r] = T(0);
 
   for (int a = af[0]; a <= al[0]; ++a) {
     int qxlo, qxhi;
@@ -196,15 +102,15 @@ ns3_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restrict__ hs,
       support(Y, b, sylo, syhi);
       for (int e = af[2]; e <= al[2]; ++e) {
         int qzlo, qzhi;
-        if (!tap_span(Z, e, i0z, jbz, N3_TZ, ADJ, qzlo, qzhi)) continue;
+        if (!tap_span(Z, e, i0z, jbz, NS_TZ, ADJ, qzlo, qzhi)) continue;
         int szlo, szhi;
         support(Z, e, szlo, szhi);
         const T* hc = hs + (((size_t)a * Y.nf + b) * Z.nf + e) * (size_t)X.nh * Y.nh * Z.nh;
-        T v[TX][N3_RT];
+        T v[TX][NS_RT];
 #pragma unroll
         for (int t = 0; t < TX; ++t)
 #pragma unroll
-          for (int r = 0; r < N3_RT; ++r) v[t][r] = T(0);
+          for (int r = 0; r < NS_RT; ++r) v[t][r] = T(0);
         for (int cx = qxlo; cx < qxhi; cx += N3_KCX) {
           const int nqx = min(N3_KCX, qxhi - cx);
           const int np = TX + nqx - 1;                              // window planes the chunk reads
@@ -212,11 +118,11 @@ ns3_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restrict__ hs,
             const int nqy = min(N3_KC, qyhi - cy);
             const int nwr = N3_TY + nqy - 1;                        // window rows the chunk reads
             for (int cz = qzlo; cz < qzhi; cz += N3_KC) {
-              const int nqz = min(N3_KC, qzhi - cz), nqz8 = (nqz + N3_RT - 1) / N3_RT * N3_RT;
-              const int nwc = N3_TZ + nqz - 1;                      // window columns with a non-zero tap
+              const int nqz = min(N3_KC, qzhi - cz), nqz8 = (nqz + NS_RT - 1) / NS_RT * NS_RT;
+              const int nwc = NS_TZ + nqz - 1;                      // window columns with a non-zero tap
               __syncthreads();                                      // the previous chunk's readers are done
               if constexpr (!ADJ) {
-                for (int m = tid; m < NP + N3_WR + N3_WC; m += N3_THREADS) {
+                for (int m = tid; m < NP + N3_WR + N3_WC; m += NS_THREADS) {
                   if (m < NP) {
                     const int j = jbx + cx + m;
                     wgx[m] = (j >= sxlo && j < sxhi) ? axis_weight(X, a, j) : 0.0;
@@ -229,7 +135,7 @@ ns3_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restrict__ hs,
                   }
                 }
               }
-              for (int s = tid; s < nqx * N3_KC * N3_KC; s += N3_THREADS) {
+              for (int s = tid; s < nqx * N3_KC * N3_KC; s += NS_THREADS) {
                 const int qx = s / (N3_KC * N3_KC), qy = s / N3_KC % N3_KC, qz = s % N3_KC;
                 T tap = T(0);
                 if (qy < nqy && qz < nqz) {
@@ -245,7 +151,7 @@ ns3_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restrict__ hs,
                 T* wm = w + (m & 1) * N3_WELEMS;
                 const int jx = jbx + cx + m;
                 const bool in_x = ADJ ? (jx >= 0 && jx < X.n) : wgx[m] != 0.0;
-                for (int s = tid; s < nwr * N3_WC; s += N3_THREADS) {
+                for (int s = tid; s < nwr * N3_WC; s += NS_THREADS) {
                   const int r = s / N3_WC, c = s - r * N3_WC;
                   const int jy = jby + cy + r, jz = jbz + cz + c;
                   T val = T(0);
@@ -263,8 +169,8 @@ ns3_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restrict__ hs,
                 }
                 __syncthreads();                                    // plane m staged; plane m - 1's readers are done
                 if (!in_x) continue;                                // an all-zero plane adds nothing
-                if constexpr (ADJ) correlate_plane<T, TX>(v, wm, hk, m, nqx, nqy, nqz8, lane, t0);
-                else correlate_plane<T, TX>(acc, wm, hk, m, nqx, nqy, nqz8, lane, t0);
+                if constexpr (ADJ) correlate_plane<T, TX, N3_KC, N3_WS>(v, wm, hk, m, nqx, nqy, nqz8, lane, t0);
+                else correlate_plane<T, TX, N3_KC, N3_WS>(acc, wm, hk, m, nqx, nqy, nqz8, lane, t0);
               }
             }
           }
@@ -279,7 +185,7 @@ ns3_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restrict__ hs,
               if (jx < sxlo || jx >= sxhi) continue;
               const double wx = axis_weight(X, a, jx);
 #pragma unroll
-              for (int r = 0; r < N3_RT; ++r) {
+              for (int r = 0; r < NS_RT; ++r) {
                 const int jz = i0z + t0 + r;
                 if (jz >= szlo && jz < szhi) acc[t][r] = fma(T(axis_weight(Z, e, jz) * wy * wx), v[t][r], acc[t][r]);
               }
@@ -296,7 +202,7 @@ ns3_kernel(const T* __restrict__ x, T* __restrict__ y, const T* __restrict__ hs,
     const int ix = i0x + t;
     if (ix >= X.n) break;
 #pragma unroll
-    for (int r = 0; r < N3_RT; ++r) {
+    for (int r = 0; r < NS_RT; ++r) {
       const int iz = i0z + t0 + r;
       if (iz < Z.n) __stcs(y + (((size_t)ix * Y.n + iy) * Z.n + iz) * p.n_inner + ci, acc[t][r]);
     }
@@ -313,7 +219,7 @@ int launch_ns3(const void* x, void* y, const void* hs, const Ns3Params& p, size_
                       (size_t)(NP + N3_WR + N3_WC) * sizeof(double);
   const int rc = b2_allow_smem<ns3_kernel<T, ADJ>>(smem);
   if (rc != B2_OK) return rc;
-  ns3_kernel<T, ADJ><<<dim3((unsigned)(tiles_x * p.tiles_y * p.tiles_z), (unsigned)p.n_inner), N3_THREADS, smem, st>>>(
+  ns3_kernel<T, ADJ><<<dim3((unsigned)(tiles_x * p.tiles_y * p.tiles_z), (unsigned)p.n_inner), NS_THREADS, smem, st>>>(
       static_cast<const T*>(x), static_cast<T*>(y), static_cast<const T*>(hs), p);
   B2_LAUNCH_CHECK();
   return B2_OK;
@@ -325,29 +231,14 @@ extern "C" int b2_nsconvolve3d(b2_ctx* ctx, const void* x, void* y, size_t nx, s
                                const void* hs, int nfx, int nfy, int nfz, int nhx, int nhy, int nhz, long long ohx,
                                long long dhx, long long ohy, long long dhy, long long ohz, long long dhz, int adjoint,
                                int dtype, void* stream) {
-  if (!ctx || !x || !y || !hs || x == y) return B2_ERR_ARG;
-  if (nx == 0 || ny == 0 || nz == 0 || (n_inner != 1 && n_inner != 2)) return B2_ERR_ARG;
-  if (nfx < 1 || nfy < 1 || nfz < 1 || nhx < 1 || nhy < 1 || nhz < 1 || dhx < 1 || dhy < 1 || dhz < 1)
+  if (!ctx || !x || !y || !hs || x == y || (n_inner != 1 && n_inner != 2)) return B2_ERR_ARG;
+  Ns3Params p;   // 32-bit axes: make_axis refuses an axis, filter size or node position of 2^29 samples or more
+  if (!make_axis(nx, nfx, nhx, ohx, dhx, p.ax[0]) || !make_axis(ny, nfy, nhy, ohy, dhy, p.ax[1]) ||
+      !make_axis(nz, nfz, nhz, ohz, dhz, p.ax[2]))
     return B2_ERR_ARG;
-  // the kernel's coordinates are 32-bit: every axis, filter and node position stays below 2^29 samples, so that no
-  // sum of two of them overflows (one filter takes any step: its weight is 1 everywhere)
-  constexpr long long LIM = 1LL << 29;
-  const long long n[3] = {(long long)min(nx, (size_t)LIM), (long long)min(ny, (size_t)LIM),
-                          (long long)min(nz, (size_t)LIM)};
-  const int nf[3] = {nfx, nfy, nfz}, nh[3] = {nhx, nhy, nhz};
-  const long long oh[3] = {ohx, ohy, ohz};
-  long long dh[3] = {dhx, dhy, dhz};
-  Ns3Params p;
-  for (int d = 0; d < 3; ++d) {
-    if (nf[d] == 1) dh[d] = 1;
-    if (n[d] >= LIM || nh[d] >= LIM || oh[d] <= -LIM || oh[d] >= LIM || dh[d] >= LIM ||
-        oh[d] + (nf[d] - 1) * dh[d] >= LIM)
-      return B2_ERR_ARG;
-    p.ax[d] = Axis{(int)n[d], (int)oh[d], (int)dh[d], nf[d], nh[d], nh[d] / 2};
-  }
   p.n_inner = (int)n_inner;
   p.tiles_y = (int)((ny + N3_TY - 1) / N3_TY);
-  p.tiles_z = (int)((nz + N3_TZ - 1) / N3_TZ);
+  p.tiles_z = (int)((nz + NS_TZ - 1) / NS_TZ);
   return b2_dispatch_real(dtype, [&](auto t) {
     using T = decltype(t);
     return adjoint ? launch_ns3<T, true>(x, y, hs, p, nx, (cudaStream_t)stream)

@@ -4,13 +4,13 @@
 // with x = inp and hs = the model); this file holds its exact transpose,
 //   g_c[kx][kz] = sum_(j in S_c) W_c[j] inp[j] d[jx + kx - hcx][jz + kz - hcz]       (terms outside the image are 0)
 // for the bank g [nfx][nfz][nhx][nhz], c = (a, b), W_c[j] = T(wx_a(jx) * wz_b(jz)) and S_c the support of filter c,
-// both exactly as in nsconvolve2d.cu (ns2_core.cuh): the cells around the node, to the image edge for end filters.
+// both exactly as in nsconvolve2d.cu (ns_core.cuh): the cells around the node, to the image edge for end filters.
 //
 // Scheme: for each filter this is a STATIONARY correlation of d with the weighted patch u_c = W_c . inp, evaluated at
 // the nhx x nhz lags: the correlation of nsconvolve2d.cu with outputs and taps swapped.  A CTA owns a 32 x 64 tile of
 // one filter's taps (lanes along kx, RT = 8 consecutive kz per thread in the register sliding window) and one PART of
 // that filter's support.  It walks the part in 32 x 32 chunks: u_c of the chunk goes to shared memory in the place of
-// the taps and d's window at origin (chunk + tap tile - hc) in the place of the image, and correlate (ns2_core.cuh)
+// the taps and d's window at origin (chunk + tap tile - hc) in the place of the image, and correlate (ns_core.cuh)
 // adds one fma per term.  The support is split into a number of parts that depends on the shape alone (enough CTAs to
 // fill the GPU when there are few filters with huge supports, one part when there are many); with more than one part
 // each CTA writes its partial tap tile to the workspace and a second launch folds the parts.
@@ -22,7 +22,7 @@
 // inputs both are exact.
 #include <algorithm>
 
-#include "ns2_core.cuh"
+#include "ns_core.cuh"
 
 namespace {
 
@@ -30,7 +30,7 @@ constexpr long long NF_TARGET_CTAS = 1024;   // a part count that reaches this m
 constexpr long long NF_MIN_CHUNKS = 4;       // but a part keeps at least this many chunks of its filter's support
 
 struct NfPlan {
-  Axis ax[2];            // x, z
+  AxisT<long long> ax[2];   // x, z
   int ktx, ktz;          // tap tiles per filter
   int px, pz;            // parts per filter along x, z
   long long cpx, cpz;    // support chunks per part along x, z
@@ -41,10 +41,8 @@ struct NfPlan {
 // the plan of a shape; false for a shape the entry points refuse
 bool nf_plan(size_t nx, size_t nz, int nfx, int nfz, int nhx, int nhz, long long ohx, long long dhx, long long ohz,
              long long dhz, NfPlan& p) {
-  if (nx == 0 || nz == 0 || nfx < 1 || nfz < 1 || nhx < 1 || nhz < 1 || dhx < 1 || dhz < 1) return false;
+  if (!make_axis(nx, nfx, nhx, ohx, dhx, p.ax[0]) || !make_axis(nz, nfz, nhz, ohz, dhz, p.ax[1])) return false;
   if (nx > (1ULL << 40) || nz > (1ULL << 40) || nz > (1ULL << 50) / nx) return false;   // nx nz <= 2^50: no wrap
-  p.ax[0] = Axis{(long long)nx, ohx, dhx, nfx, nhx, nhx / 2};
-  p.ax[1] = Axis{(long long)nz, ohz, dhz, nfz, nhz, nhz / 2};
   long long mc[2] = {1, 1};                 // the most support chunks of any filter, per axis
   for (int d = 0; d < 2; ++d)
     for (int a = 0; a < p.ax[d].nf; ++a) {
@@ -53,7 +51,7 @@ bool nf_plan(size_t nx, size_t nz, int nfx, int nfz, int nhx, int nhz, long long
       mc[d] = std::max(mc[d], (hi - lo + N2_KC - 1) / N2_KC);
     }
   p.ktx = (nhx + N2_TX - 1) / N2_TX;
-  p.ktz = (nhz + N2_TZ - 1) / N2_TZ;
+  p.ktz = (nhz + NS_TZ - 1) / NS_TZ;
   const long long base = (long long)nfx * nfz * p.ktx * p.ktz;
   long long want = std::min((NF_TARGET_CTAS + base - 1) / base, std::max(mc[0] * mc[1] / NF_MIN_CHUNKS, 1LL));
   p.cpx = (mc[0] + std::min(mc[0], want) - 1) / std::min(mc[0], want);
@@ -69,7 +67,7 @@ bool nf_plan(size_t nx, size_t nz, int nfx, int nfz, int nhx, int nhz, long long
 }
 
 template <typename T>
-__global__ void __launch_bounds__(N2_THREADS, 2)
+__global__ void __launch_bounds__(NS_THREADS, 2)
 nf_kernel(const T* __restrict__ d, const T* __restrict__ inp, T* __restrict__ out, const NfPlan p) {
   extern __shared__ __align__(64) unsigned char nf_smem[];
   T* w = reinterpret_cast<T*>(nf_smem);                          // [WR][WS] window of d
@@ -77,8 +75,8 @@ nf_kernel(const T* __restrict__ d, const T* __restrict__ inp, T* __restrict__ ou
   double* wgx = reinterpret_cast<double*>(uk + N2_KC * N2_KC);     // [KC] x weights of the chunk's rows
   double* wgz = wgx + N2_KC;                                       // [KC] z weights of the chunk's columns
 
-  const Axis& X = p.ax[0];
-  const Axis& Z = p.ax[1];
+  const auto& X = p.ax[0];
+  const auto& Z = p.ax[1];
   const int parts = p.px * p.pz;
   long long idx = blockIdx.x;
   const int part = (int)(idx % parts);
@@ -86,8 +84,8 @@ nf_kernel(const T* __restrict__ d, const T* __restrict__ inp, T* __restrict__ ou
   const int tile = (int)(idx % (p.ktx * p.ktz));
   const long long c = idx / (p.ktx * p.ktz);
   const int a = (int)(c / Z.nf), b = (int)(c % Z.nf);
-  const int k0x = tile / p.ktz * N2_TX, k0z = tile % p.ktz * N2_TZ;
-  const int tid = threadIdx.x, lane = tid % N2_LANES, t0 = tid / N2_LANES * N2_RT;
+  const int k0x = tile / p.ktz * N2_TX, k0z = tile % p.ktz * NS_TZ;
+  const int tid = threadIdx.x, lane = tid % NS_LANES, t0 = tid / NS_LANES * NS_RT;
 
   long long sxlo, sxhi, szlo, szhi;
   support(X, a, sxlo, sxhi);
@@ -95,9 +93,9 @@ nf_kernel(const T* __restrict__ d, const T* __restrict__ inp, T* __restrict__ ou
   const long long jxlo = sxlo + part / p.pz * p.cpx * N2_KC, jxhi = min(sxhi, jxlo + p.cpx * N2_KC);
   const long long jzlo = szlo + part % p.pz * p.cpz * N2_KC, jzhi = min(szhi, jzlo + p.cpz * N2_KC);
 
-  T acc[N2_RT];
+  T acc[NS_RT];
 #pragma unroll
-  for (int r = 0; r < N2_RT; ++r) acc[r] = T(0);
+  for (int r = 0; r < NS_RT; ++r) acc[r] = T(0);
 
   for (long long jx0 = jxlo; jx0 < jxhi; jx0 += N2_KC) {
     const int nqx = (int)min((long long)N2_KC, jxhi - jx0);
@@ -105,8 +103,8 @@ nf_kernel(const T* __restrict__ d, const T* __restrict__ inp, T* __restrict__ ou
     const long long ox = jx0 + k0x - X.hc;                         // sample of window row 0
     if (ox >= X.n || ox + nwr <= 0) continue;                      // every term of the chunk is 0
     for (long long jz0 = jzlo; jz0 < jzhi; jz0 += N2_KC) {
-      const int nqz = (int)min((long long)N2_KC, jzhi - jz0), nqz8 = (nqz + N2_RT - 1) / N2_RT * N2_RT;
-      const int nwc = N2_TZ + nqz - 1;                             // window columns a non-zero u meets
+      const int nqz = (int)min((long long)N2_KC, jzhi - jz0), nqz8 = (nqz + NS_RT - 1) / NS_RT * NS_RT;
+      const int nwc = NS_TZ + nqz - 1;                             // window columns a non-zero u meets
       const long long oz = jz0 + k0z - Z.hc;
       if (oz >= Z.n || oz + nwc <= 0) continue;
       __syncthreads();                                             // the previous chunk's readers are done
@@ -115,7 +113,7 @@ nf_kernel(const T* __restrict__ d, const T* __restrict__ inp, T* __restrict__ ou
         if (tid < N2_KC) wgx[m] = m < nqx ? axis_weight(X, a, jx0 + m) : 0.0;
         else wgz[m] = m < nqz ? axis_weight(Z, b, jz0 + m) : 0.0;
       }
-      for (int e = tid; e < nwr * N2_WC; e += N2_THREADS) {
+      for (int e = tid; e < nwr * N2_WC; e += NS_THREADS) {
         const int r = e / N2_WC, col = e - r * N2_WC;
         const long long jx = ox + r, jz = oz + col;
         T val = T(0);
@@ -123,7 +121,7 @@ nf_kernel(const T* __restrict__ d, const T* __restrict__ inp, T* __restrict__ ou
         w[r * N2_WS + col] = val;
       }
       __syncthreads();                                             // the weights are in
-      for (int e = tid; e < nqx * N2_KC; e += N2_THREADS) {
+      for (int e = tid; e < nqx * N2_KC; e += NS_THREADS) {
         const int qx = e / N2_KC, qz = e - qx * N2_KC;
         T val = T(0);
         if (qz < nqz) val = T(wgz[qz] * wgx[qx]) * __ldg(inp + (size_t)(jx0 + qx) * Z.n + (jz0 + qz));
@@ -137,7 +135,7 @@ nf_kernel(const T* __restrict__ d, const T* __restrict__ inp, T* __restrict__ ou
   if (kx >= X.nh) return;
   T* dst = out + ((size_t)c * parts + part) * X.nh * Z.nh + (size_t)kx * Z.nh;
 #pragma unroll
-  for (int r = 0; r < N2_RT; ++r) {
+  for (int r = 0; r < NS_RT; ++r) {
     const int kz = k0z + t0 + r;
     if (kz < Z.nh) dst[kz] = acc[r];
   }
@@ -161,7 +159,7 @@ int launch_nf(const void* d, const void* inp, void* hs, void* work, const NfPlan
   const int rc = b2_allow_smem<nf_kernel<T>>(smem);
   if (rc != B2_OK) return rc;
   T* dst = static_cast<T*>(p.work_elems ? work : hs);
-  nf_kernel<T><<<(unsigned)p.grid, N2_THREADS, smem, st>>>(static_cast<const T*>(d), static_cast<const T*>(inp), dst,
+  nf_kernel<T><<<(unsigned)p.grid, NS_THREADS, smem, st>>>(static_cast<const T*>(d), static_cast<const T*>(inp), dst,
                                                            p);
   B2_LAUNCH_CHECK();
   if (p.work_elems) {

@@ -202,9 +202,18 @@ class _KernelOperator(LocalOperator):
     _matvec, _rmatvec = matvec, rmatvec
 
 
-class _AxisOperator(_KernelOperator):
-    """A square operator applied line by line along ``axis`` of a C-ordered ``dims`` block, with real taps: complex
-    data are applied in one launch, their (re, im) pairs as the innermost dimension"""
+class _RealTapsOperator(_KernelOperator):
+    """A kernel operator with real taps: complex data are applied in one launch, their (re, im) pairs as the innermost
+    dimension, in the complex dtype of the operator's and the data's real dtypes promoted"""
+
+    def _compute_dtype(self, xdt):
+        if xdt.is_complex and not self._tdtype.is_complex:
+            return _CPLX_OF[torch.promote_types(self._tdtype, _REAL_OF[xdt])]
+        return self._tdtype
+
+
+class _AxisOperator(_RealTapsOperator):
+    """A square operator applied line by line along ``axis`` of a C-ordered ``dims`` block"""
 
     def __init__(self, dims, axis: int, dtype):
         self.dims = tuple(int(d) for d in (dims if np.ndim(dims) else (dims,)))
@@ -221,11 +230,6 @@ class _AxisOperator(_KernelOperator):
         new.dims = tuple(int(d) for d in dims)
         new.axis = int(axis) % len(new.dims)
         return new
-
-    def _compute_dtype(self, xdt):
-        if xdt.is_complex and not self._tdtype.is_complex:
-            return _CPLX_OF[torch.promote_types(self._tdtype, _REAL_OF[xdt])]
-        return self._tdtype
 
     def _lines(self, dt):
         """``(n_outer, n_axis, n_inner, real dtype)`` of a launch on data of dtype ``dt``"""
@@ -415,7 +419,54 @@ def _regular_nodes(name, ih, nfilt, n):
     return int(ih[0]), dh
 
 
-class NonStationaryConvolve2D(_KernelOperator):
+def _bank_nodes(names, ihs, nfilt, dims, nh):
+    """``(oh, dh)``, one entry per axis, of a bank of ``nfilt`` filters of sizes ``nh`` at the indices ``ihs`` of a
+    ``dims`` block: ``ValueError`` for an even size, and :func:`_regular_nodes`' per axis"""
+    if any(int(n) % 2 == 0 for n in nh):
+        raise ValueError("filters hs must have odd length")
+    nodes = [_regular_nodes(*a) for a in zip(names, ihs, nfilt, dims)]
+    return tuple(o for o, _ in nodes), tuple(d for _, d in nodes)
+
+
+class _NonStationaryConvolve(_RealTapsOperator):
+    """The shared part of :class:`NonStationaryConvolve2D` / :class:`NonStationaryConvolve3D` on the axes ``_axes``
+    (``"xz"`` / ``"xyz"``): the argument checks, the bank (uploaded once, in both real precisions), the geometry
+    tuples and one ``_entry`` launch per apply"""
+
+    def __init__(self, dims, hs, ihs, engine, num_threads_per_blocks, dtype):
+        hs = hs.detach().cpu().numpy() if isinstance(hs, torch.Tensor) else np.asarray(hs)
+        if np.iscomplexobj(hs):
+            raise NotImplementedError("complex filters are not supported")
+        ax, nd = self._axes, len(self._axes)
+        dims = tuple(int(d) for d in (dims if np.ndim(dims) else (dims,)))
+        if len(dims) != nd:
+            raise ValueError(f"dims must hold {('two', 'three')[nd - 2]} entries ({', '.join('n' + a for a in ax)}); "
+                             f"got {dims}")
+        if hs.ndim != 2 * nd:
+            shape = ", ".join([f"nf{a}" for a in ax] + [f"nh{a}" for a in ax])
+            raise ValueError(f"hs must be a {2 * nd}-D array of filters ({shape}); got shape {hs.shape}")
+        self.oh, self.dh = _bank_nodes([f"ih{a}" for a in ax], ihs, hs.shape[:nd], dims, hs.shape[nd:])
+        self.dims = self.dimsd = dims
+        n = math.prod(dims)
+        self.shape = (n, n)
+        self._tdtype = _lib.torch_dtype(dtype)
+        self.dtype = _lib.numpy_dtype(self._tdtype)
+        self.engine, self.num_threads_per_blocks = engine, num_threads_per_blocks
+        _lib.ctx()
+        self._bank = _real_filters(hs)[1]
+        self.nfilt = tuple(int(v) for v in hs.shape[:nd])
+        self.nh = tuple(int(v) for v in hs.shape[nd:])
+        self.hc = tuple(v // 2 for v in self.nh)
+        self._geom = (*self.nfilt, *self.nh, *(v for od in zip(self.oh, self.dh) for v in od))
+
+    def _launch(self, x, y, dt, adjoint):
+        real = _REAL_OF.get(dt, dt)
+        _lib.check(getattr(_lib.lib, self._entry)(_lib.ctx(), x.data_ptr(), y.data_ptr(), *self.dims,
+                                                  2 if dt.is_complex else 1, self._bank[real].data_ptr(), *self._geom,
+                                                  adjoint, _lib.code(real), _lib.stream()), self._entry)
+
+
+class NonStationaryConvolve2D(_NonStationaryConvolve):
     """Rank-local non-stationary 2-D convolution of a C-ordered ``dims = (nx, nz)`` image,
     pylops.signalprocessing.NonStationaryConvolve2D (pylops 2.x) inside MPIBlockDiag: image-domain least-squares
     migration, with point-spread functions for filters.  ``hs`` of shape ``(nfx, nfz, nhx, nhz)`` holds real filters
@@ -430,48 +481,14 @@ class NonStationaryConvolve2D(_KernelOperator):
     ``ValueError`` for even filter sizes, irregular or decreasing indices, indices outside ``[0, dims)``,
     ``len(ihx) != nfx``, ``len(ihz) != nfz``, an ``hs`` that is not 4-D and ``dims`` without two entries; complex
     filters are not provided.  ``engine`` and ``num_threads_per_blocks`` are accepted and ignored."""
+    _axes, _entry = "xz", "b2_nsconvolve2d"
 
     def __init__(self, dims, hs, ihx, ihz, engine="numpy", num_threads_per_blocks=(32, 32), dtype="float64"):
-        hs = hs.detach().cpu().numpy() if isinstance(hs, torch.Tensor) else np.asarray(hs)
-        if np.iscomplexobj(hs):
-            raise NotImplementedError("complex filters are not supported")
-        dims = tuple(int(d) for d in (dims if np.ndim(dims) else (dims,)))
-        if len(dims) != 2:
-            raise ValueError(f"dims must hold two entries (nx, nz); got {dims}")
-        if hs.ndim != 4:
-            raise ValueError(f"hs must be a 4-D array of filters (nfx, nfz, nhx, nhz); got shape {hs.shape}")
-        if hs.shape[2] % 2 == 0 or hs.shape[3] % 2 == 0:
-            raise ValueError("filters hs must have odd length")
-        self.ohx, self.dhx = _regular_nodes("ihx", ihx, hs.shape[0], dims[0])
-        self.ohz, self.dhz = _regular_nodes("ihz", ihz, hs.shape[1], dims[1])
-        self.dims = self.dimsd = dims
-        n = dims[0] * dims[1]
-        self.shape = (n, n)
-        self._tdtype = _lib.torch_dtype(dtype)
-        self.dtype = _lib.numpy_dtype(self._tdtype)
-        self.engine, self.num_threads_per_blocks = engine, num_threads_per_blocks
-        _lib.ctx()
-        self._bank = _real_filters(hs)[1]
-        self.nfilt = (int(hs.shape[0]), int(hs.shape[1]))
-        self.nh = (int(hs.shape[2]), int(hs.shape[3]))
-        self.hc = (self.nh[0] // 2, self.nh[1] // 2)
-        self.oh = (self.ohx, self.ohz)
-        self.dh = (self.dhx, self.dhz)
-
-    def _compute_dtype(self, xdt):
-        if xdt.is_complex and not self._tdtype.is_complex:
-            return _CPLX_OF[torch.promote_types(self._tdtype, _REAL_OF[xdt])]
-        return self._tdtype
-
-    def _launch(self, x, y, dt, adjoint):
-        real = _REAL_OF.get(dt, dt)
-        _lib.check(_lib.lib.b2_nsconvolve2d(_lib.ctx(), x.data_ptr(), y.data_ptr(), *self.dims,
-                                            2 if dt.is_complex else 1, self._bank[real].data_ptr(), *self.nfilt,
-                                            *self.nh, self.ohx, self.dhx, self.ohz, self.dhz, adjoint,
-                                            _lib.code(real), _lib.stream()), "b2_nsconvolve2d")
+        super().__init__(dims, hs, (ihx, ihz), engine, num_threads_per_blocks, dtype)
+        (self.ohx, self.ohz), (self.dhx, self.dhz) = self.oh, self.dh
 
 
-class NonStationaryConvolve3D(_KernelOperator):
+class NonStationaryConvolve3D(_NonStationaryConvolve):
     """Rank-local non-stationary 3-D convolution of a C-ordered volume of shape ``dims`` (three entries),
     pylops.signalprocessing.NonStationaryConvolve3D (pylops 2.x as remembered: pylops is not installed here to check
     the signature, defaults or weight clamp) inside MPIBlockDiag: image-domain least-squares migration in 3-D, with
@@ -489,47 +506,11 @@ class NonStationaryConvolve3D(_KernelOperator):
     rounded to float32.  ``ValueError`` for even filter sizes, irregular or decreasing indices, indices outside
     ``[0, dims)``, ``len(ihx) != nfx`` (and for y, z), an ``hs`` that is not 6-D and ``dims`` without three entries;
     complex filters are not provided.  ``engine`` and ``num_threads_per_blocks`` are accepted and ignored."""
+    _axes, _entry = "xyz", "b2_nsconvolve3d"
 
     def __init__(self, dims, hs, ihx, ihy, ihz, engine="numpy", num_threads_per_blocks=(2, 16, 16),
                  dtype="float64"):
-        hs = hs.detach().cpu().numpy() if isinstance(hs, torch.Tensor) else np.asarray(hs)
-        if np.iscomplexobj(hs):
-            raise NotImplementedError("complex filters are not supported")
-        dims = tuple(int(d) for d in (dims if np.ndim(dims) else (dims,)))
-        if len(dims) != 3:
-            raise ValueError(f"dims must hold three entries (nx, ny, nz); got {dims}")
-        if hs.ndim != 6:
-            raise ValueError(f"hs must be a 6-D array of filters (nfx, nfy, nfz, nhx, nhy, nhz); got shape {hs.shape}")
-        if any(n % 2 == 0 for n in hs.shape[3:]):
-            raise ValueError("filters hs must have odd length")
-        nodes = [_regular_nodes(name, ih, nf, n) for name, ih, nf, n in zip(("ihx", "ihy", "ihz"), (ihx, ihy, ihz),
-                                                                               hs.shape[:3], dims)]
-        self.dims = self.dimsd = dims
-        n = dims[0] * dims[1] * dims[2]
-        self.shape = (n, n)
-        self._tdtype = _lib.torch_dtype(dtype)
-        self.dtype = _lib.numpy_dtype(self._tdtype)
-        self.engine, self.num_threads_per_blocks = engine, num_threads_per_blocks
-        _lib.ctx()
-        self._bank = _real_filters(hs)[1]
-        self.nfilt = tuple(int(v) for v in hs.shape[:3])
-        self.nh = tuple(int(v) for v in hs.shape[3:])
-        self.hc = tuple(v // 2 for v in self.nh)
-        self.oh = tuple(o for o, _ in nodes)
-        self.dh = tuple(d for _, d in nodes)
-
-    def _compute_dtype(self, xdt):
-        if xdt.is_complex and not self._tdtype.is_complex:
-            return _CPLX_OF[torch.promote_types(self._tdtype, _REAL_OF[xdt])]
-        return self._tdtype
-
-    def _launch(self, x, y, dt, adjoint):
-        real = _REAL_OF.get(dt, dt)
-        axes = [v for o, d in zip(self.oh, self.dh) for v in (o, d)]
-        _lib.check(_lib.lib.b2_nsconvolve3d(_lib.ctx(), x.data_ptr(), y.data_ptr(), *self.dims,
-                                            2 if dt.is_complex else 1, self._bank[real].data_ptr(), *self.nfilt,
-                                            *self.nh, *axes, adjoint, _lib.code(real), _lib.stream()),
-                   "b2_nsconvolve3d")
+        super().__init__(dims, hs, (ihx, ihy, ihz), engine, num_threads_per_blocks, dtype)
 
 
 class _NonStationaryFilters(_KernelOperator):
@@ -600,10 +581,8 @@ class NonStationaryFilters1D(_NonStationaryFilters):
     def __init__(self, inp, hsize, ih, dtype="float64", name="C"):
         inp = self._host_input(inp, 1)
         self.hsize, self.name = int(hsize), name
-        if self.hsize % 2 == 0:
-            raise ValueError("filters hs must have odd length")
         self.n, self.nfilt = int(inp.shape[0]), len(np.ravel(ih))
-        self.oh, self.dh = _regular_nodes("ih", ih, self.nfilt, self.n)
+        (self.oh,), (self.dh,) = _bank_nodes(("ih",), (ih,), (self.nfilt,), (self.n,), (self.hsize,))
         self.hc = self.hsize // 2
         self._setup(inp, (self.nfilt, self.hsize), (self.n,),
                     (1, self.n, 1, self.nfilt, 1, self.hsize, 0, 1, self.oh, self.dh), dtype)
@@ -640,14 +619,11 @@ class NonStationaryFilters2D(_NonStationaryFilters):
         self.hshape = self.nh = tuple(int(h) for h in hshape)
         if len(self.nh) != 2:
             raise ValueError(f"hshape must hold two entries (nhx, nhz); got {hshape}")
-        if self.nh[0] % 2 == 0 or self.nh[1] % 2 == 0:
-            raise ValueError("filters hs must have odd length")
         nx, nz = (int(v) for v in inp.shape)
         self.nfilt = (len(np.ravel(ihx)), len(np.ravel(ihz)))
-        self.ohx, self.dhx = _regular_nodes("ihx", ihx, self.nfilt[0], nx)
-        self.ohz, self.dhz = _regular_nodes("ihz", ihz, self.nfilt[1], nz)
+        self.oh, self.dh = _bank_nodes(("ihx", "ihz"), (ihx, ihz), self.nfilt, (nx, nz), self.nh)
+        (self.ohx, self.ohz), (self.dhx, self.dhz) = self.oh, self.dh
         self.hc = (self.nh[0] // 2, self.nh[1] // 2)
-        self.oh, self.dh = (self.ohx, self.ohz), (self.dhx, self.dhz)
         self.engine, self.num_threads_per_blocks, self.name = engine, num_threads_per_blocks, name
         self._setup(inp, self.nfilt + self.nh, (nx, nz),
                     (nx, nz, *self.nfilt, *self.nh, self.ohx, self.dhx, self.ohz, self.dhz), dtype)

@@ -18,9 +18,9 @@ import pytest
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "golden"))
 import make_golden_nsconvolve2d as mg2  # noqa: E402
+from ns_reference import axis_weights, c_ns, check_close, ns_matrix, point_weights, run_kernel  # noqa: E402
 
 GOLD = np.load(os.path.join(HERE, "golden", "nsconvolve2d_golden.npz"), allow_pickle=False)
-U = {np.float32: 2.0 ** -24, np.float64: 2.0 ** -53}
 
 
 def refshim():
@@ -31,41 +31,6 @@ def refshim():
     finally:
         sys.path.remove(path)
     return NonStationaryConvolve2D
-
-
-def axis_weights(j, oh, dh, nf):
-    """{filter: float64 weight} of sample j by the definition: weight 1 on the end filter outside the nodes"""
-    v = (j - oh) / dh
-    lo = int(np.floor(v))
-    if lo < 0:
-        return {0: 1.0}
-    if lo >= nf - 1:
-        return {nf - 1: 1.0}
-    w = v - lo
-    return {lo: 1.0 - w, lo + 1: w} if w != 0.0 else {lo: 1.0}
-
-
-def point_weights(jx, jz, ohx, dhx, ohz, dhz, nfx, nfz, dt):
-    """[((a, b), W_ab)] of point j, W = dt(wz * wx)"""
-    wx, wz = axis_weights(jx, ohx, dhx, nfx), axis_weights(jz, ohz, dhz, nfz)
-    return [((a, b), float(dt(wz[b] * wx[a]))) for a in wx for b in wz]
-
-
-def ns2_matrix(hs, dims, ohx, dhx, ohz, dhz, absolute=False):
-    """M[i, j] = h_j[hc + i - j] in float64, h_j = sum W_ab hs[a, b] with W rounded to the dtype of hs (absolute:
-    sum W_ab |hs[a, b]|, the magnitude of the terms)"""
-    nfx, nfz, nhx, nhz = hs.shape
-    nx, nz = dims
-    hcx, hcz = nhx // 2, nhz // 2
-    h64 = np.abs(hs.astype(np.float64)) if absolute else hs.astype(np.float64)
-    M = np.zeros((nx, nz, nx, nz))
-    for jx in range(nx):
-        for jz in range(nz):
-            h = sum(W * h64[a, b] for (a, b), W in point_weights(jx, jz, ohx, dhx, ohz, dhz, nfx, nfz, hs.dtype.type))
-            x0, x1 = max(0, jx - hcx), min(nx, jx + hcx + 1)
-            z0, z1 = max(0, jz - hcz), min(nz, jz + hcz + 1)
-            M[x0:x1, z0:z1, jx, jz] = h[x0 - jx + hcx:x1 - jx + hcx, z0 - jz + hcz:z1 - jz + hcz]
-    return M.reshape(nx * nz, nx * nz)
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -80,7 +45,7 @@ def test_refshim_restatement_is_the_definition(nh, nf, dh, oh):
     ihx, ihz = oh[0] + dh[0] * np.arange(nf[0]), oh[1] + dh[1] * np.arange(nf[1])
     dims = (11, 13)
     Op = NS2(dims, hs, ihx, ihz)
-    M = ns2_matrix(hs, dims, oh[0], dh[0], oh[1], dh[1])
+    M = ns_matrix(hs, dims, oh, dh)
     x = rng.standard_normal(dims[0] * dims[1])
     np.testing.assert_allclose(Op.matvec(x), M @ x, rtol=0, atol=1e-12)
     np.testing.assert_allclose(Op.rmatvec(x), M.T @ x, rtol=0, atol=1e-12)
@@ -107,7 +72,7 @@ def test_interpolation_weights_and_clamps(nf, dh, oh):
     Op = NS2((40, 12), hs, oh + dh * np.arange(nf), [1, 5, 9])
     for jx in range(0, 40, 3):
         for jz in range(12):
-            want = sum(W * hs[a, b] for (a, b), W in point_weights(jx, jz, oh, dh, 1, 4, nf, 3, np.float64))
+            want = sum(W * hs[a, b] for (a, b), W in point_weights((jx, jz), (oh, 1), (dh, 4), (nf, 3), np.float64))
             np.testing.assert_allclose(Op.interpolate_h(jx, jz), want, rtol=0, atol=1e-15)
 
 
@@ -195,55 +160,6 @@ def host(t):
     return t.cpu().numpy()
 
 
-def c_ns2(pm, x, y, nx, nz, ni, hs, nf, nh, oh, dh, adjoint, code):
-    L = pm._lib
-    return L.lib.b2_nsconvolve2d(L.ctx(), x, y, nx, nz, ni, hs, *nf, *nh, oh[0], dh[0], oh[1], dh[1], adjoint, code,
-                                 L.stream())
-
-
-def run_kernel(pm, x_np, hs_np, oh, dh, adjoint, dt, guard=5):
-    """apply to x_np (nx, nz[, 2]) through the C ABI into a guarded interior view; returns (y, guards intact,
-    second apply bit-equal)"""
-    import torch
-    tdt = {np.float32: torch.float32, np.float64: torch.float64}[dt]
-    N = x_np.size
-    x = torch.as_tensor(np.ascontiguousarray(x_np.ravel(), dtype=dt)).cuda()
-    yb = torch.full((N + 2 * guard,), 7.25, dtype=tdt, device="cuda")
-    y = yb[guard:guard + N]
-    hs = torch.as_tensor(np.ascontiguousarray(hs_np, dtype=dt)).cuda()
-    ni = x_np.shape[2] if x_np.ndim == 3 else 1
-    code = pm._lib.F32 if dt == np.float32 else pm._lib.F64
-    args = (x_np.shape[0], x_np.shape[1], ni, hs.data_ptr(), hs_np.shape[:2], hs_np.shape[2:], oh, dh, int(adjoint),
-            code)
-    assert c_ns2(pm, x.data_ptr(), y.data_ptr(), *args) == 0
-    first = y.clone()
-    assert c_ns2(pm, x.data_ptr(), y.data_ptr(), *args) == 0
-    torch.cuda.synchronize()
-    g = host(yb)
-    guards_ok = bool(np.all(g[:guard] == 7.25) and np.all(g[guard + N:] == 7.25))
-    return host(first).reshape(x_np.shape), guards_ok, bool(torch.equal(first, y))
-
-
-def check_close(got, x, hs, oh, dh, adjoint, dt):
-    """componentwise |got - ref| <= gamma_n (sum |terms|) against the float64 product of the definition, n the
-    number of rounded operations in one output's longest chain (4 nhx nhz fma, a weight and a product per term)"""
-    dims = x.shape[:2]
-    key = (hs.astype(dt).tobytes(), hs.shape, dims, oh, dh)
-    if key not in _MATRICES:
-        _MATRICES.clear()
-        _MATRICES[key] = tuple(ns2_matrix(hs.astype(dt), dims, oh[0], dh[0], oh[1], dh[1], absolute=a)
-                               for a in (False, True))
-    M, B = _MATRICES[key]
-    M, B = (M.T, B.T) if adjoint else (M, B)
-    xs = x.reshape(dims[0] * dims[1], -1).astype(np.float64)
-    ref, bnd = M @ xs, B @ np.abs(xs)
-    n = 4 * hs.shape[2] * hs.shape[3] + 8
-    tol = n * U[dt] / (1 - n * U[dt]) * bnd
-    err = np.abs(got.reshape(ref.shape).astype(np.float64) - ref)
-    assert np.all(err <= tol), f"max err {err.max():.3e}, excess {(err - tol).max():.3e}"
-
-
-_MATRICES = {}
 SHAPES = [(1, 1), (1, 37), (29, 1), (5, 7), (33, 65), (70, 130)]
 
 
@@ -305,8 +221,8 @@ def test_kernel_error_codes_leave_y_untouched(pm):
         a.update(kw)
         if a["y"] == "x":
             a["y"] = a["x"]
-        rc = c_ns2(pm, a["x"], a["y"], a["nx"], a["nz"], a["ni"], a["hs"], a["nf"], a["nh"], (0, 0), a["dh"], 0,
-                   a["dtype"])
+        rc = c_ns(pm, a["x"], a["y"], (a["nx"], a["nz"]), a["ni"], a["hs"], a["nf"], a["nh"], (0, 0), a["dh"], 0,
+                  a["dtype"])
         assert rc == want, (kw, rc)
     torch.cuda.synchronize()
     assert torch.all(y == 3.5)
@@ -390,7 +306,7 @@ def test_operator_attributes_dtypes_and_out(pm):
                 with pytest.raises(ValueError, match="dimension mismatch"):
                     f(x[:-1])
     # float32 data of a float64-bank float32 operator: the bank rounded to float32
-    M = ns2_matrix(hs.astype(np.float32), (20, 9), 2, 4, 1, 3)
+    M = ns_matrix(hs.astype(np.float32), (20, 9), (2, 1), (4, 3))
     x = rng.standard_normal(180).astype(np.float32)
     y = host(Op.matvec(torch.as_tensor(x).cuda()))
     np.testing.assert_allclose(y, M @ x, rtol=0, atol=1e-4 * np.abs(M).sum(1).max())

@@ -18,48 +18,13 @@ import pytest
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "golden"))
 import make_golden_nsconvolve3d as mg3  # noqa: E402
+from ns_reference import axis_weights, c_ns, check_close, ns_matrix, point_weights, reference, run_kernel  # noqa: E402
 
 GOLD = np.load(os.path.join(HERE, "golden", "nsconvolve3d_golden.npz"), allow_pickle=False)
-U = {np.float32: 2.0 ** -24, np.float64: 2.0 ** -53}
 
 
 def refshim():
     return mg3.refshim_modules()[2]
-
-
-def axis_weights(j, oh, dh, nf):
-    """{filter: float64 weight} of sample j by the definition: weight 1 on the end filter outside the nodes"""
-    v = (j - oh) / dh
-    lo = int(np.floor(v))
-    if lo < 0:
-        return {0: 1.0}
-    if lo >= nf - 1:
-        return {nf - 1: 1.0}
-    w = v - lo
-    return {lo: 1.0 - w, lo + 1: w} if w != 0.0 else {lo: 1.0}
-
-
-def point_weights(j, oh, dh, nf, dt):
-    """[((a, b, e), W_abe)] of point j = (jx, jy, jz), W = dt(wz * wy * wx)"""
-    wx, wy, wz = (axis_weights(j[d], oh[d], dh[d], nf[d]) for d in range(3))
-    return [((a, b, e), float(dt(wz[e] * wy[b] * wx[a]))) for a in wx for b in wy for e in wz]
-
-
-def ns3_matrix(hs, dims, oh, dh, absolute=False):
-    """M[i, j] = h_j[hc + i - j] in float64, h_j = sum W_abe hs[a, b, e] with W rounded to the dtype of hs (absolute:
-    sum W_abe |hs[a, b, e]|, the magnitude of the terms)"""
-    nf, nh = hs.shape[:3], hs.shape[3:]
-    hc = tuple(n // 2 for n in nh)
-    h64 = np.abs(hs.astype(np.float64)) if absolute else hs.astype(np.float64)
-    M = np.zeros(tuple(dims) * 2)
-    for j in np.ndindex(*dims):
-        h = sum(W * h64[c] for c, W in point_weights(j, oh, dh, nf, hs.dtype.type))
-        lo = [max(0, j[d] - hc[d]) for d in range(3)]
-        hi = [min(dims[d], j[d] + hc[d] + 1) for d in range(3)]
-        M[lo[0]:hi[0], lo[1]:hi[1], lo[2]:hi[2]][(...,) + j] = \
-            h[tuple(slice(lo[d] - j[d] + hc[d], hi[d] - j[d] + hc[d]) for d in range(3))]
-    n = int(np.prod(dims))
-    return M.reshape(n, n)
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -75,7 +40,7 @@ def test_refshim_restatement_is_the_definition(nh, nf, dh, oh):
     ih = [o + d * np.arange(f) for o, d, f in zip(oh, dh, nf)]
     dims = (6, 11, 7)
     Op = NS3(dims, hs, *ih)
-    M = ns3_matrix(hs, dims, oh, dh)
+    M = ns_matrix(hs, dims, oh, dh)
     x = rng.standard_normal(int(np.prod(dims)))
     np.testing.assert_allclose(Op.matvec(x), M @ x, rtol=0, atol=1e-12)
     np.testing.assert_allclose(Op.rmatvec(x), M.T @ x, rtol=0, atol=1e-12)
@@ -198,59 +163,6 @@ def host(t):
     return t.cpu().numpy()
 
 
-def c_ns3(pm, x, y, dims, ni, hs, nf, nh, oh, dh, adjoint, code):
-    L = pm._lib
-    return L.lib.b2_nsconvolve3d(L.ctx(), x, y, *dims, ni, hs, *nf, *nh, oh[0], dh[0], oh[1], dh[1], oh[2], dh[2],
-                                 adjoint, code, L.stream())
-
-
-def run_kernel(pm, x_np, hs_np, oh, dh, adjoint, dt, guard=5):
-    """apply to x_np (nx, ny, nz[, 2]) through the C ABI into a guarded interior view; returns (y, guards intact,
-    second apply bit-equal)"""
-    import torch
-    tdt = {np.float32: torch.float32, np.float64: torch.float64}[dt]
-    N = x_np.size
-    x = torch.as_tensor(np.ascontiguousarray(x_np.ravel(), dtype=dt)).cuda()
-    yb = torch.full((N + 2 * guard,), 7.25, dtype=tdt, device="cuda")
-    y = yb[guard:guard + N]
-    hs = torch.as_tensor(np.ascontiguousarray(hs_np, dtype=dt)).cuda()
-    ni = x_np.shape[3] if x_np.ndim == 4 else 1
-    code = pm._lib.F32 if dt == np.float32 else pm._lib.F64
-    args = (x_np.shape[:3], ni, hs.data_ptr(), hs_np.shape[:3], hs_np.shape[3:], oh, dh, int(adjoint), code)
-    assert c_ns3(pm, x.data_ptr(), y.data_ptr(), *args) == 0
-    first = y.clone()
-    assert c_ns3(pm, x.data_ptr(), y.data_ptr(), *args) == 0
-    torch.cuda.synchronize()
-    g = host(yb)
-    guards_ok = bool(np.all(g[:guard] == 7.25) and np.all(g[guard + N:] == 7.25))
-    return host(first).reshape(x_np.shape), guards_ok, bool(torch.equal(first, y))
-
-
-_MATRICES = {}
-
-
-def reference(x, hs, oh, dh, adjoint, dt):
-    """(float64 product of the definition, gamma_n sum |terms|) for x (dims[, ni]), n the number of rounded
-    operations in one output's longest chain (8 nhx nhy nhz fma, a weight and a product per term)"""
-    dims = x.shape[:3]
-    key = (hs.astype(dt).tobytes(), hs.shape, dims, oh, dh)
-    if key not in _MATRICES:
-        _MATRICES.clear()
-        _MATRICES[key] = tuple(ns3_matrix(hs.astype(dt), dims, oh, dh, absolute=a) for a in (False, True))
-    M, B = _MATRICES[key]
-    M, B = (M.T, B.T) if adjoint else (M, B)
-    xs = x.reshape(int(np.prod(dims)), -1).astype(np.float64)
-    n = 8 * int(np.prod(hs.shape[3:])) + 12
-    return M @ xs, n * U[dt] / (1 - n * U[dt]) * (B @ np.abs(xs))
-
-
-def check_close(got, x, hs, oh, dh, adjoint, dt):
-    """componentwise |got - ref| <= gamma_n (sum |terms|) against the float64 product of the definition"""
-    ref, tol = reference(x, hs, oh, dh, adjoint, dt)
-    err = np.abs(got.reshape(ref.shape).astype(np.float64) - ref)
-    assert np.all(err <= tol), f"max err {err.max():.3e}, excess {(err - tol).max():.3e}"
-
-
 # singleton axes, tiles that are not full along every axis (x tiles of 4 / 2 / 1 planes, y of 32, z of 64)
 SHAPES = [(1, 1, 1), (1, 1, 37), (1, 29, 1), (7, 1, 1), (3, 5, 7), (5, 33, 3), (2, 7, 70), (6, 35, 5)]
 
@@ -348,8 +260,8 @@ def test_kernel_error_codes_leave_y_untouched(pm):
         a.update(kw)
         if a["y"] == "x":
             a["y"] = a["x"]
-        rc = c_ns3(pm, a["x"], a["y"], a["dims"], a["ni"], a["hs"], a["nf"], a["nh"], (0, 0, 0), a["dh"], 0,
-                   a["dtype"])
+        rc = c_ns(pm, a["x"], a["y"], a["dims"], a["ni"], a["hs"], a["nf"], a["nh"], (0, 0, 0), a["dh"], 0,
+                  a["dtype"])
         assert rc == want, (kw, rc)
     torch.cuda.synchronize()
     assert torch.all(y == 3.5)
@@ -439,7 +351,7 @@ def test_operator_attributes_dtypes_and_out(pm):
                 with pytest.raises(ValueError, match="dimension mismatch"):
                     f(x[:-1])
     # float32 data of a float64-bank float32 operator: the bank rounded to float32
-    M = ns3_matrix(hs.astype(np.float32), dims, (2, 1, 0), (4, 3, 5))
+    M = ns_matrix(hs.astype(np.float32), dims, (2, 1, 0), (4, 3, 5))
     x = rng.standard_normal(N).astype(np.float32)
     y = host(Op.matvec(torch.as_tensor(x).cuda()))
     np.testing.assert_allclose(y, M @ x, rtol=0, atol=1e-4 * np.abs(M).sum(1).max())

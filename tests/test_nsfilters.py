@@ -18,9 +18,9 @@ import pytest
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "golden"))
 import make_golden_nsfilters as mgf  # noqa: E402
+from ns_reference import U, assert_within, axis_w, gamma, guarded_twice  # noqa: E402
 
 GOLD = np.load(os.path.join(HERE, "golden", "nsfilters_golden.npz"), allow_pickle=False)
-U = {np.float32: 2.0 ** -24, np.float64: 2.0 ** -53}
 
 
 def refshim():
@@ -46,21 +46,6 @@ def dense(kind, inp, bshape, ih):
         else:
             M[:, c] = c2.NonStationaryConvolve2D(inp.shape, e.reshape(bshape), *ih).matvec(inp.astype(np.float64))
     return M
-
-
-def axis_w(n, oh, dh, nf):
-    """(nf, n) float64 weights of every sample on every filter, by the definition (1 on the end filter outside)"""
-    W = np.zeros((nf, n))
-    for j in range(n):
-        v = (j - oh) / dh
-        lo = int(np.floor(v))
-        if lo < 0:
-            W[0, j] = 1.0
-        elif lo >= nf - 1:
-            W[nf - 1, j] = 1.0
-        else:
-            W[lo, j], W[lo + 1, j] = 1.0 - (v - lo), v - lo
-    return W
 
 
 def adjoint_ref(d, inp, nf, nh, oh, dh, dt):
@@ -232,26 +217,17 @@ def work_bytes(pm, g, code):
 def run_adjoint(pm, d_np, inp_np, nf, nh, oh, dh, dt, guard=5):
     """g through the C ABI into a guarded view; returns (g, guards intact, second apply bit-equal, work bytes)"""
     import torch
-    tdt = {np.float32: torch.float32, np.float64: torch.float64}[dt]
     code = pm._lib.F32 if dt == np.float32 else pm._lib.F64
     d = torch.as_tensor(np.ascontiguousarray(d_np, dtype=dt)).cuda()
     inp = torch.as_tensor(np.ascontiguousarray(inp_np, dtype=dt)).cuda()
-    nb = int(np.prod(nf + nh))
-    gb = torch.full((nb + 2 * guard,), 7.25, dtype=tdt, device="cuda")
-    g = gb[guard:guard + nb]
     gm = geom(d_np.shape, nf, nh, oh, dh)
     nw = work_bytes(pm, gm, code)
     work = torch.empty(max(nw, 1), dtype=torch.uint8, device="cuda")
     L = pm._lib
-    call = lambda: L.lib.b2_nsfilters2d_adjoint(L.ctx(), d.data_ptr(), inp.data_ptr(), g.data_ptr(), *gm,  # noqa
-                                                work.data_ptr(), nw, code, L.stream())
-    assert call() == 0
-    first = g.clone()
-    assert call() == 0
-    torch.cuda.synchronize()
-    b = host(gb)
-    guards_ok = bool(np.all(b[:guard] == 7.25) and np.all(b[guard + nb:] == 7.25))
-    return host(first).reshape(nf + nh), guards_ok, bool(torch.equal(first, g)), nw
+    g, guards_ok, same = guarded_twice(
+        lambda gp: L.lib.b2_nsfilters2d_adjoint(L.ctx(), d.data_ptr(), inp.data_ptr(), gp, *gm, work.data_ptr(), nw,
+                                                code, L.stream()), int(np.prod(nf + nh)), dt, guard)
+    return g.reshape(nf + nh), guards_ok, same, nw
 
 
 def check_adjoint(pm, shape, nf, nh, oh, dh, dt, seed=0, want_split=None):
@@ -266,10 +242,7 @@ def check_adjoint(pm, shape, nf, nh, oh, dh, dt, seed=0, want_split=None):
     # operations than there are points), plus the rounded weight and the rounded product W_c inp of each term
     Wx, Wz = axis_w(shape[0], oh[0], dh[0], nf[0]), axis_w(shape[1], oh[1], dh[1], nf[1])
     K = np.count_nonzero(Wx, 1)[:, None] * np.count_nonzero(Wz, 1)[None, :] + 3
-    gamma = K * U[dt] / (1 - K * U[dt])
-    tol = gamma[:, :, None, None] * bnd
-    err = np.abs(g.astype(np.float64) - ref)
-    assert np.all(err <= tol), f"max err {err.max():.3e}, excess {(err - tol).max():.3e}"
+    assert_within(g, ref, gamma(K, dt)[:, :, None, None] * bnd)
 
 
 @pytest.mark.gpu
