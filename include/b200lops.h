@@ -36,6 +36,8 @@ enum { B2_FD_FORWARD = 0, B2_FD_BACKWARD = 1, B2_FD_CENTERED = 2 };
 /* op(A) for gemv/gemm */
 enum { B2_OP_N = 0, B2_OP_T = 1, B2_OP_H = 2 };
 enum { B2_THRESH_NONE = 0, B2_THRESH_SOFT = 1, B2_THRESH_HARD = 2, B2_THRESH_HALF = 3 };
+/* curve kinds of b2_radon (pylops.signalprocessing.Radon2D / Radon3D kind=) */
+enum { B2_RADON_LINEAR = 0, B2_RADON_PARABOLIC = 1, B2_RADON_HYPERBOLIC = 2 };
 
 /* error codes >= 2000 are library-level */
 enum { B2_OK = 0, B2_ERR_DTYPE = 2001, B2_ERR_ARG = 2002, B2_ERR_HALO = 2003,
@@ -288,6 +290,23 @@ int b2_kirchhoff(b2_ctx* ctx, const void* x, void* y, const double* trav_srcs, c
 int b2_kirchhoff_chunk(b2_ctx* ctx, const void* x, void* y, const double* trav_srcs, const double* trav_recs,
                        size_t ni, size_t i0, size_t nc, size_t ns, size_t nr, size_t nt, double dt, int adjoint,
                        int accumulate, int dtype, void* stream);
+/* rank-local Radon transform: pylops.signalprocessing.Radon2D / Radon3D (Spread's per-sample tables).  Model x
+ * [npy][npx][nt][n_inner], data [nhy][nhx][nt][n_inner] (n_inner 1, or 2 for complex data as (re, im) pairs of the
+ * real dtype); forward x -> y is model -> data, adjoint the reverse.  hy, hx, py, px are float64 device arrays of the
+ * unitless offsets (samples of dh) and slownesses (linear, parabolic) or velocities (hyperbolic); hy = py = NULL is
+ * 2-D (nhy = npy = 1, no y term is formed).  For model sample (p, t0) and trace h, in float64 rounded to nearest
+ * operation by operation: linear tdec = (t0 + px*hx) + py*hy, parabolic (t0 + px*(hx*hx)) + py*(hy*hy), hyperbolic
+ * sqrt((t0*t0 + (hx/px)*(hx/px)) + (hy/py)*(hy/py)).  interp != 0: used iff 0 <= tdec < nt - 1, it = trunc(tdec),
+ * d = tdec - it, forward y[h][it] += (1-d) x[p][t0], y[h][it+1] += d x[p][t0]; interp = 0: used iff
+ * 0 <= tdec < nt, y[h][trunc(tdec)] += x[p][t0]; the adjoint is the exact transpose.  Sums are float64, rounded once
+ * to the dtype: forward over (py, px, t0) ascending, adjoint over (hy, hx) ascending.  One launch, no atomics, no
+ * allocation: repeated applies give identical bits.  dtype F32 / F64.  B2_ERR_ARG: a null pointer (hy / py excepted,
+ * which are NULL together), x == y, a zero size, nhy or npy other than 1 in 2-D, an axis of 2^31 samples or more,
+ * n_inner not 1 or 2, an unknown kind, more CTAs than one grid holds; B2_ERR_DTYPE: another dtype; y is untouched on
+ * every error */
+int b2_radon(b2_ctx* ctx, const void* x, void* y, size_t nt, size_t n_inner, size_t nhy, size_t nhx, size_t npy,
+             size_t npx, const double* hy, const double* hx, const double* py, const double* px, int kind, int interp,
+             int adjoint, int dtype, void* stream);
 /* analytic (constant-velocity) traveltime table of pylops.waveeqprocessing.Kirchhoff, in b2_kirchhoff_chunk's
  * layout: table[p][j] = |grid point i0 + j - point p| / vel for p < n, j < nc (row stride nc).  Axes are float64
  * device arrays; y = NULL for 2-D (ny ignored), where the grid is meshgrid(x, z, indexing="ij") raveled,

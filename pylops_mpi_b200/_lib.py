@@ -22,6 +22,7 @@ NRM_COUNT_NONZERO, NRM_SUM_ABS, NRM_SUM_SQ, NRM_MAX_ABS, NRM_MIN_ABS, NRM_SUM_PO
 FD_FORWARD, FD_BACKWARD, FD_CENTERED = 0, 1, 2
 OP_N, OP_T, OP_H = 0, 1, 2
 THRESH_NONE, THRESH_SOFT, THRESH_HARD, THRESH_HALF = 0, 1, 2, 3
+RADON_LINEAR, RADON_PARABOLIC, RADON_HYPERBOLIC = 0, 1, 2
 
 _TORCH2CODE = {torch.float32: F32, torch.float64: F64, torch.complex64: C64,
                torch.complex128: C128, torch.bfloat16: BF16, torch.int64: I64}
@@ -99,6 +100,7 @@ def _load():
         "b2_nsfilters2d_work_bytes": ([sz, sz, i, i, i, i, ll, ll, ll, ll, i, C.POINTER(sz)], i),
         "b2_kirchhoff": ([vp, vp, vp, vp, vp, sz, sz, sz, sz, d, i, i, vp], i),
         "b2_kirchhoff_chunk": ([vp, vp, vp, vp, vp, sz, sz, sz, sz, sz, sz, d, i, i, i, vp], i),
+        "b2_radon": ([vp, vp, vp, sz, sz, sz, sz, sz, sz, vp, vp, vp, vp, i, i, i, i, vp], i),
         "b2_kirchhoff_tables": ([vp, vp, vp, vp, sz, sz, sz, vp, sz, d, sz, sz, vp, vp], i),
         "b2_eikonal_tables": ([vp, vp, sz, sz, sz, d, d, d, vp, sz, sz, vp, vp, vp, vp], i),
         "b2_eikonal_work_bytes": ([sz, sz, sz, sz], sz),

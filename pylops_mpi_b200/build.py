@@ -18,7 +18,7 @@ OUT = os.path.join(HERE, "libb200lops.so")
 INCLUDE = os.path.join(os.path.dirname(HERE), "include")
 
 SOURCES = ["ctx.cu", "elementwise.cu", "reduce.cu", "sparsity.cu", "stencil.cu", "convolve.cu", "nsconvolve.cu", "nsconvolve2d.cu",
-           "nsconvolve3d.cu", "nsfilters.cu", "kirchhoff.cu", "eikonal.cu", "lsqr.cu", "gemv.cu",
+           "nsconvolve3d.cu", "nsfilters.cu", "radon.cu", "kirchhoff.cu", "eikonal.cu", "lsqr.cu", "gemv.cu",
            "gemm_simt.cu", "gemm_tc.cu", "fredholm_tc.cu", "host_pipe.cu", "comm.cu", "peer.cu"]
 
 

@@ -1018,6 +1018,105 @@ class LSM:
         return x.local_array.reshape(self.Demop.dims)
 
 
+_RADON_KINDS = {"linear": _lib.RADON_LINEAR, "parabolic": _lib.RADON_PARABOLIC, "hyperbolic": _lib.RADON_HYPERBOLIC}
+
+
+def _radon_sampling(name, axis):
+    """``|axis[1] - axis[0]|`` of a float64 axis, or ValueError for one too short to have a sampling"""
+    if axis.size < 2:
+        raise ValueError(f"{name} needs at least 2 samples to define its sampling; got {axis.size}")
+    return abs(axis[1] - axis[0])
+
+
+class _Radon(_RealTapsOperator):
+    """The shared part of :class:`Radon2D` / :class:`Radon3D`: the unitless axes (computed here in float64 and
+    uploaded once) and one b2_radon launch per apply.  ``haxes`` / ``paxes`` hold one axis (2-D) or the (y, x) pair
+    (3-D).  The unit conventions (pylops 2.x as remembered: pylops is not installed here to check them) all live in
+    this constructor:
+
+    - ``dt = |taxis[1] - taxis[0]|``, ``dh = |haxis[1] - haxis[0]|`` per spatial axis;
+    - offsets: ``centeredh`` gives ``arange(nh) - nh // 2 + ((nh + 1) % 2) / 2``, else ``haxis / dh``;
+    - slownesses: linear ``paxis * (dh / dt)``, parabolic ``paxis * (dh * dh / dt)``, hyperbolic (a velocity)
+      ``paxis * (dt / dh)``."""
+
+    def __init__(self, taxis, haxes, paxes, kind, centeredh, interp, onthefly, engine, dtype, name):
+        if engine not in ("numpy", "numba", "cuda"):
+            raise KeyError("engine must be numpy or numba or cuda")
+        if kind not in _RADON_KINDS:
+            raise NotImplementedError(f"kind={kind!r} is not supported (linear, parabolic or hyperbolic)")
+        self._tdtype = _lib.torch_dtype(dtype)
+        if self._tdtype not in (torch.float32, torch.float64):
+            raise NotImplementedError(f"dtype={dtype!r} is not supported (float32 or float64; complex data are "
+                                      f"applied by a real operator)")
+        self.dtype = _lib.numpy_dtype(self._tdtype)
+        self.kind, self.centeredh, self.interp = kind, bool(centeredh), bool(interp)
+        self.onthefly, self.engine, self.name = onthefly, engine, name
+        taxis = np.asarray(taxis, dtype=np.float64).ravel()
+        dt = _radon_sampling("taxis", taxis)
+        hs, ps = [], []
+        for hname, haxis, paxis in zip(("haxis",) if len(haxes) == 1 else ("hyaxis", "hxaxis"), haxes, paxes):
+            haxis = np.asarray(haxis, dtype=np.float64).ravel()
+            paxis = np.asarray(paxis, dtype=np.float64).ravel()
+            dh = _radon_sampling(hname, haxis)
+            nh = haxis.size
+            hs.append(np.arange(nh) - nh // 2 + ((nh + 1) % 2) / 2 if self.centeredh else haxis / dh)
+            ps.append(paxis * {"linear": dh / dt, "parabolic": dh * dh / dt, "hyperbolic": dt / dh}[kind])
+        self._nt = taxis.size
+        nh, npp = tuple(h.size for h in hs), tuple(p.size for p in ps)
+        self.dims, self.dimsd = npp + (self._nt,), nh + (self._nt,)
+        self.shape = (math.prod(self.dimsd), math.prod(self.dims))
+        _lib.ctx()
+        self._axes = [torch.as_tensor(np.ascontiguousarray(a, dtype=np.float64)).to("cuda") for a in hs + ps]
+        if len(hs) == 1:
+            hy, hx, py, px = None, self._axes[0], None, self._axes[1]
+        else:
+            hy, hx, py, px = self._axes
+        nhy, nhx = (1,) + nh if len(nh) == 1 else nh
+        npy, npx = (1,) + npp if len(npp) == 1 else npp
+        self._geom = (nhy, nhx, npy, npx, _lib.ptr(hy), hx.data_ptr(), _lib.ptr(py), px.data_ptr(),
+                      _RADON_KINDS[kind], int(self.interp))
+
+    def _launch(self, x, y, dt, adjoint):
+        real = _REAL_OF.get(dt, dt)
+        _lib.check(_lib.lib.b2_radon(_lib.ctx(), x.data_ptr(), y.data_ptr(), self._nt, 2 if dt.is_complex else 1,
+                                     *self._geom, adjoint, _lib.code(real), _lib.stream()), "b2_radon")
+
+
+class Radon2D(_Radon):
+    """Rank-local 2-D Radon transform of one gather, pylops.signalprocessing.Radon2D (pylops 2.x as remembered) inside
+    MPIBlockDiag: each CMP gather is one block.  The model is ``dims = (npx, nt)``, the data ``dimsd = (nh, nt)``.
+    On the unitless axes of :class:`_Radon`, model sample ``(p, t0)`` (``t0`` an integer sample index) reaches trace
+    ``h`` at ``tdec`` = ``t0 + p*h`` (linear), ``t0 + p*(h*h)`` (parabolic) or ``sqrt(t0*t0 + (h/p)*(h/p))``
+    (hyperbolic), in float64.  With ``interp`` the pair is used iff ``0 <= tdec < nt - 1`` and spreads onto samples
+    ``it = trunc(tdec)`` and ``it + 1`` with weights ``1 - d`` and ``d`` (``d = tdec - it``); without, iff
+    ``0 <= tdec < nt`` onto sample ``it``.  The adjoint is the exact transpose.
+
+    One b2_radon launch per apply (csrc/radon.cu), complex data included (applied in the complex dtype of the
+    operator's and the data's real dtypes promoted).  Index and weights are float64 and every sum is float64,
+    rounded once to the data's dtype.  ``dtype`` is float32 or float64: a complex dtype, or a ``kind`` other than
+    linear / parabolic / hyperbolic, raises ``NotImplementedError``; an axis with fewer than 2 samples (taxis, haxis)
+    ``ValueError``; an ``engine`` other than numpy / numba / cuda ``KeyError``.  ``onthefly`` and ``engine`` do not
+    change the values and are otherwise ignored."""
+
+    def __init__(self, taxis, haxis, pxaxis, kind="linear", centeredh=True, interp=True, onthefly=False,
+                 engine="numpy", dtype="float64", name="R"):
+        super().__init__(taxis, (haxis,), (pxaxis,), kind, centeredh, interp, onthefly, engine, dtype, name)
+
+
+class Radon3D(_Radon):
+    """Rank-local 3-D Radon transform of one gather, pylops.signalprocessing.Radon3D (pylops 2.x as remembered) inside
+    MPIBlockDiag.  The model is ``dims = (npy, npx, nt)``, the data ``dimsd = (nhy, nhx, nt)``.  As :class:`Radon2D`
+    with the y term added last: ``tdec`` = ``(t0 + px*hx) + py*hy`` (linear), ``(t0 + px*(hx*hx)) + py*(hy*hy)``
+    (parabolic) or ``sqrt((t0*t0 + (hx/px)*(hx/px)) + (hy/py)*(hy/py))`` (hyperbolic), each spatial axis made
+    unitless with its own sampling.  Same launch, dtypes and errors as :class:`Radon2D` (hyaxis and hxaxis need 2
+    samples each)."""
+
+    def __init__(self, taxis, hyaxis, hxaxis, pyaxis, pxaxis, kind="linear", centeredh=True, interp=True,
+                 onthefly=False, engine="numpy", dtype="float64", name="R"):
+        super().__init__(taxis, (hyaxis, hxaxis), (pyaxis, pxaxis), kind, centeredh, interp, onthefly, engine, dtype,
+                         name)
+
+
 class FFT(LocalOperator):
     """Rank-local real FFT along ``axis`` of a ``dims`` block -- the role of third-party
     ``pylops.signalprocessing.FFT(dims, axis, real=True, ifftshift_before=..., norm="ortho")`` inside
