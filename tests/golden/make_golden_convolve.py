@@ -25,6 +25,7 @@ import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
+from fixture_codec import encode, rows_of  # noqa: E402
 
 DIMS = (7, 9, 33)
 AXES = (-1, 0, 1)
@@ -69,11 +70,6 @@ def along_rows(axis):
     return axis % len(DIMS) == 0
 
 
-def rows_of(P, dims=DIMS):
-    """rows of axis 0 per rank (the reference's SCATTER split)"""
-    return [dims[0] // P + (1 if r < dims[0] % P else 0) for r in range(P)]
-
-
 def case_inputs(nh, dt):
     """taps h (float64) and the global x (forward input) and v (adjoint input) of one case, in dtype dt"""
     h = np.random.default_rng(100 + nh).choice([-1.0, -0.5, 0.5, 1.0], nh)
@@ -83,21 +79,6 @@ def case_inputs(nh, dt):
     if dt == "complex128":
         x, v = x + 1j * xi, v + 1j * vi
     return h, x.astype(dt), v.astype(dt)
-
-
-def expected(gold, P, axis, nh, off, dt):
-    """the reference's gathered (forward, adjoint) outputs of one case, decoded from the fixture, in dtype dt"""
-    k = key(P, axis, nh, off)
-    f = [gold[f"{k}/{n}"].astype(np.float64) / ENC for n in ("y", "ya", "yi", "yai")[:4 if dt == "complex128" else 2]]
-    if dt == "complex128":
-        return f[0] + 1j * f[2], f[1] + 1j * f[3]
-    return f[0].astype(dt), f[1].astype(dt)
-
-
-def encode(y):
-    e = np.rint(np.asarray(y, dtype=np.float64) * ENC)
-    assert np.array_equal(e / ENC, y) and np.abs(e).max() <= 127
-    return e.astype(np.int8)
 
 
 def refl_inputs():
@@ -128,7 +109,7 @@ def main():
 
     def t_conv(rank, P, axis, nh, off, dt):
         h, x, v = case_inputs(nh, dt)
-        ny = rows_of(P)
+        ny = rows_of(P, DIMS[0])
         ls = [(r * DIMS[1] * DIMS[2],) for r in ny]
         Op = BD([Convolve1D((ny[rank],) + DIMS[1:], h, offset=off, axis=axis, dtype=dt)])
         fwd = Op @ DA.to_dist(x, local_shapes=ls)
@@ -150,11 +131,11 @@ def main():
                     k = key(P, axis, nh, off)
                     enc = {}
                     for n in ("y", "ya"):
-                        enc[n] = encode(runs["float64"][n])
+                        enc[n] = encode(runs["float64"][n], ENC, np.int8)
                         assert np.array_equal(runs["float32"][n], runs["float64"][n])
                         if "complex128" in runs:
                             assert np.array_equal(runs["complex128"][n].real, runs["float64"][n])
-                            enc[f"{n}i"] = encode(runs["complex128"][n].imag)
+                            enc[f"{n}i"] = encode(runs["complex128"][n].imag, ENC, np.int8)
                     for n, e in enc.items():
                         if f"{k}/{n}" in out:                   # P-independent case, stored at P = 1
                             assert np.array_equal(out[f"{k}/{n}"], e)
@@ -163,7 +144,7 @@ def main():
 
     def t_refl(rank, P):
         wav, m, alpha = refl_inputs()
-        ny = rows_of(P, REFL_DIMS)
+        ny = rows_of(P, REFL_DIMS[0])
         ls = [(r * REFL_DIMS[1] * REFL_DIMS[2],) for r in ny]
         dims = (ny[rank],) + REFL_DIMS[1:]
         DDiag = BD([pylops.FirstDerivative(dims, axis=-1)])

@@ -29,6 +29,7 @@ import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
+from fixture_codec import encode, rows_of  # noqa: E402
 import make_golden_poststack as mgp  # noqa: E402
 
 DIMS = (60, 2, 24)
@@ -68,10 +69,6 @@ def post_cases():
             for dt in DTYPES if dt != "complex128" or complex_post(kind, nw)]
 
 
-def rows_of(P, n=DIMS[0]):
-    return [n // P + (1 if r < n % P else 0) for r in range(P)]
-
-
 def ns_key(P, axis, nh, nf, dh):
     return f"ns/P{P if axis == 0 else 'any'}/ax{axis}/nh{nh}/nf{nf}/dh{dh}"
 
@@ -101,19 +98,6 @@ def post_inputs(nw, dt):
     wav = taps((NT0, nw), 400 + nw).astype(np.real(np.ones(1, dt)).dtype)
     _, x, v = mgp.case_inputs(1, dt)
     return wav, x, v
-
-
-def decode(gold, k, dt):
-    f = [gold[f"{k}/{n}"].astype(np.float64) / ENC for n in ("y", "ya", "yi", "yai")[:4 if dt == "complex128" else 2]]
-    if dt == "complex128":
-        return f[0] + 1j * f[2], f[1] + 1j * f[3]
-    return f[0].astype(dt), f[1].astype(dt)
-
-
-def encode(y):
-    e = np.rint(np.asarray(y, dtype=np.float64) * ENC)
-    assert np.array_equal(e / ENC, y) and np.abs(e).max() <= 32767
-    return e.astype(np.int16)
 
 
 def ricker(t, f0):
@@ -161,11 +145,11 @@ def main():
     def store(k, runs):
         enc = {}
         for n in ("y", "ya"):
-            enc[n] = encode(runs["float64"][n])
+            enc[n] = encode(runs["float64"][n], ENC, np.int16)
             assert np.array_equal(runs["float32"][n], runs["float64"][n])
             if "complex128" in runs:
                 assert np.array_equal(runs["complex128"][n].real, runs["float64"][n])
-                enc[f"{n}i"] = encode(runs["complex128"][n].imag)
+                enc[f"{n}i"] = encode(runs["complex128"][n].imag, ENC, np.int16)
         for n, e in enc.items():
             if f"{k}/{n}" in out:                       # P-independent case, stored at P = 1
                 assert np.array_equal(out[f"{k}/{n}"], e)
@@ -174,7 +158,7 @@ def main():
 
     def t_ns(rank, P, axis, nh, nf, dh, dt):
         hs, ih, x, v = ns_inputs(nh, nf, dh, dt)
-        ny = rows_of(P)
+        ny = rows_of(P, DIMS[0])
         ls = [(r * DIMS[1] * DIMS[2],) for r in ny]
         Op = BD([NonStationaryConvolve1D((ny[rank],) + DIMS[1:], hs, ih, axis=axis, dtype=dt)], dtype=dt)
         return {"y": (Op @ DA.to_dist(x, local_shapes=ls)).asarray(),
@@ -196,7 +180,7 @@ def main():
 
     def t_post(rank, layout, P, kind, nw, dt):
         wav, x, v = post_inputs(nw, dt)
-        ny = mgp.rows_of(P)
+        ny = rows_of(P, mgp.NY)
         ls = [(r * NX * NT0,) for r in ny]
         Op = BD([local_post(layout, ny[rank], wav, kind)], dtype=dt)
         return {"y": (Op @ DA.to_dist(x, local_shapes=ls)).asarray(),
@@ -213,7 +197,7 @@ def main():
     def t_flow(rank, P):
         """tutorials/poststack.py's modelling and cgls, with one wavelet per time sample"""
         wav, m3d, mback3d = flow_inputs()
-        ny = mgp.rows_of(P, FLOW_NY)
+        ny = rows_of(P, FLOW_NY)
         y0, ny_i = sum(ny[:rank]), ny[rank]
         ls = [(r * NX * NT0,) for r in ny]
         m3d_dist = DA(global_shape=FLOW_NY * NX * NT0, local_shapes=ls)

@@ -32,6 +32,7 @@ import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
+from fixture_codec import encode, rows_of  # noqa: E402
 
 NY, NX, NZ = 4, 20, 24
 NHS = ((1, 1), (3, 5), (7, 3), (1, 9), (41, 41))
@@ -62,10 +63,6 @@ def key(nh, bank):
     return f"op/nh{nh[0]}x{nh[1]}/nf{nfx}x{nfz}/dh{dhx}x{dhz}"
 
 
-def rows_of(P, n=NY):
-    return [n // P + (1 if r < n % P else 0) for r in range(P)]
-
-
 def nodes(bank):
     """(ihx, ihz) of a bank: 1 + dh * arange(nf) per axis"""
     (nfx, nfz), (dhx, dhz) = bank
@@ -84,19 +81,6 @@ def case_inputs(nh, bank, dt):
     if dt == "complex128":
         x, v = x + 1j * xi, v + 1j * vi
     return hs, ihx, ihz, x.astype(dt), v.astype(dt)
-
-
-def decode(gold, k, dt):
-    f = [gold[f"{k}/{n}"].astype(np.float64) / ENC for n in ("y", "ya", "yi", "yai")[:4 if dt == "complex128" else 2]]
-    if dt == "complex128":
-        return f[0] + 1j * f[2], f[1] + 1j * f[3]
-    return f[0].astype(dt), f[1].astype(dt)
-
-
-def encode(y):
-    e = np.rint(np.asarray(y, dtype=np.float64) * ENC)
-    assert np.array_equal(e / ENC, y) and np.abs(e).max() < 2 ** 31
-    return e.astype(np.int32)
 
 
 def refshim_kirchhoff():
@@ -160,7 +144,7 @@ def main():
 
     def t_op(rank, P, nh, bank, dt):
         hs, ihx, ihz, x, v = case_inputs(nh, bank, dt)
-        ny = rows_of(P)
+        ny = rows_of(P, NY)
         k0 = sum(ny[:rank])
         ls = [(r * NX * NZ,) for r in ny]
         Op = BD([NonStationaryConvolve2D((NX, NZ), hs[k], ihx, ihz, dtype=dt) for k in range(k0, k0 + ny[rank])],
@@ -183,10 +167,10 @@ def main():
             k = key(nh, bank)
             for n in ("y", "ya"):
                 assert np.array_equal(runs["float32"][n], runs["float64"][n])
-                out[f"{k}/{n}"] = encode(runs["float64"][n])
+                out[f"{k}/{n}"] = encode(runs["float64"][n], ENC, np.int32)
                 if "complex128" in runs:
                     assert np.array_equal(runs["complex128"][n].real, runs["float64"][n])
-                    out[f"{k}/{n}i"] = encode(runs["complex128"][n].imag)
+                    out[f"{k}/{n}i"] = encode(runs["complex128"][n].imag, ENC, np.int32)
 
     # flow: the PSF bank and the migrated images from the restated Kirchhoff, in float64
     kirchhoff, _ = refshim_kirchhoff()

@@ -38,6 +38,7 @@ import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
+from fixture_codec import encode, rows_of  # noqa: E402
 
 NV, NX, NY, NZ = 4, 10, 11, 13
 NHS = ((1, 1, 1), (3, 5, 1), (1, 3, 7), (5, 3, 3), (13, 3, 15))
@@ -69,10 +70,6 @@ def key(nh, bank):
     return "op/nh{}x{}x{}/nf{}x{}x{}/dh{}x{}x{}".format(*nh, *nf, *dh)
 
 
-def rows_of(P, n=NV):
-    return [n // P + (1 if r < n % P else 0) for r in range(P)]
-
-
 def nodes(bank):
     """(ihx, ihy, ihz) of a bank: 1 + dh * arange(nf) per axis"""
     nf, dh = bank
@@ -90,19 +87,6 @@ def case_inputs(nh, bank, dt):
     if dt == "complex128":
         x, v = x + 1j * xi, v + 1j * vi
     return hs, nodes(bank), x.astype(dt), v.astype(dt)
-
-
-def decode(gold, k, dt):
-    f = [gold[f"{k}/{n}"].astype(np.float64) / ENC for n in ("y", "ya", "yi", "yai")[:4 if dt == "complex128" else 2]]
-    if dt == "complex128":
-        return f[0] + 1j * f[2], f[1] + 1j * f[3]
-    return f[0].astype(dt), f[1].astype(dt)
-
-
-def encode(y):
-    e = np.rint(np.asarray(y, dtype=np.float64) * ENC)
-    assert np.array_equal(e / ENC, y) and np.abs(e).max() < 2 ** 31
-    return e.astype(np.int32)
 
 
 def refshim_modules():
@@ -191,7 +175,7 @@ def main():
 
     def t_op(rank, P, nh, bank, dt):
         hs, ih, x, v = case_inputs(nh, bank, dt)
-        nv = rows_of(P)
+        nv = rows_of(P, NV)
         k0 = sum(nv[:rank])
         ls = [(r * NX * NY * NZ,) for r in nv]
         Op = BD([NonStationaryConvolve3D((NX, NY, NZ), hs[k], *ih, dtype=dt) for k in range(k0, k0 + nv[rank])],
@@ -214,10 +198,10 @@ def main():
             k = key(nh, bank)
             for n in ("y", "ya"):
                 assert np.array_equal(runs["float32"][n], runs["float64"][n])
-                out[f"{k}/{n}"] = encode(runs["float64"][n])
+                out[f"{k}/{n}"] = encode(runs["float64"][n], ENC, np.int32)
                 if "complex128" in runs:
                     assert np.array_equal(runs["complex128"][n].real, runs["float64"][n])
-                    out[f"{k}/{n}i"] = encode(runs["complex128"][n].imag)
+                    out[f"{k}/{n}i"] = encode(runs["complex128"][n].imag, ENC, np.int32)
 
     # flow: the PSF bank and the migrated volumes from the restated 3-D Kirchhoff, in float64
     kirchhoff3d, _, _ = refshim_modules()

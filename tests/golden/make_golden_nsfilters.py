@@ -49,6 +49,7 @@ import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
+from fixture_codec import encode, rows_of  # noqa: E402
 import make_golden_nsconvolve as mgn  # noqa: E402
 import make_golden_nsconvolve2d as mg2  # noqa: E402
 from make_golden_nsconvolve2d import BANKS as BANKS2, NX, NZ, nodes  # noqa: E402
@@ -83,10 +84,6 @@ def key(kind, nh, bank):
     return f"f2/nh{nh[0]}x{nh[1]}/nf{nfx}x{nfz}/dh{dhx}x{dhz}"
 
 
-def rows_of(P, n=NI):
-    return [n // P + (1 if r < n % P else 0) for r in range(P)]
-
-
 def case_inputs(kind, nh, bank, dt):
     """NI inputs (the real dtype of dt, shape (NI, N1) or (NI, NX, NZ)), the node indices (a tuple of arrays), the
     bank shape, the model x (dtype dt) and the global data v (dtype dt)"""
@@ -104,19 +101,6 @@ def case_inputs(kind, nh, bank, dt):
     if dt == "complex128":
         x, v = x + 1j * xi, v + 1j * vi
     return inp, ih, bshape, x.astype(dt), v.astype(dt)
-
-
-def decode(gold, k, dt):
-    f = [gold[f"{k}/{n}"].astype(np.float64) / ENC for n in ("y", "ya", "yi", "yai")[:4 if dt == "complex128" else 2]]
-    if dt == "complex128":
-        return f[0] + 1j * f[2], f[1] + 1j * f[3]
-    return f[0].astype(dt), f[1].astype(dt)
-
-
-def encode(y):
-    e = np.rint(np.asarray(y, dtype=np.float64) * ENC)
-    assert np.array_equal(e / ENC, y) and np.abs(e).max() < 2 ** 31
-    return e.astype(np.int32)
 
 
 def restated(name):
@@ -163,7 +147,7 @@ def main():
 
     def t_op(rank, P, kind, nh, bank, dt):
         inp, ih, bshape, x, v = case_inputs(kind, nh, bank, dt)
-        ny = rows_of(P)
+        ny = rows_of(P, NI)
         k0 = sum(ny[:rank])
         plane = int(np.prod(inp.shape[1:]))
         if kind == 1:
@@ -192,10 +176,10 @@ def main():
                     assert np.array_equal(res[n], runs[dt][n])
         for n in ("y", "ya"):
             assert np.array_equal(runs["float32"][n], runs["float64"][n])
-            out[f"{k}/{n}"] = encode(runs["float64"][n])
+            out[f"{k}/{n}"] = encode(runs["float64"][n], ENC, np.int32)
             if "complex128" in runs:
                 assert np.array_equal(runs["complex128"][n].real, runs["float64"][n])
-                out[f"{k}/{n}i"] = encode(runs["complex128"][n].imag)
+                out[f"{k}/{n}i"] = encode(runs["complex128"][n].imag, ENC, np.int32)
 
     # flows, in float64
     import importlib

@@ -29,6 +29,7 @@ import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
+from fixture_codec import encode, rows_of  # noqa: E402
 
 NY, NX, NT0 = 5, 4, 33
 LAYOUTS = ("native", "tut")
@@ -51,11 +52,6 @@ def cases():
             for dt in DTYPES if dt != "complex128" or complex_case(layout, kind, nh)]
 
 
-def rows_of(P, ny=NY):
-    """rows of y per rank (the reference's SCATTER split)"""
-    return [ny // P + (1 if r < ny % P else 0) for r in range(P)]
-
-
 def block_dims(layout, ny_r):
     return (NT0, ny_r, NX) if layout == "native" else (ny_r, NX, NT0)
 
@@ -75,21 +71,6 @@ def case_inputs(nh, dt):
     if dt == "complex128":
         x, v = x + 1j * xi, v + 1j * vi
     return wav, x.astype(dt), v.astype(dt)
-
-
-def expected(gold, layout, P, kind, nh, dt):
-    """the reference's gathered (forward, adjoint) outputs of one case, decoded from the fixture, in dtype dt"""
-    k = key(layout, P, kind, nh)
-    f = [gold[f"{k}/{n}"].astype(np.float64) / ENC for n in ("y", "ya", "yi", "yai")[:4 if dt == "complex128" else 2]]
-    if dt == "complex128":
-        return f[0] + 1j * f[2], f[1] + 1j * f[3]
-    return f[0].astype(dt), f[1].astype(dt)
-
-
-def encode(y):
-    e = np.rint(np.asarray(y, dtype=np.float64) * ENC)
-    assert np.array_equal(e / ENC, y) and np.abs(e).max() <= 32767
-    return e.astype(np.int16)
 
 
 def ricker(t, f0):
@@ -140,7 +121,7 @@ def main():
 
     def t_op(rank, layout, P, kind, nh, dt):
         wav, x, v = case_inputs(nh, dt)
-        ny = rows_of(P)
+        ny = rows_of(P, NY)
         ls = [(r * NX * NT0,) for r in ny]
         Op = BD([local_op(layout, ny[rank], wav, kind)], dtype=dt)
         fwd = Op @ DA.to_dist(x, local_shapes=ls)
@@ -160,11 +141,11 @@ def main():
                     k = key(layout, P, kind, nh)
                     enc = {}
                     for n in ("y", "ya"):
-                        enc[n] = encode(runs["float64"][n])
+                        enc[n] = encode(runs["float64"][n], ENC, np.int16)
                         assert np.array_equal(runs["float32"][n], runs["float64"][n])
                         if "complex128" in runs:
                             assert np.array_equal(runs["complex128"][n].real, runs["float64"][n])
-                            enc[f"{n}i"] = encode(runs["complex128"][n].imag)
+                            enc[f"{n}i"] = encode(runs["complex128"][n].imag, ENC, np.int16)
                     for n, e in enc.items():
                         if f"{k}/{n}" in out:                   # P-independent case, stored at P = 1
                             assert np.array_equal(out[f"{k}/{n}"], e)

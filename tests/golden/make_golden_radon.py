@@ -39,6 +39,7 @@ import numpy as np
 HERE = os.path.dirname(os.path.abspath(__file__))
 REFSHIM = os.path.join(HERE, "refshim")
 sys.path.insert(0, HERE)
+from fixture_codec import encode, rows_of  # noqa: E402
 
 NG = 6
 DT = 2.0 ** -8
@@ -84,10 +85,6 @@ def key(ndim, kind, interp, centeredh, nh):
     return f"op/{ndim}d/{kind}/i{int(interp)}/c{int(centeredh)}" + (f"/nh{nh}" if ndim == 2 else "")
 
 
-def rows_of(P, n=NG):
-    return [n // P + (1 if r < n % P else 0) for r in range(P)]
-
-
 def haxis(nh, dh, centeredh):
     """physical offsets: centred gathers any origin (the operator recentres them), else traces -1 .. nh - 2"""
     return (np.arange(nh) - (nh // 2 if centeredh else 1)) * dh
@@ -125,20 +122,6 @@ def case_inputs(ndim, kind, interp, centeredh, nh, dt):
     if dt == "complex128":
         x, v = x + 1j * xi, v + 1j * vi
     return x.astype(dt), v.astype(dt)
-
-
-def decode(gold, k, dt, exact_case=True):
-    names = ("y", "ya", "yi", "yai")[:4 if dt == "complex128" else 2]
-    f = [gold[f"{k}/{n}"].astype(np.float64) / (ENC if exact_case else 1) for n in names]
-    if dt == "complex128":
-        return f[0] + 1j * f[2], f[1] + 1j * f[3]
-    return f[0].astype(dt), f[1].astype(dt)
-
-
-def encode(y):
-    e = np.rint(np.asarray(y, dtype=np.float64) * ENC)
-    assert np.array_equal(e / ENC, y) and np.abs(e).max() < 2 ** 31
-    return e.astype(np.int32)
 
 
 def restated(ndim):
@@ -190,7 +173,7 @@ def main():
     def t_op(rank, P, ndim, kind, interp, centeredh, nh, dt):
         x, v = case_inputs(ndim, kind, interp, centeredh, nh, dt)
         nm, nd = sizes(ndim, kind, nh)
-        ny = rows_of(P)
+        ny = rows_of(P, NG)
         R = restated(ndim)
         ops = [R(taxis(ndim), *axes(ndim, kind, centeredh, nh), kind=kind, centeredh=centeredh, interp=interp,
                  dtype="float32" if dt == "float32" else "float64") for _ in range(ny[rank])]
@@ -214,13 +197,13 @@ def main():
         for n in ("y", "ya"):
             if ex:
                 assert np.array_equal(runs["float32"][n], runs["float64"][n])
-                out[f"{k}/{n}"] = encode(runs["float64"][n])
+                out[f"{k}/{n}"] = encode(runs["float64"][n], ENC, np.int32)
             else:
                 assert np.array_equal(runs["float32"][n], runs["float64"][n].astype(np.float32))
                 out[f"{k}/{n}"] = runs["float64"][n]
             if "complex128" in runs:
                 assert np.array_equal(runs["complex128"][n].real, runs["float64"][n])
-                out[f"{k}/{n}i"] = encode(runs["complex128"][n].imag)
+                out[f"{k}/{n}i"] = encode(runs["complex128"][n].imag, ENC, np.int32)
 
     # flow, in float64
     t, h, p = flow_axes()

@@ -11,6 +11,8 @@ import itertools
 
 import numpy as np
 
+from op_checks import guarded_twice
+
 U = {np.float32: 2.0 ** -24, np.float64: 2.0 ** -53}
 
 
@@ -105,22 +107,6 @@ def check_close(got, x, hs, oh, dh, adjoint, dt):
 # ---------------------------------------------------------------------------------------------------------------
 # the kernels through the C ABI
 # ---------------------------------------------------------------------------------------------------------------
-def guarded_twice(call, n, dt, guard=5):
-    """``call(y)`` twice, y the interior n elements of a buffer with ``guard`` cells of 7.25 on either side; returns
-    (the first result on the host, guards intact, second call bit-equal)"""
-    import torch
-    tdt = {np.float32: torch.float32, np.float64: torch.float64}[dt]
-    yb = torch.full((n + 2 * guard,), 7.25, dtype=tdt, device="cuda")
-    y = yb[guard:guard + n]
-    assert call(y.data_ptr()) == 0
-    first = y.clone()
-    assert call(y.data_ptr()) == 0
-    torch.cuda.synchronize()
-    g = yb.cpu().numpy()
-    guards_ok = bool(np.all(g[:guard] == 7.25) and np.all(g[guard + n:] == 7.25))
-    return first.cpu().numpy(), guards_ok, bool(torch.equal(first, y))
-
-
 def c_ns(pm, x, y, dims, ni, hs, nf, nh, oh, dh, adjoint, code):
     """b2_nsconvolve2d / b2_nsconvolve3d, by the rank of ``dims``"""
     L = pm._lib

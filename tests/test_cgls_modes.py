@@ -3,6 +3,7 @@ it as a CUDA graph, ``run()`` executing it eagerly for an operator that is not g
 ``show=True`` and a callback (both of which run per iteration)."""
 import numpy as np
 import pytest
+from op_checks import host
 
 pytestmark = pytest.mark.gpu
 
@@ -14,10 +15,6 @@ FIELDS = ("x", "cost", "cost1", "iiter", "istop", "r1norm", "r2norm")
 def pm():
     import pylops_mpi_b200 as pm
     return pm
-
-
-def host(t):
-    return t.cpu().numpy()
 
 
 def problem(pm, dtype, layout):

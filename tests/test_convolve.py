@@ -6,18 +6,18 @@
 CPU: refshim's restatement of pylops 2.x against that definition, and the fixtures of
 tests/golden/convolve_golden.npz (made by make_golden_convolve.py: the reference's MPIBlockDiag and ISTA over the
 restatement; inputs exactly representable, so every dtype must match them bit for bit).  GPU: the b2_convolve_axis kernel through the C ABI and the operator through the public interface."""
-import ctypes as C
 import os
-import subprocess
 import sys
 
 import numpy as np
 import pytest
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
 sys.path.insert(0, os.path.join(HERE, "golden"))
 import make_golden_convolve as mgc  # noqa: E402
+from fixture_codec import decode, rows_of  # noqa: E402
+from op_checks import (assert_cgls_replay_matches_steps, assert_rejected, device_input, guarded_twice, host,  # noqa: E402
+                       needs_gpus, run_on_ranks)
 
 GOLD = np.load(os.path.join(HERE, "golden", "convolve_golden.npz"), allow_pickle=False)
 CASES = mgc.cases()
@@ -101,11 +101,11 @@ def test_convolve_fixture_inventory():
 def test_fixtures_follow_the_pinned_definition(case):
     P, axis, nh, off, dt = case
     h, x, y = mgc.case_inputs(nh, dt)
-    parts = np.cumsum([0] + mgc.rows_of(P))
+    parts = np.cumsum([0] + rows_of(P, mgc.DIMS[0]))
     x3, y3 = x.reshape(mgc.DIMS), y.reshape(mgc.DIMS)
     fwd = np.concatenate([conv_ref(x3[a:b], h, off, False, axis) for a, b in zip(parts[:-1], parts[1:])])
     adj = np.concatenate([conv_ref(y3[a:b], h, off, True, axis) for a, b in zip(parts[:-1], parts[1:])])
-    gy, gya = mgc.expected(GOLD, P, axis, nh, off, dt)
+    gy, gya = decode(GOLD, mgc.key(P, axis, nh, off), dt, mgc.ENC)
     np.testing.assert_array_equal(gy, fwd.ravel())       # exact: every value is a multiple of 1/2
     np.testing.assert_array_equal(gya, adj.ravel())
 
@@ -117,10 +117,6 @@ def test_fixtures_follow_the_pinned_definition(case):
 def pm():
     import pylops_mpi_b200 as pm
     return pm
-
-
-def host(t):
-    return t.cpu().numpy()
 
 
 def c_conv(pm, x, y, shape, h, nh, off, adjoint, dtype_code):
@@ -138,26 +134,12 @@ def axis_lengths(nh):
 
 def run_kernel(pm, x_np, h_np, off, adjoint, dt, misalign=False, guard=5):
     """apply through the C ABI into a guarded interior view; returns (y, guards intact, second apply bit-equal)"""
-    import torch
-    tdt = {np.float32: torch.float32, np.float64: torch.float64}[dt]
-    N = x_np.size
-    s = 1 if misalign else 0
-    xb = torch.zeros(N + s, dtype=tdt, device="cuda")
-    xb[s:] = torch.as_tensor(x_np.ravel().astype(dt))
-    x = xb[s:]
-    yb = torch.full((N + 2 * guard + s,), 7.25, dtype=tdt, device="cuda")
-    y = yb[guard + s:guard + s + N]
-    h = torch.as_tensor(np.asarray(h_np, dtype=dt)).cuda()
+    x, h = device_input(x_np, dt, misalign), device_input(h_np, dt)
     code = pm._lib.F32 if dt == np.float32 else pm._lib.F64
-    rc = c_conv(pm, x.data_ptr(), y.data_ptr(), x_np.shape, h.data_ptr(), h.numel(), off, int(adjoint), code)
-    assert rc == 0, pm._lib.lib.b2_strerror(rc)
-    first = y.clone()
-    rc = c_conv(pm, x.data_ptr(), y.data_ptr(), x_np.shape, h.data_ptr(), h.numel(), off, int(adjoint), code)
-    assert rc == 0
-    torch.cuda.synchronize()
-    g = host(yb)
-    guards_ok = bool(np.all(g[:guard + s] == 7.25) and np.all(g[guard + s + N:] == 7.25))
-    return host(first).reshape(x_np.shape), guards_ok, bool(torch.equal(first, y))
+    y, guards_ok, same = guarded_twice(
+        lambda yp: c_conv(pm, x.data_ptr(), yp, x_np.shape, h.data_ptr(), h.numel(), off, int(adjoint), code),
+        x_np.size, dt, guard, int(misalign))
+    return y.reshape(x_np.shape), guards_ok, same
 
 
 def check_close(got, x, h, off, adjoint, dt, axis=1):
@@ -227,13 +209,8 @@ def test_kernel_error_codes_leave_y_untouched(pm):
         (dict(h=None), ARG), (dict(x=None), ARG), (dict(y=None), ARG), (dict(y="x"), ARG),
         (dict(dtype=L.C64), DT), (dict(dtype=L.BF16), DT), (dict(dtype=99), DT),
     ]
-    for kw, want in cases:
-        a = dict(x=x.data_ptr(), y=y.data_ptr(), h=h.data_ptr(), nh=4, off=1, dtype=L.F64)
-        a.update(kw)
-        if a["y"] == "x":
-            a["y"] = a["x"]
-        rc = c_conv(pm, a["x"], a["y"], (2, 3, 4), a["h"], a["nh"], a["off"], 0, a["dtype"])
-        assert rc == want, (kw, rc)
+    assert_rejected(lambda a: c_conv(pm, a["x"], a["y"], (2, 3, 4), a["h"], a["nh"], a["off"], 0, a["dtype"]),
+                    dict(x=x.data_ptr(), y=y.data_ptr(), h=h.data_ptr(), nh=4, off=1, dtype=L.F64), cases, y)
     for shape in ((0, 3, 4), (2, 0, 4), (2, 3, 0)):
         assert c_conv(pm, x.data_ptr(), y.data_ptr(), shape, h.data_ptr(), 4, 1, 0, L.F64) == 0
     torch.cuda.synchronize()
@@ -245,7 +222,7 @@ def test_kernel_error_codes_leave_y_untouched(pm):
 # ---------------------------------------------------------------------------------------------------------------
 def blockdiag(pm, P, axis, h, off, dt):
     return pm.MPIBlockDiag([pm.local.Convolve1D((ny,) + mgc.DIMS[1:], h, offset=off, axis=axis, dtype=dt)
-                            for ny in mgc.rows_of(P)])
+                            for ny in rows_of(P, mgc.DIMS[0])])
 
 
 @pytest.mark.gpu
@@ -259,7 +236,7 @@ def test_operator_vs_reference_fixtures(pm, case):
     got = host((Op @ pm.DistributedArray.to_dist(x)).asarray())
     gota = host((Op.H @ pm.DistributedArray.to_dist(y)).asarray())
     assert got.dtype == np.dtype(dt) and gota.dtype == np.dtype(dt)
-    gy, gya = mgc.expected(GOLD, P, axis, nh, off, dt)
+    gy, gya = decode(GOLD, mgc.key(P, axis, nh, off), dt, mgc.ENC)
     np.testing.assert_array_equal(got, gy)
     np.testing.assert_array_equal(gota, gya)
 
@@ -277,9 +254,6 @@ def test_real_taps_on_complex_data_keep_the_imaginary_part(pm):
         assert y.dtype == np.complex128
         np.testing.assert_allclose(y, conv_ref(x.reshape(6, 40), h, 4, False, axis).ravel(), rtol=1e-12, atol=1e-12)
         np.testing.assert_allclose(ya, conv_ref(x.reshape(6, 40), h, 4, True, axis).ravel(), rtol=1e-12, atol=1e-12)
-        out = torch.zeros(240, dtype=torch.complex128, device="cuda")
-        Cop.matvec(torch.as_tensor(x).cuda(), out=out)
-        np.testing.assert_array_equal(host(out), y)
 
 
 @pytest.mark.gpu
@@ -320,7 +294,7 @@ def test_operator_dottest(pm, dt):
 def test_reflectivity_ista_vs_reference(pm, P):
     wav, m, alpha = mgc.refl_inputs()
     assert alpha == float(GOLD["refl/alpha"])
-    dims = [(ny,) + mgc.REFL_DIMS[1:] for ny in mgc.rows_of(P, mgc.REFL_DIMS)]
+    dims = [(ny,) + mgc.REFL_DIMS[1:] for ny in rows_of(P, mgc.REFL_DIMS[0])]
     DDiag = pm.MPIBlockDiag([pm.local.FirstDerivative(d, axis=-1) for d in dims])
     CDiag = pm.MPIBlockDiag([pm.local.Convolve1D(d, wav, offset=mgc.REFL_OFF, axis=-1) for d in dims])
     d = CDiag @ (DDiag @ pm.DistributedArray.to_dist(m))
@@ -335,26 +309,11 @@ def test_reflectivity_ista_vs_reference(pm, P):
 @pytest.mark.gpu
 @pytest.mark.parametrize("axis", [-1, 0])
 def test_cgls_graph_replay_matches_step_loop(pm, axis):
-    from pylops_mpi_b200.optimization.cls_basic import CGLS, _graph_safe
     rng = np.random.default_rng(12)
     dims = (16, 24, 40)
     Op = pm.MPIBlockDiag([pm.local.Convolve1D(dims, rng.standard_normal(11), offset=5, axis=axis)])
-    assert _graph_safe(Op)
     y = Op @ pm.DistributedArray.to_dist(rng.standard_normal(int(np.prod(dims))))
-    x0 = np.zeros(int(np.prod(dims)))
-    a = CGLS(Op)
-    xa = a.setup(y=y, x0=pm.DistributedArray.to_dist(x0), niter=25, damp=0.0, tol=0.0)
-    xa = a.run(xa, 25)
-    a.finalize()
-    assert a.graph_error is None, a.graph_error
-    assert a.graph_replays >= 20
-    b = CGLS(Op)
-    xb = b.setup(y=y, x0=pm.DistributedArray.to_dist(x0), niter=25, damp=0.0, tol=0.0)
-    for _ in range(25):
-        xb = b.step(xb)
-    b.finalize()
-    np.testing.assert_array_equal(host(xa.asarray()), host(xb.asarray()))
-    np.testing.assert_array_equal(np.asarray(a.cost), np.asarray(b.cost))
+    assert_cgls_replay_matches_steps(pm, Op, y, pm.DistributedArray.to_dist(np.zeros(int(np.prod(dims)))), 25, 20)
 
 
 @pytest.mark.gpu
@@ -376,12 +335,48 @@ def test_axis_last_matches_torch_conv1d(pm, dt, nh, off):
 
 
 @pytest.mark.gpu
-def test_multi_rank_fixtures_p2():
-    import torch
-    if torch.cuda.device_count() < 2:
-        pytest.skip(f"needs 2 GPUs, box has {torch.cuda.device_count()}")
-    r = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node=2",
-                        "--master-addr", "127.0.0.1", "--master-port", "29811",
-                        os.path.join(HERE, "convolve_worker.py")], capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, (r.stdout[-4000:] + r.stderr[-8000:])
-    assert r.stdout.count("CONVOLVE_WORKER_OK") == 2
+@pytest.mark.parametrize("nproc", [1, 2])
+def test_multi_rank_fixtures(nproc):
+    needs_gpus(nproc)
+    run_on_ranks("test_convolve", nproc)
+
+
+def on_ranks(pm, comm):
+    """each rank's MPIBlockDiag([Convolve1D]) block against its slice of the gathered fixtures, and the reflectivity
+    ISTA flow against its fixture"""
+    rank, P = comm.Get_rank(), comm.Get_size()
+
+    def block(dims_global):
+        """this rank's rows of a global array split along axis 0: (local_shapes, flat slice, local dims)"""
+        rows = rows_of(P, dims_global[0])
+        plane = int(np.prod(dims_global[1:]))
+        lo, hi = sum(rows[:rank]) * plane, sum(rows[:rank + 1]) * plane
+        return [(r * plane,) for r in rows], slice(lo, hi), (rows[rank],) + tuple(dims_global[1:])
+
+    def check(name, got, ref, rtol, atol):
+        np.testing.assert_allclose(got, ref, rtol=rtol, atol=atol, err_msg=f"[rank {rank}] {name}")
+
+    ls, sl, dims = block(mgc.DIMS)
+    for (Pc, axis, nh, off, dt) in CASES:
+        if Pc != P:
+            continue
+        h, x, v = mgc.case_inputs(nh, dt)
+        Op = pm.MPIBlockDiag([pm.local.Convolve1D(dims, h, offset=off, axis=axis, dtype=dt)])
+        gy, gya = decode(GOLD, mgc.key(P, axis, nh, off), dt, mgc.ENC)   # exact: the inputs are exactly representable
+        name = f"{mgc.key(P, axis, nh, off)}/{dt}"
+        np.testing.assert_array_equal(host((Op @ pm.DistributedArray.to_dist(x, local_shapes=ls)).local_array),
+                                      gy[sl], err_msg=f"[rank {rank}] {name}/y")
+        np.testing.assert_array_equal(host((Op.H @ pm.DistributedArray.to_dist(v, local_shapes=ls)).local_array),
+                                      gya[sl], err_msg=f"[rank {rank}] {name}/ya")
+
+    ls, sl, dims = block(mgc.REFL_DIMS)
+    wav, m, alpha = mgc.refl_inputs()
+    DDiag = pm.MPIBlockDiag([pm.local.FirstDerivative(dims, axis=-1)])
+    CDiag = pm.MPIBlockDiag([pm.local.Convolve1D(dims, wav, offset=mgc.REFL_OFF, axis=-1)])
+    d = CDiag @ (DDiag @ pm.DistributedArray.to_dist(m, local_shapes=ls))
+    check("refl/d", host(d.local_array), GOLD["refl/d"][sl], 1e-12, 1e-12)
+    x0 = pm.DistributedArray.to_dist(np.zeros_like(m), local_shapes=ls)
+    x, iiter, cost = pm.ista(CDiag, d, x0, niter=mgc.REFL_NITER, eps=mgc.REFL_EPS, alpha=alpha, tol=1e-10)
+    assert iiter == int(GOLD[f"refl/P{P}/iiter"])
+    check("refl/cost", np.asarray(cost), GOLD[f"refl/P{P}/cost"], 1e-10, 0)
+    check("refl/x", host(x.local_array), GOLD[f"refl/P{P}/x"][sl], 1e-9, 1e-11)

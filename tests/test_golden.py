@@ -13,6 +13,7 @@ import numpy as np
 import pytest
 
 import pylops_mpi_oracle as o
+from op_checks import host
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 GOLD = np.load(os.path.join(HERE, "golden", "reference_golden.npz"), allow_pickle=False)
@@ -218,10 +219,6 @@ def test_oracle_fredholm(case):
 def pm():
     import pylops_mpi_b200 as pm
     return pm
-
-
-def host(t):
-    return t.cpu().numpy()
 
 
 @pytest.mark.gpu

@@ -2,23 +2,15 @@
 on any GPU box (the whole worker through the torchrun/NCCL-less path); 2 / 4 / 8 need that many GPUs
 (4 also covers the square-grid MPIMatrixMult paths) and are skipped otherwise."""
 import os
-import subprocess
-import sys
 
 import pytest
-import torch
+
+from op_checks import HERE, needs_gpus, run_on_ranks
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 @pytest.mark.parametrize("nproc", [1, 2, 4, 8])
 def test_multi_rank_parity(nproc):
-    if torch.cuda.device_count() < nproc:
-        pytest.skip(f"needs {nproc} GPUs, box has {torch.cuda.device_count()}")
-    r = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", f"--nproc-per-node={nproc}",
-                        "--master-addr", "127.0.0.1", "--master-port", str(29700 + nproc),
-                        os.path.join(ROOT, "tests", "multi_worker.py")],
-                       capture_output=True, text=True, timeout=1500)
-    assert r.returncode == 0, (r.stdout[-4000:] + r.stderr[-8000:])
-    assert r.stdout.count("MULTI_WORKER_OK") == nproc
+    needs_gpus(nproc)
+    assert run_on_ranks(os.path.join(HERE, "multi_worker.py"), nproc, timeout=1500).count("MULTI_WORKER_OK") == nproc

@@ -7,6 +7,7 @@ import pytest
 import torch
 
 import pylops_mpi_oracle as o
+from op_checks import host
 
 pytestmark = pytest.mark.gpu
 
@@ -15,10 +16,6 @@ pytestmark = pytest.mark.gpu
 def pm():
     import pylops_mpi_b200 as pm
     return pm
-
-
-def host(t):
-    return t.cpu().numpy() if isinstance(t, torch.Tensor) else np.asarray(t)
 
 
 # ---- DistributedArray: test_distributedarray.py ------------------------------------------

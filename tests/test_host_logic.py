@@ -147,12 +147,9 @@ print("WORKER_OK", rank)
 def test_comm_shim_world_size_2_gloo(tmp_path):
     script = tmp_path / "worker.py"
     script.write_text(_WORKER)
-    env = dict(os.environ, CUDA_VISIBLE_DEVICES="")
-    r = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node=2",
-                        "--master-addr", "127.0.0.1", "--master-port", "29631", str(script), ROOT],
-                       capture_output=True, text=True, timeout=300, env=env)
-    assert r.returncode == 0, r.stdout + r.stderr
-    assert r.stdout.count("WORKER_OK") == 2
+    from op_checks import run_on_ranks
+    out = run_on_ranks(str(script), 2, args=(ROOT,), env=dict(CUDA_VISIBLE_DEVICES=""), timeout=300)
+    assert out.count("WORKER_OK") == 2
 
 
 # ---- the boundary is a C ABI: a plain-C99 client must compile against the header and link the library ------------

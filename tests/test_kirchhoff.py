@@ -5,7 +5,6 @@ CPU: refshim's restatement against explicit dense matrices built from the defini
 make_golden_kirchhoff.py: the reference's MPIVStack and cgls over the restatement).  GPU: the b2_kirchhoff kernel
 through the C ABI against the vectorised NumPy restatement, and the operators through the public interface."""
 import os
-import subprocess
 import sys
 
 import numpy as np
@@ -14,6 +13,8 @@ import pytest
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "golden"))
 import make_golden_kirchhoff as mgk  # noqa: E402
+from op_checks import (assert_cgls_replay_matches_steps, assert_rejected, guarded_twice, host,  # noqa: E402
+                       needs_gpus, run_on_ranks)
 
 GOLD = np.load(os.path.join(HERE, "golden", "kirchhoff_golden.npz"), allow_pickle=False)
 KREF, WAVELETS_MOD = mgk.refshim()
@@ -188,10 +189,6 @@ def pm():
     return pm
 
 
-def host(t):
-    return t.cpu().numpy()
-
-
 def c_kirch(pm, x, y, ts, tr, ni, ns, nr, nt, dt, adjoint, code):
     L = pm._lib
     return L.lib.b2_kirchhoff(L.ctx(), x, y, ts, tr, ni, ns, nr, nt, dt, adjoint, code, L.stream())
@@ -212,24 +209,15 @@ def run_kernel(pm, x_np, ts, tr, nt, dt, adjoint, dtype, guard=3):
     """b2_kirchhoff into an output at an odd element offset inside a guarded buffer; returns (y, guards intact,
     second apply bit-equal)"""
     import torch
-    tdt = {np.float32: torch.float32, np.float64: torch.float64}[dtype]
     ni, ns = ts.shape
     nr = tr.shape[1]
-    nout = ni if adjoint else ns * nr * nt
     x = torch.as_tensor(np.ascontiguousarray(x_np.ravel().astype(dtype))).cuda()
-    yb = torch.full((nout + 2 * guard + 1,), 7.25, dtype=tdt, device="cuda")
-    y = yb[guard + 1:guard + 1 + nout]
     tsd = torch.as_tensor(np.ascontiguousarray(ts.T)).cuda()
     trd = torch.as_tensor(np.ascontiguousarray(tr.T)).cuda()
     code = pm._lib.F32 if dtype == np.float32 else pm._lib.F64
     args = (tsd.data_ptr(), trd.data_ptr(), ni, ns, nr, nt, dt, int(adjoint), code)
-    assert c_kirch(pm, x.data_ptr(), y.data_ptr(), *args) == 0
-    first = y.clone()
-    assert c_kirch(pm, x.data_ptr(), y.data_ptr(), *args) == 0
-    torch.cuda.synchronize()
-    g = host(yb)
-    guards = bool(np.all(g[:guard + 1] == 7.25) and np.all(g[guard + 1 + nout:] == 7.25))
-    return host(first), guards, bool(torch.equal(first, y))
+    return guarded_twice(lambda yp: c_kirch(pm, x.data_ptr(), yp, *args), ni if adjoint else ns * nr * nt, dtype,
+                         guard, 1)
 
 
 def forward_bound(x, ts, tr, dt, nt):
@@ -343,20 +331,10 @@ def test_kernel_error_codes_leave_y_untouched(pm):
         (dict(dtype=L.C64), DT), (dict(dtype=L.C128), DT), (dict(dtype=L.BF16), DT), (dict(dtype=99), DT),
     ]
     for adjoint in (0, 1):
-        for kw, want in cases:
-            a = dict(x=x.data_ptr(), y=y.data_ptr(), ts=ts.data_ptr(), tr=tr.data_ptr(), ni=ni, ns=ns, nr=nr, nt=nt,
-                     dt=0.004, dtype=L.F64)
-            a.update(kw)
-            if a["y"] == "x":
-                a["y"] = a["x"]
-            rc = L.lib.b2_kirchhoff(L.ctx(), a["x"], a["y"], a["ts"], a["tr"], a["ni"], a["ns"], a["nr"], a["nt"],
-                                    a["dt"], adjoint, a["dtype"], L.stream())
-            assert rc == want, (kw, adjoint, rc)
-        rc = L.lib.b2_kirchhoff(None, x.data_ptr(), y.data_ptr(), ts.data_ptr(), tr.data_ptr(), ni, ns, nr, nt, 0.004,
-                                adjoint, L.F64, L.stream())
-        assert rc == ARG
-    torch.cuda.synchronize()
-    assert torch.all(y == 3.5)
+        assert_rejected(lambda a: L.lib.b2_kirchhoff(a["ctx"], a["x"], a["y"], a["ts"], a["tr"], a["ni"], a["ns"], a["nr"],
+                                                     a["nt"], a["dt"], adjoint, a["dtype"], L.stream()),
+                        dict(ctx=L.ctx(), x=x.data_ptr(), y=y.data_ptr(), ts=ts.data_ptr(), tr=tr.data_ptr(), ni=ni,
+                             ns=ns, nr=nr, nt=nt, dt=0.004, dtype=L.F64), cases + [(dict(ctx=None), ARG)], y)
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -440,16 +418,6 @@ def test_operator_complex_data_and_out(pm):
         f = K.rmatvec if adjoint else K.matvec
         y = f(a)
         assert y.dtype == torch.complex128
-        assert torch.equal(y.real, f(a.real.contiguous())) and torch.equal(y.imag, f(a.imag.contiguous()))
-        out = torch.zeros(K.shape[1] if adjoint else K.shape[0], dtype=torch.complex128, device="cuda")
-        f(a, out=out)
-        assert torch.equal(out, y)
-        r = a.real.contiguous()
-        outr = torch.full_like(out.real, 5.0).contiguous()
-        f(r, out=outr)
-        assert torch.equal(outr, f(r))
-    with pytest.raises(ValueError):
-        K.matvec(torch.zeros(K.shape[1] + 1, dtype=torch.float64, device="cuda"))
 
 
 @pytest.mark.gpu
@@ -567,34 +535,52 @@ def test_tutorial_flow_vs_reference(pm, P):
 
 @pytest.mark.gpu
 def test_cgls_graph_replay_matches_step_loop(pm):
-    from pylops_mpi_b200.optimization.cls_basic import CGLS, _graph_safe
     Op = op_vstack(pm, 2, "ricker21")
-    assert _graph_safe(Op)
     rng = np.random.default_rng(12)
     y = Op @ bcast(pm, rng.standard_normal(Op.shape[1]))
-    x0 = np.zeros(Op.shape[1])
-    a = CGLS(Op)
-    xa = a.setup(y=y, x0=bcast(pm, x0), niter=25, damp=0.0, tol=0.0)
-    xa = a.run(xa, 25)
-    a.finalize()
-    assert a.graph_error is None, a.graph_error
-    assert a.graph_replays >= 20
-    b = CGLS(Op)
-    xb = b.setup(y=y, x0=bcast(pm, x0), niter=25, damp=0.0, tol=0.0)
-    for _ in range(25):
-        xb = b.step(xb)
-    b.finalize()
-    np.testing.assert_array_equal(host(xa.asarray()), host(xb.asarray()))
-    np.testing.assert_array_equal(np.asarray(a.cost), np.asarray(b.cost))
+    assert_cgls_replay_matches_steps(pm, Op, y, bcast(pm, np.zeros(Op.shape[1])), 25, 20)
 
 
 @pytest.mark.gpu
-def test_multi_rank_fixtures_p2():
-    import torch
-    if torch.cuda.device_count() < 2:
-        pytest.skip(f"needs 2 GPUs, box has {torch.cuda.device_count()}")
-    r = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node=2",
-                        "--master-addr", "127.0.0.1", "--master-port", "29817",
-                        os.path.join(HERE, "kirchhoff_worker.py")], capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, (r.stdout[-4000:] + r.stderr[-8000:])
-    assert r.stdout.count("KIRCHHOFF_WORKER_OK") == 2
+@pytest.mark.parametrize("nproc", [1, 2])
+def test_multi_rank_fixtures(nproc):
+    needs_gpus(nproc)
+    run_on_ranks("test_kirchhoff", nproc)
+
+
+def on_ranks(pm, comm):
+    """each rank's MPIVStack([Kirchhoff]) against its slice of the gathered fixtures, and the LSM flow against its
+    fixture"""
+    rank, P = comm.Get_rank(), comm.Get_size()
+
+    def close(name, got, ref, atol_rel):
+        np.testing.assert_allclose(got, ref, rtol=0, atol=atol_rel * np.abs(ref).max(), err_msg=f"[rank {rank}] {name}")
+
+    n = mgk.OP_NS * mgk.OP_NR * mgk.OP_NT
+    ls = [(n,)] * P
+    for wav in mgk.WAVELETS:
+        h, off = mgk.wavelet(wav)
+        z, x, t, srcs, recs, vel = mgk.op_geometry(P, rank)
+        Op = pm.MPIVStack([pm.local.Kirchhoff(z, x, t, srcs, recs, vel, h, off, mode="analytic")])
+        m, d = mgk.op_inputs(P)
+        y = Op @ pm.DistributedArray.to_dist(m, partition=pm.Partition.BROADCAST)
+        ya = Op.H @ pm.DistributedArray.to_dist(d, local_shapes=ls)
+        k = mgk.key(P, wav)
+        close(f"{k}/y", host(y.local_array), GOLD[f"{k}/y"][rank * n:(rank + 1) * n], 1e-12)
+        close(f"{k}/ya", host(ya.local_array), GOLD[f"{k}/ya"], 1e-12)
+
+    z, x, t, srcs, recs, v0, wav, wavc, refl = mgk.flow_setup(P, rank)
+    lsm = pm.local.LSM(z, x, t, srcs, recs, v0, wav, wavc, mode="analytic", engine="numba")
+    VStack = pm.MPIVStack(ops=[lsm.Demop, ])
+    refl_dist = pm.DistributedArray(global_shape=refl.size, partition=pm.Partition.BROADCAST)
+    refl_dist[:] = refl.flatten()
+    d_dist = VStack @ refl_dist
+    madj = VStack.H @ d_dist
+    x0 = pm.DistributedArray(VStack.shape[1], partition=pm.Partition.BROADCAST)
+    x0[:] = 0
+    minv, _, iiter, _, _, cost = pm.cgls(VStack, d_dist, x0=x0, niter=mgk.FLOW_NITER)
+    g = f"flow/P{P}"
+    close(f"{g}/madj", host(madj.local_array), GOLD[f"{g}/madj"], 1e-12)
+    assert int(iiter) == int(GOLD[f"{g}/iiter"])
+    np.testing.assert_allclose(np.asarray(cost), GOLD[f"{g}/cost"], rtol=FLOW_COST_RTOL, err_msg=f"[rank {rank}] cost")
+    close(f"{g}/minv", host(minv.local_array), GOLD[f"{g}/minv"], FLOW_MINV_ATOL)

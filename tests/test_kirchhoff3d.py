@@ -8,7 +8,6 @@ b2_kirchhoff_chunk through the C ABI (bit for bit against NumPy and against one 
 chunked operators through the public interface."""
 import math
 import os
-import subprocess
 import sys
 
 import numpy as np
@@ -18,6 +17,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "golden"))
 import make_golden_kirchhoff as mgk  # noqa: E402
 import make_golden_kirchhoff3d as m3  # noqa: E402
+from op_checks import assert_cgls_replay_matches_steps, host, needs_gpus, run_on_ranks  # noqa: E402
 
 GOLD = np.load(os.path.join(HERE, "golden", "kirchhoff3d_golden.npz"), allow_pickle=False)
 KREF, _ = mgk.refshim()
@@ -174,10 +174,6 @@ def test_kirchhoff3d_flow_fixture_madj_follows_the_restatement(P):
 def pm():
     import pylops_mpi_b200 as pm
     return pm
-
-
-def host(t):
-    return t.cpu().numpy()
 
 
 def dev(a):
@@ -518,26 +514,12 @@ def test_chunked_apply_allocates_nothing(pm, chunk_budget):
 
 @pytest.mark.gpu
 def test_cgls_graph_replay_matches_step_loop_chunked(pm, chunk_budget):
-    from pylops_mpi_b200.optimization.cls_basic import CGLS, _graph_safe
     chunk_budget(m3.OP_NS + m3.OP_NR, 64)
     Op = op_vstack(pm, 2, "ricker21")
-    assert all(op.chunked for op in Op.ops) and _graph_safe(Op)
+    assert all(op.chunked for op in Op.ops)
     rng = np.random.default_rng(12)
     y = Op @ bcast(pm, rng.standard_normal(Op.shape[1]))
-    x0 = np.zeros(Op.shape[1])
-    a = CGLS(Op)
-    xa = a.setup(y=y, x0=bcast(pm, x0), niter=25, damp=0.0, tol=0.0)
-    xa = a.run(xa, 25)
-    a.finalize()
-    assert a.graph_error is None, a.graph_error
-    assert a.graph_replays >= 20
-    b = CGLS(Op)
-    xb = b.setup(y=y, x0=bcast(pm, x0), niter=25, damp=0.0, tol=0.0)
-    for _ in range(25):
-        xb = b.step(xb)
-    b.finalize()
-    np.testing.assert_array_equal(host(xa.asarray()), host(xb.asarray()))
-    np.testing.assert_array_equal(np.asarray(a.cost), np.asarray(b.cost))
+    assert_cgls_replay_matches_steps(pm, Op, y, bcast(pm, np.zeros(Op.shape[1])), 25, 20)
 
 
 def run_flow(pm, P):
@@ -592,12 +574,53 @@ def test_operator_y_geometry_errors(pm):
 
 
 @pytest.mark.gpu
-def test_multi_rank_fixtures3d_p2():
-    import torch
-    if torch.cuda.device_count() < 2:
-        pytest.skip(f"needs 2 GPUs, box has {torch.cuda.device_count()}")
-    r = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node=2",
-                        "--master-addr", "127.0.0.1", "--master-port", "29827",
-                        os.path.join(HERE, "kirchhoff3d_worker.py")], capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, (r.stdout[-4000:] + r.stderr[-8000:])
-    assert r.stdout.count("KIRCHHOFF3D_WORKER_OK") == 2
+@pytest.mark.parametrize("nproc", [1, 2])
+def test_multi_rank_fixtures3d(nproc):
+    needs_gpus(nproc)
+    run_on_ranks("test_kirchhoff3d", nproc)
+
+
+def on_ranks(pm, comm):
+    """each rank's MPIVStack([3-D Kirchhoff]) against its slice of the gathered fixtures, resident and in chunks,
+    and the 3-D LSM flow against its fixture"""
+    rank, P = comm.Get_rank(), comm.Get_size()
+    BUDGET = pm.local.KIRCHHOFF_TABLE_BYTES
+
+    def close(name, got, ref, atol_rel):
+        np.testing.assert_allclose(got, ref, rtol=0, atol=atol_rel * np.abs(ref).max(), err_msg=f"[rank {rank}] {name}")
+
+    n = m3.OP_NS * m3.OP_NR * m3.OP_NT
+    ls = [(n,)] * P
+    try:
+        for budget in (BUDGET, (m3.OP_NS + m3.OP_NR) * 8 * 64):          # resident, then chunks of 64 image points
+            pm.local.KIRCHHOFF_TABLE_BYTES = budget
+            for wav in mgk.WAVELETS:
+                h, off = mgk.wavelet(wav)
+                z, x, t, srcs, recs, vel, y = m3.op_geometry(P, rank)
+                K = pm.local.Kirchhoff(z, x, t, srcs, recs, vel, h, off, y=y, mode="analytic")
+                assert K.chunked == (budget != BUDGET)
+                Op = pm.MPIVStack([K])
+                m, d = m3.op_inputs(P)
+                yf = Op @ pm.DistributedArray.to_dist(m, partition=pm.Partition.BROADCAST)
+                ya = Op.H @ pm.DistributedArray.to_dist(d, local_shapes=ls)
+                k = mgk.key(P, wav)
+                close(f"{k}/y", host(yf.local_array), GOLD[f"{k}/y"][rank * n:(rank + 1) * n], 1e-12)
+                close(f"{k}/ya", host(ya.local_array), GOLD[f"{k}/ya"], 1e-12)
+    finally:
+        pm.local.KIRCHHOFF_TABLE_BYTES = BUDGET
+
+    z, x, t, srcs, recs, v0, wav, wavc, refl, y = m3.flow_setup(P, rank)
+    lsm = pm.local.LSM(z, x, t, srcs, recs, v0, wav, wavc, y=y, mode="analytic")
+    VStack = pm.MPIVStack(ops=[lsm.Demop, ])
+    refl_dist = pm.DistributedArray(global_shape=refl.size, partition=pm.Partition.BROADCAST)
+    refl_dist[:] = refl.flatten()
+    d_dist = VStack @ refl_dist
+    madj = VStack.H @ d_dist
+    x0 = pm.DistributedArray(VStack.shape[1], partition=pm.Partition.BROADCAST)
+    x0[:] = 0
+    minv, _, iiter, _, _, cost = pm.cgls(VStack, d_dist, x0=x0, niter=m3.FLOW_NITER)
+    g = f"flow/P{P}"
+    close(f"{g}/madj", host(madj.local_array), GOLD[f"{g}/madj"], 1e-12)
+    assert int(iiter) == int(GOLD[f"{g}/iiter"])
+    np.testing.assert_allclose(np.asarray(cost), GOLD[f"{g}/cost"], rtol=FLOW_COST_RTOL, err_msg=f"[rank {rank}] cost")
+    close(f"{g}/minv", host(minv.local_array), GOLD[f"{g}/minv"], FLOW_MINV_ATOL)

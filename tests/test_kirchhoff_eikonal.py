@@ -18,6 +18,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "golden"))
 import make_golden_kirchhoff as mgk  # noqa: E402
 import make_golden_kirchhoff_eikonal as mge  # noqa: E402
+from op_checks import assert_cgls_replay_matches_steps, host  # noqa: E402
 
 GOLD = np.load(os.path.join(HERE, "golden", "kirchhoff_eikonal_golden.npz"), allow_pickle=False)
 KE, EK = mge.refshim_eikonal()
@@ -201,10 +202,6 @@ def test_fixtures_follow_the_restatement(tag, wav):
 def pm():
     import pylops_mpi_b200 as pm
     return pm
-
-
-def host(t):
-    return t.cpu().numpy()
 
 
 def dev(a):
@@ -424,29 +421,14 @@ def test_byot_round_trip_bitwise(pm, tag):
 
 @pytest.mark.gpu
 def test_lsm_pass_through_and_graph_replay(pm):
-    from pylops_mpi_b200.optimization.cls_basic import CGLS, _graph_safe
     z, x, t, srcs, recs, vel = mge.op_geometry(2)
     h, off = mgk.wavelet("ricker21")
     lsm = pm.local.LSM(z, x, t, srcs, recs, vel, h, off, mode="eikonal", dtype="float32")
     assert lsm.Demop.mode == "eikonal" and lsm.Demop.dtype == np.float32
     Op = op_vstack(pm, "op", 2, "ricker21")
-    assert _graph_safe(Op)
     rng = np.random.default_rng(12)
     yv = Op @ bcast(pm, rng.standard_normal(Op.shape[1]))
-    x0 = np.zeros(Op.shape[1])
-    a = CGLS(Op)
-    xa = a.setup(y=yv, x0=bcast(pm, x0), niter=25, damp=0.0, tol=0.0)
-    xa = a.run(xa, 25)
-    a.finalize()
-    assert a.graph_error is None, a.graph_error
-    assert a.graph_replays >= 20
-    b = CGLS(Op)
-    xb = b.setup(y=yv, x0=bcast(pm, x0), niter=25, damp=0.0, tol=0.0)
-    for _ in range(25):
-        xb = b.step(xb)
-    b.finalize()
-    np.testing.assert_array_equal(host(xa.asarray()), host(xb.asarray()))
-    np.testing.assert_array_equal(np.asarray(a.cost), np.asarray(b.cost))
+    assert_cgls_replay_matches_steps(pm, Op, yv, bcast(pm, np.zeros(Op.shape[1])), 25, 20)
 
 
 @pytest.mark.gpu

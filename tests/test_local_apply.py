@@ -1,6 +1,6 @@
 """The shared apply of the rank-local kernel operators (``local._KernelOperator``): the result dtype for every data
-dtype, ``out=`` in every form against ``out=None`` bit for bit, length errors, no allocation on the direct path, and
-CUDA-graph safety by type."""
+dtype, ``out=`` in every form against ``out=None`` bit for bit, complex data equal to its real and imaginary parts,
+length errors, no allocation on the direct path, and CUDA-graph safety by type."""
 import numpy as np
 import pytest
 import torch
@@ -19,8 +19,21 @@ RESULT = {
     "Convolve1D": (F32, F32, C64, C128),                # float32
     "PoststackLinearModelling": (F64, F64, C128, C128),  # float64 wavelet
     "Kirchhoff": (F32, F64, C64, C128),                 # float32; float64 data run in float64; complex part by part
+    "NonStationaryConvolve1D": (F32, F32, C64, C128),   # float32 real taps; complex data: one launch, promoted
+    "NonStationaryConvolve2D": (F32, F32, C64, C128),   # float32
+    "NonStationaryConvolve2D-float64": (F64, F64, C128, C128),
+    "NonStationaryConvolve3D": (F32, F32, C64, C128),   # float32
+    "NonStationaryConvolve3D-float64": (F64, F64, C128, C128),
+    "NonStationaryFilters1D": (F64, F64, C128, C128),   # float64; complex data part by part
+    "NonStationaryFilters2D": (F32, F32, C64, C128),    # float32
+    "NonStationaryFilters2D-float64": (F64, F64, C128, C128),
+    "Radon2D": (F64, F64, C128, C128),                  # float64 real taps
+    "Radon3D": (F32, F32, C64, C128),                   # float32
 }
-SQUARE = ("MatrixMult", "FirstDerivative", "SecondDerivative", "Convolve1D", "PoststackLinearModelling")
+SQUARE = ("MatrixMult", "FirstDerivative", "SecondDerivative", "Convolve1D", "PoststackLinearModelling",
+          "NonStationaryConvolve1D", "NonStationaryConvolve2D", "NonStationaryConvolve2D-float64",
+          "NonStationaryConvolve3D", "NonStationaryConvolve3D-float64")
+REAL_OF = {C64: F32, C128: F64}
 
 
 @pytest.fixture(scope="module")
@@ -49,6 +62,25 @@ def make(pm, name):
         recs = np.array([[10.0, 30.0, 40.0], [0.0, 0.0, 0.0]])
         return L.Kirchhoff(np.arange(4) * 10.0, np.arange(5) * 10.0, np.arange(32) * 0.004, srcs, recs, 1000.0,
                            np.array([1.0, -2.0, 4.0, -1.0, 0.5]), 2, mode="analytic", dtype="float32")
+    name, _, dt = name.partition("-")
+    dt = dt or "float32"
+    if name == "NonStationaryConvolve1D":
+        return L.NonStationaryConvolve1D((9, 4), rng.standard_normal((3, 5)), [1, 4, 7], axis=0, dtype=dt)
+    if name == "NonStationaryConvolve2D":
+        return L.NonStationaryConvolve2D((6, 5), rng.standard_normal((2, 2, 3, 3)), [1, 4], [1, 3], dtype=dt)
+    if name == "NonStationaryConvolve3D":
+        return L.NonStationaryConvolve3D((5, 4, 6), rng.standard_normal((2, 2, 2, 3, 3, 3)), [1, 3], [1, 2], [1, 4],
+                                         dtype=dt)
+    if name == "NonStationaryFilters1D":
+        return L.NonStationaryFilters1D(rng.standard_normal(12), 5, [3, 8], dtype="float64")
+    if name == "NonStationaryFilters2D":
+        return L.NonStationaryFilters2D(rng.standard_normal((10, 9)), (3, 5), [2, 6], [1, 4], dtype=dt)
+    t = np.arange(16) * 0.004
+    if name == "Radon2D":
+        return L.Radon2D(t, np.arange(5) * 10.0, np.linspace(-1e-3, 1e-3, 4), dtype="float64")
+    if name == "Radon3D":
+        return L.Radon3D(t, np.arange(3) * 20.0, np.arange(4) * 10.0, np.linspace(-1e-3, 1e-3, 2),
+                         np.linspace(-2e-3, 2e-3, 3), dtype="float32")
     raise KeyError(name)
 
 
@@ -112,6 +144,28 @@ def test_out_aliasing_x(pm, name, adjoint, kind):
     ref = f(x.clone())
     assert ref.dtype == x.dtype
     assert f(x, out=x) is x and torch.equal(x, ref)
+
+
+@pytest.mark.parametrize("adjoint", [False, True])
+@pytest.mark.parametrize("name", list(RESULT))
+def test_complex_data_equals_its_parts(pm, name, adjoint):
+    """complex data: torch.complex(f(re), f(im)) bit for bit, re and im the parts the apply computes on: the parts
+    themselves when it applies them one after the other, the parts in the real dtype of its launch on (re, im) pairs
+    otherwise -- except where no real apply computes in that dtype (complex128 data of a float32 operator with real
+    taps, computed in float64)"""
+    op = make(pm, name)
+    f = op.rmatvec if adjoint else op.matvec
+    compared = 0
+    for xdt in (C64, C128):
+        x = data(sizes(op, adjoint)[0], xdt)
+        ref = f(x)
+        cdt = op._compute_dtype(xdt)
+        pdt = REAL_OF[cdt] if cdt.is_complex else REAL_OF[xdt]
+        re, im = f(x.real.to(pdt)), f(x.imag.to(pdt))
+        if not cdt.is_complex or re.dtype == pdt:
+            assert torch.equal(ref, torch.complex(re, im).to(ref.dtype)), xdt
+            compared += 1
+    assert compared or name == "MatrixMult-complex"
 
 
 @pytest.mark.parametrize("name", list(RESULT))

@@ -9,7 +9,6 @@ the fixtures of tests/golden/nsconvolve2d_golden.npz (made by make_golden_nsconv
 MPIBlockDiag and cgls over the restatement; operator inputs exactly representable, so every dtype must match them
 bit for bit).  GPU: b2_nsconvolve2d through the C ABI, and the operator through the public interface."""
 import os
-import subprocess
 import sys
 
 import numpy as np
@@ -19,6 +18,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "golden"))
 import make_golden_nsconvolve2d as mg2  # noqa: E402
 from ns_reference import axis_weights, c_ns, check_close, ns_matrix, point_weights, run_kernel  # noqa: E402
+from fixture_codec import decode, rows_of  # noqa: E402
+from op_checks import assert_cgls_replay_matches_steps, assert_rejected, host, needs_gpus, run_on_ranks  # noqa: E402
 
 GOLD = np.load(os.path.join(HERE, "golden", "nsconvolve2d_golden.npz"), allow_pickle=False)
 
@@ -128,12 +129,12 @@ def test_fixtures_follow_the_restatement_in_every_dtype(case):
     ops = [NS2((mg2.NX, mg2.NZ), hs[k], ihx, ihz, dtype=dt) for k in range(mg2.NY)]
     y = np.concatenate([op.matvec(s) for op, s in zip(ops, slices(x))])
     ya = np.concatenate([op.rmatvec(s) for op, s in zip(ops, slices(v))])
-    gy, gya = mg2.decode(GOLD, mg2.key(nh, bank), dt)
+    gy, gya = decode(GOLD, mg2.key(nh, bank), dt, mg2.ENC)
     assert y.dtype == np.dtype(dt) and gy.dtype == np.dtype(dt)
     np.testing.assert_array_equal(y, gy)
     np.testing.assert_array_equal(ya, gya)
     if dt != "complex128":          # the other real dtype gives the same values (the generator checks all three)
-        other = mg2.decode(GOLD, mg2.key(nh, bank), "float32" if dt == "float64" else "float64")
+        other = decode(GOLD, mg2.key(nh, bank), "float32" if dt == "float64" else "float64", mg2.ENC)
         np.testing.assert_array_equal(gy.astype(np.float64), other[0].astype(np.float64))
 
 
@@ -154,10 +155,6 @@ def test_flow_psfs_follow_the_restated_kirchhoff():
 def pm():
     import pylops_mpi_b200 as pm
     return pm
-
-
-def host(t):
-    return t.cpu().numpy()
 
 
 SHAPES = [(1, 1), (1, 37), (29, 1), (5, 7), (33, 65), (70, 130)]
@@ -215,17 +212,10 @@ def test_kernel_error_codes_leave_y_untouched(pm):
         (dict(dh=(0, 1)), ARG), (dict(dh=(1, -2)), ARG),
         (dict(dtype=L.C64), DT), (dict(dtype=L.C128), DT), (dict(dtype=L.BF16), DT), (dict(dtype=99), DT),
     ]
-    for kw, want in cases:
-        a = dict(x=x.data_ptr(), y=y.data_ptr(), hs=hs.data_ptr(), nx=4, nz=3, ni=2, nf=(2, 2), nh=(3, 3), dh=(2, 1),
-                 dtype=L.F64)
-        a.update(kw)
-        if a["y"] == "x":
-            a["y"] = a["x"]
-        rc = c_ns(pm, a["x"], a["y"], (a["nx"], a["nz"]), a["ni"], a["hs"], a["nf"], a["nh"], (0, 0), a["dh"], 0,
-                  a["dtype"])
-        assert rc == want, (kw, rc)
-    torch.cuda.synchronize()
-    assert torch.all(y == 3.5)
+    assert_rejected(lambda a: c_ns(pm, a["x"], a["y"], (a["nx"], a["nz"]), a["ni"], a["hs"], a["nf"], a["nh"], (0, 0),
+                                   a["dh"], 0, a["dtype"]),
+                    dict(x=x.data_ptr(), y=y.data_ptr(), hs=hs.data_ptr(), nx=4, nz=3, ni=2, nf=(2, 2), nh=(3, 3),
+                         dh=(2, 1), dtype=L.F64), cases, y)
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -246,7 +236,7 @@ def test_operator_vs_reference_fixtures(pm, case):
     got = host((Op @ pm.DistributedArray.to_dist(x)).asarray())
     gota = host((Op.H @ pm.DistributedArray.to_dist(v)).asarray())
     assert got.dtype == np.dtype(dt) and gota.dtype == np.dtype(dt)
-    gy, gya = mg2.decode(GOLD, mg2.key(nh, bank), dt)
+    gy, gya = decode(GOLD, mg2.key(nh, bank), dt, mg2.ENC)
     np.testing.assert_array_equal(got, gy)
     np.testing.assert_array_equal(gota, gya)
 
@@ -277,34 +267,6 @@ def test_operator_attributes_dtypes_and_out(pm):
     assert Op.dims == (20, 9) and Op.shape == (180, 180) and Op.dtype == np.float32
     assert (Op.nfilt, Op.nh, Op.hc, Op.oh, Op.dh) == ((3, 2), (5, 7), (2, 3), (2, 1), (4, 3))
     assert pm.local.NonStationaryConvolve2D((20, 9), hs[:1, :1], [7], [0]).dh == (1, 1)
-    F32, F64, C64, C128 = torch.float32, torch.float64, torch.complex64, torch.complex128
-    op64 = pm.local.NonStationaryConvolve2D((20, 9), hs, [2, 6, 10], [1, 4])
-    for op, results in ((Op, (F32, F32, C64, C128)), (op64, (F64, F64, C128, C128))):
-        for adjoint in (False, True):
-            f = op.rmatvec if adjoint else op.matvec
-            for xdt, want in zip((F32, F64, C64, C128), results):
-                x = torch.as_tensor(rng.standard_normal(180)).to(xdt).cuda()
-                if xdt.is_complex:
-                    x = x + 1j * torch.as_tensor(rng.standard_normal(180)).to(xdt).cuda()
-                ref = f(x)
-                assert ref.dtype == want
-                out = torch.full((180,), 7.0, dtype=ref.dtype, device="cuda")
-                assert f(x, out=out) is out and torch.equal(out, ref)
-                out = torch.full((180,), 7.0, dtype=C128 if ref.dtype.is_complex else F64, device="cuda")
-                f(x, out=out)
-                assert torch.equal(out, ref.to(out.dtype))
-                buf = torch.full((180, 2), 7.0, dtype=ref.dtype, device="cuda")
-                f(x, out=buf[:, 0])
-                assert torch.equal(buf[:, 0], ref) and bool((buf[:, 1] == 7.0).all())
-                if xdt == want:
-                    xc = x.clone()
-                    assert f(xc, out=xc) is xc and torch.equal(xc, ref)
-                re = f(x.real.contiguous().to(_real(want)))
-                if ref.dtype.is_complex and re.dtype == _real(want):   # the parts computed in the same dtype:
-                    im = f(x.imag.contiguous().to(_real(want)))       # one launch on (re, im) pairs, the same bits
-                    assert torch.equal(ref, torch.complex(re, im))
-                with pytest.raises(ValueError, match="dimension mismatch"):
-                    f(x[:-1])
     # float32 data of a float64-bank float32 operator: the bank rounded to float32
     M = ns_matrix(hs.astype(np.float32), (20, 9), (2, 1), (4, 3))
     x = rng.standard_normal(180).astype(np.float32)
@@ -312,36 +274,16 @@ def test_operator_attributes_dtypes_and_out(pm):
     np.testing.assert_allclose(y, M @ x, rtol=0, atol=1e-4 * np.abs(M).sum(1).max())
 
 
-def _real(dt):
-    import torch
-    return {torch.complex64: torch.float32, torch.complex128: torch.float64}.get(dt, dt)
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("dt", ["float32", "float64"])
 def test_cgls_graph_replay_matches_step_loop(pm, dt):
-    from pylops_mpi_b200.optimization.cls_basic import CGLS, _graph_safe
     rng = np.random.default_rng(12)
     hs = rng.standard_normal((4, 3, 9, 7)).astype(dt)
     Op = pm.MPIBlockDiag([pm.local.NonStationaryConvolve2D((40, 30), hs, [3, 13, 23, 33], [2, 12, 22], dtype=dt)
                           for _ in range(2)])
-    assert _graph_safe(Op)
     n = Op.shape[0]
     y = Op @ pm.DistributedArray.to_dist(rng.standard_normal(n).astype(dt))
-    x0 = np.zeros(n, dtype=dt)
-    a = CGLS(Op)
-    xa = a.setup(y=y, x0=pm.DistributedArray.to_dist(x0), niter=25, damp=0.0, tol=0.0)
-    xa = a.run(xa, 25)
-    a.finalize()
-    assert a.graph_error is None, a.graph_error
-    assert a.graph_replays >= 20
-    b = CGLS(Op)
-    xb = b.setup(y=y, x0=pm.DistributedArray.to_dist(x0), niter=25, damp=0.0, tol=0.0)
-    for _ in range(25):
-        xb = b.step(xb)
-    b.finalize()
-    np.testing.assert_array_equal(host(xa.asarray()), host(xb.asarray()))
-    np.testing.assert_array_equal(np.asarray(a.cost), np.asarray(b.cost))
+    assert_cgls_replay_matches_steps(pm, Op, y, pm.DistributedArray.to_dist(np.zeros(n, dtype=dt)), 25, 20)
 
 
 @pytest.mark.gpu
@@ -365,7 +307,7 @@ def test_image_domain_lsm_flow_vs_reference(pm, P):
     blocks of P ranks' rows as one rank's blocks.  The PSF operator's condition number is about 2e6, so 20 iterations
     summed in another order than pylops' may move x by about cond * 2^-53 ~ 2e-10 of max |x|"""
     ops = [pm.local.NonStationaryConvolve2D((mg2.FLOW_NX, mg2.FLOW_NZ), GOLD["flow/hs"], mg2.FLOW_IHX, mg2.FLOW_IHZ)
-           for ny in mg2.rows_of(P, mg2.FLOW_NY) for _ in range(ny)]
+           for ny in rows_of(P, mg2.FLOW_NY) for _ in range(ny)]
     Op = pm.MPIBlockDiag(ops)
     d = pm.DistributedArray.to_dist(GOLD["flow/mmig"])
     x0 = pm.DistributedArray.to_dist(np.zeros_like(GOLD["flow/mmig"]))
@@ -377,12 +319,43 @@ def test_image_domain_lsm_flow_vs_reference(pm, P):
 
 
 @pytest.mark.gpu
-def test_multi_rank_fixtures_p2():
-    import torch
-    if torch.cuda.device_count() < 2:
-        pytest.skip(f"needs 2 GPUs, box has {torch.cuda.device_count()}")
-    r = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node=2",
-                        "--master-addr", "127.0.0.1", "--master-port", "29833",
-                        os.path.join(HERE, "nsconvolve2d_worker.py")], capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, (r.stdout[-4000:] + r.stderr[-8000:])
-    assert r.stdout.count("NSCONVOLVE2D_WORKER_OK") == 2
+@pytest.mark.parametrize("nproc", [1, 2])
+def test_multi_rank_fixtures(nproc):
+    needs_gpus(nproc)
+    run_on_ranks("test_nsconvolve2d", nproc)
+
+
+def on_ranks(pm, comm):
+    """each rank's MPIBlockDiag block of NonStationaryConvolve2D against its slice of the gathered fixtures, and
+    the image-domain cgls flow against its fixture"""
+    rank, P = comm.Get_rank(), comm.Get_size()
+    def block(ny_global, plane):
+        """this rank's slices of a (ny_global, ...) stack: (local_shapes, flat slice, first slice, slice count)"""
+        rows = rows_of(P, ny_global)
+        k0 = sum(rows[:rank])
+        return [(r * plane,) for r in rows], slice(k0 * plane, (k0 + rows[rank]) * plane), k0, rows[rank]
+
+    ls, sl, k0, ny = block(mg2.NY, mg2.NX * mg2.NZ)
+    for nh, bank, dt in mg2.cases():
+        hs, ihx, ihz, x, v = mg2.case_inputs(nh, bank, dt)
+        Op = pm.MPIBlockDiag([pm.local.NonStationaryConvolve2D((mg2.NX, mg2.NZ), hs[k], ihx, ihz, dtype=hs.dtype)
+                              for k in range(k0, k0 + ny)], dtype=dt)
+        gy, gya = decode(GOLD, mg2.key(nh, bank), dt, mg2.ENC)
+        name = f"{mg2.key(nh, bank)}/{dt}"
+        np.testing.assert_array_equal(host((Op @ pm.DistributedArray.to_dist(x, local_shapes=ls)).local_array), gy[sl],
+                                      err_msg=f"[rank {rank}] {name}/y")
+        np.testing.assert_array_equal(host((Op.H @ pm.DistributedArray.to_dist(v, local_shapes=ls)).local_array),
+                                      gya[sl], err_msg=f"[rank {rank}] {name}/ya")
+
+    ls, sl, k0, ny = block(mg2.FLOW_NY, mg2.FLOW_NX * mg2.FLOW_NZ)
+    Op = pm.MPIBlockDiag([pm.local.NonStationaryConvolve2D((mg2.FLOW_NX, mg2.FLOW_NZ), GOLD["flow/hs"], mg2.FLOW_IHX,
+                                                           mg2.FLOW_IHZ)] * ny)
+    mmig = GOLD["flow/mmig"]
+    d = pm.DistributedArray.to_dist(mmig, local_shapes=ls)
+    x0 = pm.DistributedArray.to_dist(np.zeros_like(mmig), local_shapes=ls)
+    x, _, iiter, _, _, cost = pm.cgls(Op, d, x0=x0, niter=mg2.FLOW_NITER, tol=0.0)
+    assert iiter == int(GOLD[f"flow/P{P}/iiter"])
+    np.testing.assert_allclose(np.asarray(cost), GOLD[f"flow/P{P}/cost"], rtol=1e-10, err_msg=f"[rank {rank}] cost")
+    gx = GOLD[f"flow/P{P}/x"]
+    np.testing.assert_allclose(host(x.local_array), gx[sl], rtol=1e-9, atol=1e-10 * np.abs(gx).max(),
+                               err_msg=f"[rank {rank}] x")

@@ -9,7 +9,6 @@ the fixtures of tests/golden/nsconvolve3d_golden.npz (made by make_golden_nsconv
 MPIBlockDiag and cgls over the restatement; operator inputs exactly representable, so every dtype must match them
 bit for bit).  GPU: b2_nsconvolve3d through the C ABI, and the operator through the public interface."""
 import os
-import subprocess
 import sys
 
 import numpy as np
@@ -19,6 +18,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "golden"))
 import make_golden_nsconvolve3d as mg3  # noqa: E402
 from ns_reference import axis_weights, c_ns, check_close, ns_matrix, point_weights, reference, run_kernel  # noqa: E402
+from fixture_codec import decode, rows_of  # noqa: E402
+from op_checks import assert_cgls_replay_matches_steps, assert_rejected, host, needs_gpus, run_on_ranks  # noqa: E402
 
 GOLD = np.load(os.path.join(HERE, "golden", "nsconvolve3d_golden.npz"), allow_pickle=False)
 
@@ -133,7 +134,7 @@ def test_fixtures_follow_the_restatement_in_every_dtype(case):
     ops = [NS3((mg3.NX, mg3.NY, mg3.NZ), hs[k], *ih, dtype=dt) for k in range(mg3.NV)]
     y = np.concatenate([op.matvec(s) for op, s in zip(ops, volumes(x))])
     ya = np.concatenate([op.rmatvec(s) for op, s in zip(ops, volumes(v))])
-    gy, gya = mg3.decode(GOLD, mg3.key(nh, bank), dt)
+    gy, gya = decode(GOLD, mg3.key(nh, bank), dt, mg3.ENC)
     assert y.dtype == np.dtype(dt) and gy.dtype == np.dtype(dt)
     np.testing.assert_array_equal(y, gy)
     np.testing.assert_array_equal(ya, gya)
@@ -157,10 +158,6 @@ def test_flow_psfs_follow_the_restated_kirchhoff():
 def pm():
     import pylops_mpi_b200 as pm
     return pm
-
-
-def host(t):
-    return t.cpu().numpy()
 
 
 # singleton axes, tiles that are not full along every axis (x tiles of 4 / 2 / 1 planes, y of 32, z of 64)
@@ -254,17 +251,10 @@ def test_kernel_error_codes_leave_y_untouched(pm):
         (dict(dims=(4, 3, 2 ** 29)), ARG), (dict(dh=(2 ** 29, 1, 1)), ARG),     # past the kernel's 32-bit axes
         (dict(dtype=L.C64), DT), (dict(dtype=L.C128), DT), (dict(dtype=L.BF16), DT), (dict(dtype=99), DT),
     ]
-    for kw, want in cases:
-        a = dict(x=x.data_ptr(), y=y.data_ptr(), hs=hs.data_ptr(), dims=(4, 3, 2), ni=2, nf=(2, 2, 2), nh=(3, 3, 3),
-                 dh=(2, 1, 1), dtype=L.F64)
-        a.update(kw)
-        if a["y"] == "x":
-            a["y"] = a["x"]
-        rc = c_ns(pm, a["x"], a["y"], a["dims"], a["ni"], a["hs"], a["nf"], a["nh"], (0, 0, 0), a["dh"], 0,
-                  a["dtype"])
-        assert rc == want, (kw, rc)
-    torch.cuda.synchronize()
-    assert torch.all(y == 3.5)
+    assert_rejected(lambda a: c_ns(pm, a["x"], a["y"], a["dims"], a["ni"], a["hs"], a["nf"], a["nh"], (0, 0, 0), a["dh"],
+                                   0, a["dtype"]),
+                    dict(x=x.data_ptr(), y=y.data_ptr(), hs=hs.data_ptr(), dims=(4, 3, 2), ni=2, nf=(2, 2, 2),
+                         nh=(3, 3, 3), dh=(2, 1, 1), dtype=L.F64), cases, y)
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -285,7 +275,7 @@ def test_operator_vs_reference_fixtures(pm, case):
     got = host((Op @ pm.DistributedArray.to_dist(x)).asarray())
     gota = host((Op.H @ pm.DistributedArray.to_dist(v)).asarray())
     assert got.dtype == np.dtype(dt) and gota.dtype == np.dtype(dt)
-    gy, gya = mg3.decode(GOLD, mg3.key(nh, bank), dt)
+    gy, gya = decode(GOLD, mg3.key(nh, bank), dt, mg3.ENC)
     np.testing.assert_array_equal(got, gy)
     np.testing.assert_array_equal(gota, gya)
 
@@ -306,11 +296,6 @@ def test_operator_dottest(pm, dt):
                    rtol=1e-5 if dt == "float32" else 1e-12)
 
 
-def _real(dt):
-    import torch
-    return {torch.complex64: torch.float32, torch.complex128: torch.float64}.get(dt, dt)
-
-
 @pytest.mark.gpu
 def test_operator_attributes_dtypes_and_out(pm):
     import torch
@@ -322,34 +307,6 @@ def test_operator_attributes_dtypes_and_out(pm):
     assert Op.dims == Op.dimsd == dims and Op.shape == (N, N) and Op.dtype == np.float32
     assert (Op.nfilt, Op.nh, Op.hc, Op.oh, Op.dh) == ((3, 2, 2), (5, 3, 7), (2, 1, 3), (2, 1, 0), (4, 3, 5))
     assert pm.local.NonStationaryConvolve3D(dims, hs[:1, :1, :1], [7], [0], [3]).dh == (1, 1, 1)
-    F32, F64, C64, C128 = torch.float32, torch.float64, torch.complex64, torch.complex128
-    op64 = pm.local.NonStationaryConvolve3D(dims, hs, [2, 6, 10], [1, 4], [0, 5])
-    for op, results in ((Op, (F32, F32, C64, C128)), (op64, (F64, F64, C128, C128))):
-        for adjoint in (False, True):
-            f = op.rmatvec if adjoint else op.matvec
-            for xdt, want in zip((F32, F64, C64, C128), results):
-                x = torch.as_tensor(rng.standard_normal(N)).to(xdt).cuda()
-                if xdt.is_complex:
-                    x = x + 1j * torch.as_tensor(rng.standard_normal(N)).to(xdt).cuda()
-                ref = f(x)
-                assert ref.dtype == want
-                out = torch.full((N,), 7.0, dtype=ref.dtype, device="cuda")
-                assert f(x, out=out) is out and torch.equal(out, ref)
-                out = torch.full((N,), 7.0, dtype=C128 if ref.dtype.is_complex else F64, device="cuda")
-                f(x, out=out)
-                assert torch.equal(out, ref.to(out.dtype))
-                buf = torch.full((N, 2), 7.0, dtype=ref.dtype, device="cuda")
-                f(x, out=buf[:, 0])
-                assert torch.equal(buf[:, 0], ref) and bool((buf[:, 1] == 7.0).all())
-                if xdt == want:
-                    xc = x.clone()
-                    assert f(xc, out=xc) is xc and torch.equal(xc, ref)
-                re = f(x.real.contiguous().to(_real(want)))
-                if ref.dtype.is_complex and re.dtype == _real(want):   # the parts computed in the same dtype:
-                    im = f(x.imag.contiguous().to(_real(want)))       # one launch on (re, im) pairs, the same bits
-                    assert torch.equal(ref, torch.complex(re, im))
-                with pytest.raises(ValueError, match="dimension mismatch"):
-                    f(x[:-1])
     # float32 data of a float64-bank float32 operator: the bank rounded to float32
     M = ns_matrix(hs.astype(np.float32), dims, (2, 1, 0), (4, 3, 5))
     x = rng.standard_normal(N).astype(np.float32)
@@ -360,28 +317,13 @@ def test_operator_attributes_dtypes_and_out(pm):
 @pytest.mark.gpu
 @pytest.mark.parametrize("dt", ["float32", "float64"])
 def test_cgls_graph_replay_matches_step_loop(pm, dt):
-    from pylops_mpi_b200.optimization.cls_basic import CGLS, _graph_safe
     rng = np.random.default_rng(12)
     hs = rng.standard_normal((3, 2, 3, 5, 7, 3)).astype(dt)
     Op = pm.MPIBlockDiag([pm.local.NonStationaryConvolve3D((14, 20, 15), hs, [2, 7, 12], [3, 13], [1, 7, 13],
                                                            dtype=dt) for _ in range(2)])
-    assert _graph_safe(Op)
     n = Op.shape[0]
     y = Op @ pm.DistributedArray.to_dist(rng.standard_normal(n).astype(dt))
-    x0 = np.zeros(n, dtype=dt)
-    a = CGLS(Op)
-    xa = a.setup(y=y, x0=pm.DistributedArray.to_dist(x0), niter=25, damp=0.0, tol=0.0)
-    xa = a.run(xa, 25)
-    a.finalize()
-    assert a.graph_error is None, a.graph_error
-    assert a.graph_replays >= 20
-    b = CGLS(Op)
-    xb = b.setup(y=y, x0=pm.DistributedArray.to_dist(x0), niter=25, damp=0.0, tol=0.0)
-    for _ in range(25):
-        xb = b.step(xb)
-    b.finalize()
-    np.testing.assert_array_equal(host(xa.asarray()), host(xb.asarray()))
-    np.testing.assert_array_equal(np.asarray(a.cost), np.asarray(b.cost))
+    assert_cgls_replay_matches_steps(pm, Op, y, pm.DistributedArray.to_dist(np.zeros(n, dtype=dt)), 25, 20)
 
 
 @pytest.mark.gpu
@@ -416,7 +358,7 @@ def test_image_domain_lsm_flow_vs_reference(pm, P):
     blocks of P ranks' volumes as one rank's blocks"""
     ops = [pm.local.NonStationaryConvolve3D((mg3.FLOW_NY, mg3.FLOW_NX, mg3.FLOW_NZ), GOLD["flow/hs"], mg3.FLOW_IHY,
                                             mg3.FLOW_IHX, mg3.FLOW_IHZ)
-           for nv in mg3.rows_of(P, mg3.FLOW_NV) for _ in range(nv)]
+           for nv in rows_of(P, mg3.FLOW_NV) for _ in range(nv)]
     Op = pm.MPIBlockDiag(ops)
     d = pm.DistributedArray.to_dist(GOLD["flow/mmig"])
     x0 = pm.DistributedArray.to_dist(np.zeros_like(GOLD["flow/mmig"]))
@@ -429,12 +371,44 @@ def test_image_domain_lsm_flow_vs_reference(pm, P):
 
 
 @pytest.mark.gpu
-def test_multi_rank_fixtures_p2():
-    import torch
-    if torch.cuda.device_count() < 2:
-        pytest.skip(f"needs 2 GPUs, box has {torch.cuda.device_count()}")
-    r = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node=2",
-                        "--master-addr", "127.0.0.1", "--master-port", "29837",
-                        os.path.join(HERE, "nsconvolve3d_worker.py")], capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, (r.stdout[-4000:] + r.stderr[-8000:])
-    assert r.stdout.count("NSCONVOLVE3D_WORKER_OK") == 2
+@pytest.mark.parametrize("nproc", [1, 2])
+def test_multi_rank_fixtures(nproc):
+    needs_gpus(nproc)
+    run_on_ranks("test_nsconvolve3d", nproc)
+
+
+def on_ranks(pm, comm):
+    """each rank's MPIBlockDiag block of NonStationaryConvolve3D against its slice of the gathered fixtures, and
+    the 3-D image-domain cgls flow against its fixture"""
+    rank, P = comm.Get_rank(), comm.Get_size()
+    def block(nv_global, volume):
+        """this rank's volumes of a (nv_global, ...) stack: (local_shapes, flat slice, first volume, volume count)"""
+        rows = rows_of(P, nv_global)
+        k0 = sum(rows[:rank])
+        return [(r * volume,) for r in rows], slice(k0 * volume, (k0 + rows[rank]) * volume), k0, rows[rank]
+
+    ls, sl, k0, nv = block(mg3.NV, mg3.NX * mg3.NY * mg3.NZ)
+    for nh, bank, dt in mg3.cases():
+        hs, ih, x, v = mg3.case_inputs(nh, bank, dt)
+        Op = pm.MPIBlockDiag([pm.local.NonStationaryConvolve3D((mg3.NX, mg3.NY, mg3.NZ), hs[k], *ih, dtype=hs.dtype)
+                              for k in range(k0, k0 + nv)], dtype=dt)
+        gy, gya = decode(GOLD, mg3.key(nh, bank), dt, mg3.ENC)
+        name = f"{mg3.key(nh, bank)}/{dt}"
+        np.testing.assert_array_equal(host((Op @ pm.DistributedArray.to_dist(x, local_shapes=ls)).local_array), gy[sl],
+                                      err_msg=f"[rank {rank}] {name}/y")
+        np.testing.assert_array_equal(host((Op.H @ pm.DistributedArray.to_dist(v, local_shapes=ls)).local_array),
+                                      gya[sl], err_msg=f"[rank {rank}] {name}/ya")
+
+    ls, sl, k0, nv = block(mg3.FLOW_NV, mg3.FLOW_NY * mg3.FLOW_NX * mg3.FLOW_NZ)
+    Op = pm.MPIBlockDiag([pm.local.NonStationaryConvolve3D((mg3.FLOW_NY, mg3.FLOW_NX, mg3.FLOW_NZ), GOLD["flow/hs"],
+                                                           mg3.FLOW_IHY, mg3.FLOW_IHX, mg3.FLOW_IHZ)] * nv)
+    mmig = GOLD["flow/mmig"]
+    d = pm.DistributedArray.to_dist(mmig, local_shapes=ls)
+    x0 = pm.DistributedArray.to_dist(np.zeros_like(mmig), local_shapes=ls)
+    x, _, iiter, _, _, cost = pm.cgls(Op, d, x0=x0, niter=mg3.FLOW_NITER, tol=0.0)
+    assert iiter == int(GOLD[f"flow/P{P}/iiter"])
+    xtol, ctol = flow_tolerance()
+    np.testing.assert_allclose(np.asarray(cost), GOLD[f"flow/P{P}/cost"], rtol=ctol, err_msg=f"[rank {rank}] cost")
+    gx = GOLD[f"flow/P{P}/x"]
+    np.testing.assert_allclose(host(x.local_array), gx[sl], rtol=0, atol=xtol * np.abs(gx).max(),
+                               err_msg=f"[rank {rank}] x")

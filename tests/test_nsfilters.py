@@ -9,7 +9,6 @@ argument errors, and the fixtures of tests/golden/nsfilters_golden.npz (made by 
 reference's MPIVStack over the restatement; inputs exactly representable, so every dtype must match them bit for
 bit).  GPU: b2_nsfilters2d_adjoint through the C ABI, and the operators through the public interface."""
 import os
-import subprocess
 import sys
 
 import numpy as np
@@ -18,7 +17,9 @@ import pytest
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "golden"))
 import make_golden_nsfilters as mgf  # noqa: E402
-from ns_reference import U, assert_within, axis_w, gamma, guarded_twice  # noqa: E402
+from ns_reference import U, assert_within, axis_w, gamma  # noqa: E402
+from fixture_codec import decode, rows_of  # noqa: E402
+from op_checks import assert_cgls_replay_matches_steps, guarded_twice, host, needs_gpus, run_on_ranks  # noqa: E402
 
 GOLD = np.load(os.path.join(HERE, "golden", "nsfilters_golden.npz"), allow_pickle=False)
 
@@ -185,7 +186,7 @@ def test_fixtures_follow_the_restatement_in_every_dtype(case):
            F.NonStationaryFilters2D(i, nh, *ih, dtype=dt) for i in inp]
     y = np.concatenate([op.matvec(x) for op in ops])
     ya = sum(op.rmatvec(v[k * plane:(k + 1) * plane]) for k, op in enumerate(ops))
-    gy, gya = mgf.decode(GOLD, mgf.key(kind, nh, bank), dt)
+    gy, gya = decode(GOLD, mgf.key(kind, nh, bank), dt, mgf.ENC)
     np.testing.assert_array_equal(y, gy)
     np.testing.assert_array_equal(ya, gya)
 
@@ -197,10 +198,6 @@ def test_fixtures_follow_the_restatement_in_every_dtype(case):
 def pm():
     import pylops_mpi_b200 as pm
     return pm
-
-
-def host(t):
-    return t.cpu().numpy()
 
 
 def geom(shape, nf, nh, oh, dh):
@@ -360,7 +357,7 @@ def test_operator_vs_reference_fixtures(pm, case):
     got = host((Op @ pm.DistributedArray.to_dist(x, partition=pm.Partition.BROADCAST)).asarray())
     gota = host((Op.H @ pm.DistributedArray.to_dist(v)).asarray())
     assert got.dtype == np.dtype(dt) and gota.dtype == np.dtype(dt)
-    gy, gya = mgf.decode(GOLD, mgf.key(kind, nh, bank), dt)
+    gy, gya = decode(GOLD, mgf.key(kind, nh, bank), dt, mgf.ENC)
     np.testing.assert_array_equal(got, gy)
     np.testing.assert_array_equal(gota, gya)
 
@@ -393,36 +390,14 @@ def test_operator_attributes_dtypes_and_out(pm):
     assert (Op.nfilt, Op.nh, Op.hc, Op.oh, Op.dh) == ((3, 2), (5, 7), (2, 3), (2, 1), (4, 3))
     O1 = pm.local.NonStationaryFilters1D(inp[:, 0], 5, [3])
     assert O1.dims == (1, 5) and O1.dimsd == (20,) and O1.shape == (20, 5) and O1.dh == 1
-    F32, F64, C64, C128 = torch.float32, torch.float64, torch.complex64, torch.complex128
     op64 = pm.local.NonStationaryFilters2D(inp, (5, 7), [2, 6, 10], [1, 4])
-    for op, results in ((Op, (F32, F32, C64, C128)), (op64, (F64, F64, C128, C128))):
-        for adjoint in (False, True):
-            f = op.rmatvec if adjoint else op.matvec
-            nin, nout = (180, 210) if adjoint else (210, 180)
-            for xdt, want in zip((F32, F64, C64, C128), results):
-                x = torch.as_tensor(rng.standard_normal(nin)).to(xdt).cuda()
-                if xdt.is_complex:
-                    x = x + 1j * torch.as_tensor(rng.standard_normal(nin)).to(xdt).cuda()
-                ref = f(x)
-                assert ref.dtype == want and ref.numel() == nout
-                out = torch.full((nout,), 7.0, dtype=ref.dtype, device="cuda")
-                assert f(x, out=out) is out and torch.equal(out, ref)
-                buf = torch.full((nout, 2), 7.0, dtype=ref.dtype, device="cuda")
-                f(x, out=buf[:, 0])
-                assert torch.equal(buf[:, 0], ref) and bool((buf[:, 1] == 7.0).all())
-                if xdt.is_complex:                       # the real operator, applied part by part
-                    rdt = F32 if op is Op else F64
-                    re, im = f(x.real.contiguous().to(rdt)), f(x.imag.contiguous().to(rdt))
-                    assert torch.equal(ref, torch.complex(re, im).to(want))
-                with pytest.raises(ValueError, match="dimension mismatch"):
-                    f(x[:-1])
     # a complex operator computes in its real dtype and returns complex results
     opc = pm.local.NonStationaryFilters2D(inp, (5, 7), [2, 6, 10], [1, 4], dtype="complex128")
     assert opc.dtype == np.complex128
     for f, fc, nin in ((op64.matvec, opc.matvec, 210), (op64.rmatvec, opc.rmatvec, 180)):
         xr = torch.as_tensor(rng.standard_normal(nin)).cuda()
         yc = fc(xr)
-        assert yc.dtype == C128 and torch.equal(yc.real, f(xr)) and bool((yc.imag == 0).all())
+        assert yc.dtype == torch.complex128 and torch.equal(yc.real, f(xr)) and bool((yc.imag == 0).all())
         xc = xr + 1j * torch.as_tensor(rng.standard_normal(nin)).cuda()
         assert torch.equal(fc(xc), f(xc))
     # a float32 operator uses inp rounded to float32
@@ -435,31 +410,15 @@ def test_operator_attributes_dtypes_and_out(pm):
 @pytest.mark.gpu
 @pytest.mark.parametrize("dt", ["float32", "float64"])
 def test_cgls_graph_replay_matches_step_loop(pm, dt):
-    from pylops_mpi_b200.optimization.cls_basic import CGLS, _graph_safe
     rng = np.random.default_rng(12)
     ops = [pm.local.NonStationaryFilters2D(rng.standard_normal((300, 520)), (5, 5), [0], [100, 400], dtype=dt)
            for _ in range(2)]
     assert all(op._work is not None for op in ops)          # the split path, with its workspace, is captured
     Op = pm.MPIVStack(ops)
-    assert _graph_safe(Op)
     y = Op @ pm.DistributedArray.to_dist(rng.standard_normal(Op.shape[1]).astype(dt),
                                          partition=pm.Partition.BROADCAST)
-    x0 = np.zeros(Op.shape[1], dtype=dt)
-    a = CGLS(Op)
-    xa = a.setup(y=y, x0=pm.DistributedArray.to_dist(x0, partition=pm.Partition.BROADCAST), niter=15, damp=0.0,
-                 tol=0.0)
-    xa = a.run(xa, 15)
-    a.finalize()
-    assert a.graph_error is None, a.graph_error
-    assert a.graph_replays >= 10
-    b = CGLS(Op)
-    xb = b.setup(y=y, x0=pm.DistributedArray.to_dist(x0, partition=pm.Partition.BROADCAST), niter=15, damp=0.0,
-                 tol=0.0)
-    for _ in range(15):
-        xb = b.step(xb)
-    b.finalize()
-    np.testing.assert_array_equal(host(xa.asarray()), host(xb.asarray()))
-    np.testing.assert_array_equal(np.asarray(a.cost), np.asarray(b.cost))
+    x0 = pm.DistributedArray.to_dist(np.zeros(Op.shape[1], dtype=dt), partition=pm.Partition.BROADCAST)
+    assert_cgls_replay_matches_steps(pm, Op, y, x0, 15, 10)
 
 
 def flow_tolerance(f):
@@ -507,12 +466,55 @@ def test_estimation_flows_vs_reference(pm, kind, P):
 
 
 @pytest.mark.gpu
-def test_multi_rank_fixtures_p2():
-    import torch
-    if torch.cuda.device_count() < 2:
-        pytest.skip(f"needs 2 GPUs, box has {torch.cuda.device_count()}")
-    r = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node=2",
-                        "--master-addr", "127.0.0.1", "--master-port", "29839",
-                        os.path.join(HERE, "nsfilters_worker.py")], capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, (r.stdout[-4000:] + r.stderr[-8000:])
-    assert r.stdout.count("NSFILTERS_WORKER_OK") == 2
+@pytest.mark.parametrize("nproc", [1, 2])
+def test_multi_rank_fixtures(nproc):
+    needs_gpus(nproc)
+    run_on_ranks("test_nsfilters", nproc)
+
+
+def on_ranks(pm, comm):
+    """each rank's MPIVStack of NonStationaryFilters1D / 2D against its slice of the gathered fixtures, and the
+    two estimation flows against their fixtures"""
+    rank, P = comm.Get_rank(), comm.Get_size()
+    rows = rows_of(P, mgf.NI)
+    k0 = sum(rows[:rank])
+
+    for kind, nh, bank, dt in mgf.cases():
+        inp, ih, _, x, v = mgf.case_inputs(kind, nh, bank, dt)
+        plane = int(np.prod(inp.shape[1:]))
+        mine = inp[k0:k0 + rows[rank]]
+        ops = ([pm.local.NonStationaryFilters1D(i, nh, ih[0], dtype=dt) for i in mine] if kind == 1 else
+               [pm.local.NonStationaryFilters2D(i, nh, *ih, dtype=dt) for i in mine])
+        Op = pm.MPIVStack(ops, dtype=dt)
+        ls = [(r * plane,) for r in rows]
+        gy, gya = decode(GOLD, mgf.key(kind, nh, bank), dt, mgf.ENC)
+        name = f"{mgf.key(kind, nh, bank)}/{dt}"
+        y = (Op @ pm.DistributedArray.to_dist(x, partition=pm.Partition.BROADCAST)).local_array.cpu().numpy()
+        np.testing.assert_array_equal(y, gy[k0 * plane:(k0 + rows[rank]) * plane], err_msg=f"[rank {rank}] {name}/y")
+        ya = (Op.H @ pm.DistributedArray.to_dist(v, local_shapes=ls)).local_array.cpu().numpy()
+        np.testing.assert_array_equal(ya, gya, err_msg=f"[rank {rank}] {name}/ya")
+
+    # the estimation flows: cgls over this rank's inputs, the bank all-reduced
+    for kind in (1, 2):
+        f = f"flow{kind}"
+        if kind == 1:
+            inps, d, niter = GOLD["flow1/refl"], GOLD["flow1/d"], mgf.FLOW1_NITER
+        else:
+            inps, niter = GOLD["flow2/mmig"][:mgf.FLOW2_NTRAIN], mgf.FLOW2_NITER
+            d = GOLD["flow2/m"][:mgf.FLOW2_NTRAIN].ravel()
+        fr = rows_of(P, len(inps))
+        f0 = sum(fr[:rank])
+        plane = int(np.prod(inps.shape[1:]))
+        ops = [pm.local.NonStationaryFilters1D(i, 15, mgf.FLOW1_IH) if kind == 1 else
+               pm.local.NonStationaryFilters2D(i, mgf.FLOW2_NH, mgf.mg2.FLOW_IHX, mgf.mg2.FLOW_IHZ)
+               for i in inps[f0:f0 + fr[rank]]]
+        Op = pm.MPIVStack(ops)
+        x0 = pm.DistributedArray.to_dist(np.zeros(Op.shape[1]), partition=pm.Partition.BROADCAST)
+        dd = pm.DistributedArray.to_dist(d, local_shapes=[(r * plane,) for r in fr])
+        x, _, iiter, _, _, cost = pm.cgls(Op, dd, x0=x0, niter=niter, tol=0.0)
+        assert iiter == int(GOLD[f"{f}/P{P}/iiter"])
+        xtol, ctol = flow_tolerance(f)
+        np.testing.assert_allclose(np.asarray(cost), GOLD[f"{f}/P{P}/cost"], rtol=ctol, err_msg=f"[rank {rank}] {f} cost")
+        gx = GOLD[f"{f}/P{P}/x"]
+        np.testing.assert_allclose(x.local_array.cpu().numpy(), gx, rtol=0, atol=xtol * np.abs(gx).max(),
+                                   err_msg=f"[rank {rank}] {f} x")

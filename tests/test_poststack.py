@@ -9,7 +9,6 @@ make_golden_poststack.py: the reference's MPIBlockDiag and solvers over the rest
 representable, so every dtype must match them bit for bit).  GPU: the fused b2_poststack_axis kernel through the C
 ABI, against NumPy and bit for bit against the two-launch chain, and the operators through the public interface."""
 import os
-import subprocess
 import sys
 
 import numpy as np
@@ -18,6 +17,9 @@ import pytest
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "golden"))
 import make_golden_poststack as mgp  # noqa: E402
+from fixture_codec import decode, rows_of  # noqa: E402
+from op_checks import (assert_cgls_replay_matches_steps, assert_rejected, device_input, guarded_twice, host,  # noqa: E402
+                       needs_gpus, run_on_ranks)
 
 GOLD = np.load(os.path.join(HERE, "golden", "poststack_golden.npz"), allow_pickle=False)
 CASES = mgp.cases()
@@ -170,14 +172,14 @@ def test_poststack_fixture_inventory():
 def test_fixtures_follow_the_definition(case):
     layout, P, kind, nh, dt = case
     wav, x, v = mgp.case_inputs(nh, dt)
-    parts = np.cumsum([0] + [r * mgp.NX * mgp.NT0 for r in mgp.rows_of(P)])
+    parts = np.cumsum([0] + [r * mgp.NX * mgp.NT0 for r in rows_of(P, mgp.NY)])
     fwd, adj = [], []
-    for a, b, ny_r in zip(parts[:-1], parts[1:], mgp.rows_of(P)):
+    for a, b, ny_r in zip(parts[:-1], parts[1:], rows_of(P, mgp.NY)):
         dims = mgp.block_dims(layout, ny_r)
         axis = 0 if layout == "native" else 2
         fwd.append(post_ref(x[a:b].reshape(dims), wav, kind, False, axis).ravel())
         adj.append(post_ref(v[a:b].reshape(dims), wav, kind, True, axis).ravel())
-    gy, gya = mgp.expected(GOLD, layout, P, kind, nh, dt)
+    gy, gya = decode(GOLD, mgp.key(layout, P, kind, nh), dt, mgp.ENC)
     np.testing.assert_array_equal(gy, np.concatenate(fwd))       # exact: every value is a multiple of 1/4
     np.testing.assert_array_equal(gya, np.concatenate(adj))
 
@@ -191,10 +193,6 @@ def pm():
     return pm
 
 
-def host(t):
-    return t.cpu().numpy()
-
-
 def c_post(pm, x, y, shape, h, nh, off, kind, adjoint, code):
     L = pm._lib
     return L.lib.b2_poststack_axis(L.ctx(), x, y, shape[0], shape[1], shape[2], h, nh, off, kind, adjoint, code,
@@ -203,25 +201,12 @@ def c_post(pm, x, y, shape, h, nh, off, kind, adjoint, code):
 
 def run_kernel(pm, x_np, h_np, off, kind, adjoint, dt, misalign=False, guard=5):
     """apply through the C ABI into a guarded interior view; returns (y, guards intact, second apply bit-equal)"""
-    import torch
-    tdt = {np.float32: torch.float32, np.float64: torch.float64}[dt]
-    N = x_np.size
-    s = 1 if misalign else 0
-    xb = torch.zeros(N + s, dtype=tdt, device="cuda")
-    xb[s:] = torch.as_tensor(x_np.ravel().astype(dt))
-    x = xb[s:]
-    yb = torch.full((N + 2 * guard + s,), 7.25, dtype=tdt, device="cuda")
-    y = yb[guard + s:guard + s + N]
-    h = torch.as_tensor(np.asarray(h_np, dtype=dt)).cuda()
+    x, h = device_input(x_np, dt, misalign), device_input(h_np, dt)
     code = pm._lib.F32 if dt == np.float32 else pm._lib.F64
     args = (x_np.shape, h.data_ptr(), h.numel(), off, KINDS[kind], int(adjoint), code)
-    assert c_post(pm, x.data_ptr(), y.data_ptr(), *args) == 0
-    first = y.clone()
-    assert c_post(pm, x.data_ptr(), y.data_ptr(), *args) == 0
-    torch.cuda.synchronize()
-    g = host(yb)
-    guards_ok = bool(np.all(g[:guard + s] == 7.25) and np.all(g[guard + s + N:] == 7.25))
-    return host(first).reshape(x_np.shape), guards_ok, bool(torch.equal(first, y))
+    y, guards_ok, same = guarded_twice(lambda yp: c_post(pm, x.data_ptr(), yp, *args), x_np.size, dt, guard,
+                                       int(misalign))
+    return y.reshape(x_np.shape), guards_ok, same
 
 
 def check_close(got, x, h, off, kind, adjoint, dt):
@@ -330,13 +315,8 @@ def test_kernel_error_codes_leave_y_untouched(pm):
         (dict(kind=1), ARG), (dict(kind=3), ARG), (dict(kind=-1), ARG),
         (dict(dtype=L.C64), DT), (dict(dtype=L.BF16), DT), (dict(dtype=99), DT),
     ]
-    for kw, want in cases:
-        a = dict(x=x.data_ptr(), y=y.data_ptr(), h=h.data_ptr(), nh=4, off=1, kind=2, dtype=L.F64)
-        a.update(kw)
-        if a["y"] == "x":
-            a["y"] = a["x"]
-        rc = c_post(pm, a["x"], a["y"], (2, 3, 4), a["h"], a["nh"], a["off"], a["kind"], 0, a["dtype"])
-        assert rc == want, (kw, rc)
+    assert_rejected(lambda a: c_post(pm, a["x"], a["y"], (2, 3, 4), a["h"], a["nh"], a["off"], a["kind"], 0, a["dtype"]),
+                    dict(x=x.data_ptr(), y=y.data_ptr(), h=h.data_ptr(), nh=4, off=1, kind=2, dtype=L.F64), cases, y)
     for shape in ((0, 3, 4), (2, 0, 4), (2, 3, 0)):
         assert c_post(pm, x.data_ptr(), y.data_ptr(), shape, h.data_ptr(), 4, 1, 2, 0, L.F64) == 0
     torch.cuda.synchronize()
@@ -360,13 +340,13 @@ def test_operator_vs_reference_fixtures(pm, case):
     """exactly representable inputs: the operator must reproduce the reference's outputs bit for bit in every dtype"""
     layout, P, kind, nh, dt = case
     wav, x, v = mgp.case_inputs(nh, dt)
-    ops = [local_op(pm, layout, r, wav, kind) for r in mgp.rows_of(P)]
+    ops = [local_op(pm, layout, r, wav, kind) for r in rows_of(P, mgp.NY)]
     assert all(type(op).__name__ == "PoststackLinearModelling" for op in ops)          # the fold
     Op = pm.MPIBlockDiag(ops, dtype=dt)
     got = host((Op @ pm.DistributedArray.to_dist(x)).asarray())
     gota = host((Op.H @ pm.DistributedArray.to_dist(v)).asarray())
     assert got.dtype == np.dtype(dt) and gota.dtype == np.dtype(dt)
-    gy, gya = mgp.expected(GOLD, layout, P, kind, nh, dt)
+    gy, gya = decode(GOLD, mgp.key(layout, P, kind, nh), dt, mgp.ENC)
     np.testing.assert_array_equal(got, gy)
     np.testing.assert_array_equal(gota, gya)
 
@@ -386,9 +366,6 @@ def test_real_wavelet_on_complex_data_keeps_the_imaginary_part(pm):
         x3 = x.reshape((40,) + (spatdims or ()))
         np.testing.assert_allclose(y, post_ref(x3, wav, "centered").ravel(), rtol=1e-12, atol=1e-12)
         np.testing.assert_allclose(ya, post_ref(x3, wav, "centered", True).ravel(), rtol=1e-12, atol=1e-12)
-        out = torch.zeros(n, dtype=torch.complex128, device="cuda")
-        Op.matvec(torch.as_tensor(x).cuda(), out=out)
-        np.testing.assert_array_equal(host(out), y)
 
 
 @pytest.mark.gpu
@@ -524,7 +501,7 @@ def test_tutorial_poststack_line_for_line(pm):
 def test_tutorial_flows_vs_reference(pm, P):
     """the three solves with the y rows of P ranks held as P blocks of one MPIBlockDiag"""
     wav, m3d, mback3d = mgp.flow_inputs()
-    ny = mgp.rows_of(P, mgp.FLOW_NY)
+    ny = rows_of(P, mgp.FLOW_NY)
     nx, nz = mgp.NX, mgp.NT0
     ops = []
     for ny_i in ny:
@@ -552,36 +529,74 @@ def test_tutorial_flows_vs_reference(pm, P):
 @pytest.mark.gpu
 @pytest.mark.parametrize("layout", mgp.LAYOUTS)
 def test_cgls_graph_replay_matches_step_loop(pm, layout):
-    from pylops_mpi_b200.optimization.cls_basic import CGLS, _graph_safe
     rng = np.random.default_rng(12)
     wav = rng.standard_normal(21)
     Op = pm.MPIBlockDiag([local_op(pm, layout, 24, wav, "centered")])
-    assert _graph_safe(Op)
     n = Op.shape[0]
     y = Op @ pm.DistributedArray.to_dist(rng.standard_normal(n))
-    x0 = np.zeros(n)
-    a = CGLS(Op)
-    xa = a.setup(y=y, x0=pm.DistributedArray.to_dist(x0), niter=25, damp=0.0, tol=0.0)
-    xa = a.run(xa, 25)
-    a.finalize()
-    assert a.graph_error is None, a.graph_error
-    assert a.graph_replays >= 20
-    b = CGLS(Op)
-    xb = b.setup(y=y, x0=pm.DistributedArray.to_dist(x0), niter=25, damp=0.0, tol=0.0)
-    for _ in range(25):
-        xb = b.step(xb)
-    b.finalize()
-    np.testing.assert_array_equal(host(xa.asarray()), host(xb.asarray()))
-    np.testing.assert_array_equal(np.asarray(a.cost), np.asarray(b.cost))
+    assert_cgls_replay_matches_steps(pm, Op, y, pm.DistributedArray.to_dist(np.zeros(n)), 25, 20)
 
 
 @pytest.mark.gpu
-def test_multi_rank_fixtures_p2():
-    import torch
-    if torch.cuda.device_count() < 2:
-        pytest.skip(f"needs 2 GPUs, box has {torch.cuda.device_count()}")
-    r = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node=2",
-                        "--master-addr", "127.0.0.1", "--master-port", "29813",
-                        os.path.join(HERE, "poststack_worker.py")], capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, (r.stdout[-4000:] + r.stderr[-8000:])
-    assert r.stdout.count("POSTSTACK_WORKER_OK") == 2
+@pytest.mark.parametrize("nproc", [1, 2])
+def test_multi_rank_fixtures(nproc):
+    needs_gpus(nproc)
+    run_on_ranks("test_poststack", nproc)
+
+
+def on_ranks(pm, comm):
+    """each rank's MPIBlockDiag block against its slice of the gathered fixtures, and the three solves of
+    tutorials/poststack.py against their fixtures"""
+    rank, P = comm.Get_rank(), comm.Get_size()
+
+    def block(ny):
+        """this rank's rows of y: (local_shapes, flat slice, local rows)"""
+        rows = rows_of(P, ny)
+        plane = mgp.NX * mgp.NT0
+        lo, hi = sum(rows[:rank]) * plane, sum(rows[:rank + 1]) * plane
+        return [(r * plane,) for r in rows], slice(lo, hi), rows[rank]
+
+    def check(name, got, ref, rtol, atol):
+        np.testing.assert_allclose(got, ref, rtol=rtol, atol=atol, err_msg=f"[rank {rank}] {name}")
+
+    ls, sl, ny_r = block(mgp.NY)
+    for (layout, Pc, kind, nh, dt) in CASES:
+        if Pc != P:
+            continue
+        wav, x, v = mgp.case_inputs(nh, dt)
+        Op = pm.MPIBlockDiag([local_op(pm, layout, ny_r, wav, kind)], dtype=dt)
+        gy, gya = decode(GOLD, mgp.key(layout, P, kind, nh), dt, mgp.ENC)   # exact: exactly representable inputs
+        name = f"{mgp.key(layout, P, kind, nh)}/{dt}"
+        np.testing.assert_array_equal(host((Op @ pm.DistributedArray.to_dist(x, local_shapes=ls)).local_array),
+                                      gy[sl], err_msg=f"[rank {rank}] {name}/y")
+        np.testing.assert_array_equal(host((Op.H @ pm.DistributedArray.to_dist(v, local_shapes=ls)).local_array),
+                                      gya[sl], err_msg=f"[rank {rank}] {name}/ya")
+
+    ls, sl, ny_i = block(mgp.FLOW_NY)
+    wav, m3d, mback3d = mgp.flow_inputs()
+    nx, nz = mgp.NX, mgp.NT0
+    PPop = pm.local.PoststackLinearModelling(wav, nt0=nz, spatdims=(ny_i, nx))
+    Top = pm.local.Transpose((ny_i, nx, nz), (2, 0, 1))
+    BDiag = pm.MPIBlockDiag([Top.H @ PPop @ Top])
+    m = pm.DistributedArray.to_dist(m3d.ravel(), local_shapes=ls)
+    x0 = pm.DistributedArray.to_dist(mback3d.ravel(), local_shapes=ls)
+    d = BDiag @ m
+    check("flow/d", host(d.local_array), GOLD["flow/d"][sl], 1e-12, 1e-12)
+
+    def check_flow(name, x, iiter, cost):
+        g = f"flow/P{P}/{name}"
+        assert iiter == int(GOLD[f"{g}/iiter"])
+        check(f"{g}/cost", np.asarray(cost), GOLD[f"{g}/cost"], 1e-10, 0)
+        check(f"{g}/x", host(x.local_array), GOLD[f"{g}/x"][sl], 1e-9, 1e-11)
+
+    x, _, iiter, _, _, cost = pm.cgls(BDiag, d, x0=x0, niter=mgp.FLOW_NITER, tol=0.0)
+    check_flow("iter", x, iiter, cost)
+    LapOp = pm.MPILaplacian(dims=(mgp.FLOW_NY, nx, nz), axes=(0, 1, 2), weights=(1, 1, 1), sampling=(1, 1, 1),
+                            dtype=BDiag.dtype)
+    x, iiter, cost = pm.cg(BDiag.H @ BDiag + mgp.FLOW_EPSR * LapOp.H @ LapOp, BDiag.H @ d, x0=x0,
+                           niter=mgp.FLOW_NITER, tol=0.0)
+    check_flow("ne", x, iiter, cost)
+    zero = pm.DistributedArray.to_dist(np.zeros(m3d.size), local_shapes=ls)
+    x, _, iiter, _, _, cost = pm.cgls(pm.MPIStackedVStack([BDiag, np.sqrt(mgp.FLOW_EPSR) * LapOp]),
+                                      pm.StackedDistributedArray([d, zero]), x0=x0, niter=mgp.FLOW_NITER, tol=0.0)
+    check_flow("reg", x, iiter, cost)
