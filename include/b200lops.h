@@ -307,6 +307,34 @@ int b2_kirchhoff_chunk(b2_ctx* ctx, const void* x, void* y, const double* trav_s
 int b2_radon(b2_ctx* ctx, const void* x, void* y, size_t nt, size_t n_inner, size_t nhy, size_t nhx, size_t npy,
              size_t npx, const double* hy, const double* hx, const double* py, const double* px, int kind, int interp,
              int adjoint, int dtype, void* stream);
+/* b2_radon applied to every window of a section, with the tapered overlap-add of b2_sliding, in one launch: the
+ * sliding-window Radon transform of pylops.signalprocessing.Sliding2D / Sliding3D over Radon2D / Radon3D.  The section
+ * [n0][n1][nt][n_inner] holds nwins0 x nwins1 windows of nhy x nhx traces, window w = i0 * nwins1 + i1 starting at
+ * trace (i0 * step0, i1 * step1); the model is [nwins0 * nwins1][npy][npx][nt][n_inner], one b2_radon model block per
+ * window, on the window-local offsets hy, hx (2-D: hy = py = NULL, nhy = npy = 1).  tap is b2_sliding's table
+ * [nwins0 * nwins1][nhy][nhx] in the dtype (NULL: no taper).  Forward x (model) -> y (section): each section sample
+ * sums, as b2_sliding's fold, tap * v over the windows that hold its trace, v the window's b2_radon value (a float64
+ * sum rounded once to the dtype); samples no window holds are 0.  Adjoint x (section) -> y (model): each window's
+ * b2_radon stack of tap * d, the product rounded to the dtype.  Both directions equal b2_radon per window plus
+ * b2_sliding bit for bit.  One launch, no atomics, no allocation.  dtype F32 / F64.  B2_ERR_ARG: b2_radon's, and
+ * b2_sliding's window checks, more CTAs than one grid holds; B2_ERR_DTYPE: another dtype; y is untouched on every
+ * error */
+int b2_radon_windows(b2_ctx* ctx, const void* x, void* y, size_t nt, size_t n_inner, size_t n0, size_t n1, size_t nhy,
+                     size_t nhx, size_t npy, size_t npx, const double* hy, const double* hx, const double* py,
+                     const double* px, int kind, int interp, size_t nwins0, size_t nwins1, size_t step0,
+                     size_t step1, const void* tap, int adjoint, int dtype, void* stream);
+/* tapered overlap-add: the combining stage of pylops.signalprocessing.Sliding2D / Sliding3D.  Windows
+ * [nwins0][nwins1][nwin0][nwin1][nt][n_inner] (n_inner values per sample: 2 for the (re, im) pairs of complex data in
+ * the real dtype), data [n0][n1][nt][n_inner]; window w = i0 * nwins1 + i1 starts at trace (i0 * step0, i1 * step1).
+ * tap [nwins0 * nwins1][nwin0][nwin1] is one taper value per window trace in the dtype (NULL: no taper).  Forward
+ * (fold) x = windows -> y = data: each sample is the sum over i0 ascending of the sum over i1 ascending of
+ * tap * window over the windows that hold its trace, every product and sum rounded to the dtype; samples no window
+ * holds are 0.  Adjoint (unfold) x = data -> y = windows: tap * data.  One launch, no atomics, no allocation.  dtype
+ * F32 / F64.  B2_ERR_ARG: a null pointer (tap excepted), x == y, a zero size, an axis of 2^31 or more, windows that
+ * leave the section, 2^62 or more values; B2_ERR_DTYPE: another dtype; y is untouched on every error */
+int b2_sliding(b2_ctx* ctx, const void* x, void* y, size_t n0, size_t n1, size_t nt, size_t n_inner, size_t nwins0,
+               size_t nwins1, size_t nwin0, size_t nwin1, size_t step0, size_t step1, const void* tap, int adjoint,
+               int dtype, void* stream);
 /* analytic (constant-velocity) traveltime table of pylops.waveeqprocessing.Kirchhoff, in b2_kirchhoff_chunk's
  * layout: table[p][j] = |grid point i0 + j - point p| / vel for p < n, j < nc (row stride nc).  Axes are float64
  * device arrays; y = NULL for 2-D (ny ignored), where the grid is meshgrid(x, z, indexing="ij") raveled,

@@ -18,7 +18,7 @@ OUT = os.path.join(HERE, "libb200lops.so")
 INCLUDE = os.path.join(os.path.dirname(HERE), "include")
 
 SOURCES = ["ctx.cu", "elementwise.cu", "reduce.cu", "sparsity.cu", "stencil.cu", "convolve.cu", "nsconvolve.cu", "nsconvolve2d.cu",
-           "nsconvolve3d.cu", "nsfilters.cu", "radon.cu", "kirchhoff.cu", "eikonal.cu", "lsqr.cu", "gemv.cu",
+           "nsconvolve3d.cu", "nsfilters.cu", "radon.cu", "sliding.cu", "kirchhoff.cu", "eikonal.cu", "lsqr.cu", "gemv.cu",
            "gemm_simt.cu", "gemm_tc.cu", "fredholm_tc.cu", "host_pipe.cu", "comm.cu", "peer.cu"]
 
 
@@ -57,6 +57,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
                 and os.path.getmtime(obj) > os.path.getmtime(os.path.join(CSRC, "fd_axis.cuh"))
                 and os.path.getmtime(obj) > os.path.getmtime(os.path.join(CSRC, "peer.cuh"))
                 and os.path.getmtime(obj) > os.path.getmtime(os.path.join(CSRC, "ns_core.cuh"))
+                and os.path.getmtime(obj) > os.path.getmtime(os.path.join(CSRC, "sliding.cuh"))
                 and os.path.getmtime(obj) > os.path.getmtime(os.path.join(INCLUDE, "b200lops.h"))):
             continue
         cmd = [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",

@@ -27,9 +27,17 @@
 // until tdec leaves the range.  A model trace whose terms are not finite (hyperbolic p = 0) gives NaN or inf for
 // every t0 and is skipped, as the mask drops all its pairs.  No atomics and no workspace: one launch per apply, the
 // same bits on every run.
+//
+// Windows (b2_radon_windows: pylops.signalprocessing.Sliding2D / Sliding3D over Radon2D / Radon3D, on the window
+// geometry of sliding.cuh).  The same two kernels, compiled a second time with WIN: the section [n0][n1][nt] holds
+// windows of nhy x nhx traces, each with its own model block [npy][npx][nt] and the window-local offsets hy, hx.
+// Forward: one thread per section sample; for each window that holds its trace (i1 inside i0, both ascending) it forms
+// that window's value exactly as above (a float64 sum rounded once to T), multiplies it by the window's taper in T and
+// adds it in T in b2_sliding's order.  Adjoint: one thread per model sample of window w, reading tap * d rounded to T
+// where the one-gather kernel reads d.  Both equal b2_radon per window plus b2_sliding bit for bit.
 #include <math.h>
 
-#include "common.cuh"
+#include "sliding.cuh"
 
 namespace {
 
@@ -37,6 +45,11 @@ constexpr int RD_THREADS = 256;
 
 template <typename T>
 __device__ __forceinline__ double ld(const T* p) { return (double)__ldg(p); }
+// a data value as the windowed stack reads it: tap * d rounded to T when tapered
+template <typename T>
+__device__ __forceinline__ double ldt(const T* p, T tap, bool tapered) {
+  return tapered ? (double)mul_rn(tap, __ldg(p)) : ld(p);
+}
 
 // the offset term of one (trace, model trace) pair on one axis
 template <int KIND>
@@ -69,17 +82,22 @@ __device__ __forceinline__ long long first_guess(double lo, double c, long long 
 }
 
 // ---- adjoint: stacking ------------------------------------------------------------------------------------------
-// CTA b covers t0 in [(b % ntb) * RD_THREADS, +RD_THREADS) of model trace b / ntb (= ipy * npx + ipx)
-template <typename T, int C, int KIND>
-__global__ void __launch_bounds__(RD_THREADS)
-radon_stack_kernel(const T* __restrict__ x, T* __restrict__ y, long long nt, long long ntb, long long nhy,
-                   long long nhx, long long npx, const double* __restrict__ hy, const double* __restrict__ hx,
-                   const double* __restrict__ py, const double* __restrict__ px, bool interp) {
+// CTA b covers t0 in [(b % ntb) * RD_THREADS, +RD_THREADS) of model trace b / ntb (= ipy * npx + ipx; WIN: of window
+// w's block, (w * npy + ipy) * npx + ipx, whose traces are the section traces of window w, each value tap * d in T)
+template <typename T, int C, int KIND, bool WIN>
+__device__ __forceinline__ void stack(const T* __restrict__ x, T* __restrict__ y, long long nt, long long ntb,
+                                      long long nhy, long long nhx, long long npy, long long npx,
+                                      const double* __restrict__ hy, const double* __restrict__ hx,
+                                      const double* __restrict__ py, const double* __restrict__ px, bool interp,
+                                      const Windows& win, const T* __restrict__ tap) {
   __shared__ double sx[RD_THREADS];
   const long long iq = blockIdx.x / ntb;
   const long long t0 = (blockIdx.x - iq * ntb) * RD_THREADS + threadIdx.x;
-  const long long ipy = iq / npx, ipx = iq - ipy * npx;
-  const bool three = hy != nullptr, live = t0 < nt;
+  const long long w = WIN ? iq / (npy * npx) : 0, ip = iq - w * npy * npx;
+  const long long ipy = ip / npx, ipx = ip - ipy * npx;
+  const bool three = hy != nullptr, live = t0 < nt, tapered = WIN && tap != nullptr;
+  const long long i0 = WIN ? w / win.nw1 : 0;
+  const long long a0 = i0 * win.step0, b0 = (w - i0 * win.nw1) * win.step1;   // WIN: the window's first trace
   const double pxv = __ldg(px + ipx);
   const double lim = (double)(interp ? nt - 1 : nt);
   double acc[C];
@@ -93,20 +111,23 @@ radon_stack_kernel(const T* __restrict__ x, T* __restrict__ y, long long nt, lon
       if ((int)threadIdx.x < nk) sx[threadIdx.x] = term<KIND>(__ldg(hx + j0 + threadIdx.x), pxv);
       __syncthreads();
       if (!live) continue;
-      const T* xt = x + (size_t)(jy * nhx + j0) * nt * C;
+      const T* xt = x + (size_t)(WIN ? (a0 + jy) * win.n1 + b0 + j0 : jy * nhx + j0) * nt * C;
+      const T* tp = tapered ? tap + (w * nhy + jy) * nhx + j0 : nullptr;
       for (int k = 0; k < nk; ++k, xt += (size_t)nt * C) {
         const double v = curve<KIND>(t0, sx[k], cy, three);
         if (!(v >= 0.0 && v < lim)) continue;
         const long long it = (long long)v;
         const T* xs = xt + (size_t)it * C;
+        const T tv = tapered ? __ldg(tp + k) : T(1);
         if (interp) {
           const double d = __dadd_rn(v, -(double)it), w0 = __dadd_rn(1.0, -d);
 #pragma unroll
           for (int c = 0; c < C; ++c)
-            acc[c] = __dadd_rn(acc[c], __dadd_rn(__dmul_rn(ld(xs + c), w0), __dmul_rn(ld(xs + C + c), d)));
+            acc[c] = __dadd_rn(acc[c], __dadd_rn(__dmul_rn(ldt(xs + c, tv, tapered), w0),
+                                                 __dmul_rn(ldt(xs + C + c, tv, tapered), d)));
         } else {
 #pragma unroll
-          for (int c = 0; c < C; ++c) acc[c] = __dadd_rn(acc[c], ld(xs + c));
+          for (int c = 0; c < C; ++c) acc[c] = __dadd_rn(acc[c], ldt(xs + c, tv, tapered));
         }
       }
     }
@@ -118,95 +139,169 @@ radon_stack_kernel(const T* __restrict__ x, T* __restrict__ y, long long nt, lon
 }
 
 // ---- forward: spreading ------------------------------------------------------------------------------------------
-// CTA b covers samples s in [(b % ntb) * RD_THREADS, +RD_THREADS) of trace b / ntb (= jy * nhx + jx)
-template <typename T, int C, int KIND>
-__global__ void __launch_bounds__(RD_THREADS)
-radon_spread_kernel(const T* __restrict__ x, T* __restrict__ y, long long nt, long long ntb, long long nhx,
-                    long long npy, long long npx, const double* __restrict__ hy, const double* __restrict__ hx,
-                    const double* __restrict__ py, const double* __restrict__ px, bool interp) {
+// CTA b covers samples s in [(b % ntb) * RD_THREADS, +RD_THREADS) of trace b / ntb (= jy * nhx + jx; WIN: of section
+// trace a * n1 + b, which sums the tapered values of the windows that hold it, each from that window's model block)
+template <typename T, int C, int KIND, bool WIN>
+__device__ __forceinline__ void spread(const T* __restrict__ x, T* __restrict__ y, long long nt, long long ntb,
+                                       long long nhy, long long nhx, long long npy, long long npx,
+                                       const double* __restrict__ hy, const double* __restrict__ hx,
+                                       const double* __restrict__ py, const double* __restrict__ px, bool interp,
+                                       const Windows& win, const T* __restrict__ tap) {
   __shared__ double sx[RD_THREADS];
   const long long jh = blockIdx.x / ntb;
   const long long s = (blockIdx.x - jh * ntb) * RD_THREADS + threadIdx.x;
-  const long long jy = jh / nhx, jx = jh - jy * nhx;
   const bool three = hy != nullptr, live = s < nt;
-  const double hxv = __ldg(hx + jx);
   // tdec range of the model samples that reach s; with interp the mask tdec < nt - 1 caps it
   const double lo = (double)(interp && s > 0 ? s - 1 : s);
   const double hi = interp ? fmin((double)(s + 1), (double)(nt - 1)) : (double)(s + 1);
-  double acc[C];
+  // the windows [f0, l0] x [f1, l1] that hold the trace; without WIN the one gather
+  long long a = 0, b = 0, f0 = 0, l0 = 0, f1 = 0, l1 = 0;
+  if (WIN) {
+    a = jh / win.n1;
+    b = jh - a * win.n1;
+    covering(a, win.nw0, win.len0, win.step0, f0, l0);
+    covering(b, win.nw1, win.len1, win.step1, f1, l1);
+  }
+  T out[C];
 #pragma unroll
-  for (int c = 0; c < C; ++c) acc[c] = 0.0;
-  for (long long ipy = 0; ipy < npy; ++ipy) {
-    const double cy = three ? term<KIND>(__ldg(hy + jy), __ldg(py + ipy)) : 0.0;
-    for (long long i0 = 0; i0 < npx; i0 += RD_THREADS) {
-      const int nk = (int)min((long long)RD_THREADS, npx - i0);
-      __syncthreads();
-      if ((int)threadIdx.x < nk) sx[threadIdx.x] = term<KIND>(hxv, __ldg(px + i0 + threadIdx.x));
-      __syncthreads();
-      if (!live) continue;
-      const T* xm = x + (size_t)(ipy * npx + i0) * nt * C;
-      for (int k = 0; k < nk; ++k, xm += (size_t)nt * C) {
-        const double cx = sx[k];
-        const double c = three ? cx + cy : cx;
-        if (!isfinite(c)) continue;
-        long long t = first_guess<KIND>(lo, c, nt);
-        while (t > 0 && curve<KIND>(t - 1, cx, cy, three) >= lo) --t;
-        for (; t < nt; ++t) {
-          const double v = curve<KIND>(t, cx, cy, three);
-          if (!(v >= lo)) continue;             // below the range: the estimate was short
-          if (!(v < hi)) break;
-          const T* xs = xm + (size_t)t * C;
-          if (interp) {
-            const long long it = (long long)v;
-            const double d = __dadd_rn(v, -(double)it);
-            const double w = it == s ? __dadd_rn(1.0, -d) : d;
+  for (int c = 0; c < C; ++c) out[c] = T(0);
+  for (long long i0 = f0; i0 <= l0; ++i0) {
+    T part[C];
 #pragma unroll
-            for (int c = 0; c < C; ++c) acc[c] = __dadd_rn(acc[c], __dmul_rn(ld(xs + c), w));
-          } else {
+    for (int c = 0; c < C; ++c) part[c] = T(0);
+    for (long long i1 = f1; i1 <= l1; ++i1) {
+      const long long w = i0 * win.nw1 + i1;
+      const long long jy = WIN ? a - i0 * win.step0 : jh / nhx;
+      const long long jx = WIN ? b - i1 * win.step1 : jh - jy * nhx;
+      const T* xw = WIN ? x + (size_t)w * npy * npx * nt * C : x;
+      const double hxv = __ldg(hx + jx);
+      double acc[C];
 #pragma unroll
-            for (int c = 0; c < C; ++c) acc[c] = __dadd_rn(acc[c], ld(xs + c));
+      for (int c = 0; c < C; ++c) acc[c] = 0.0;
+      for (long long ipy = 0; ipy < npy; ++ipy) {
+        const double cy = three ? term<KIND>(__ldg(hy + jy), __ldg(py + ipy)) : 0.0;
+        for (long long i0p = 0; i0p < npx; i0p += RD_THREADS) {
+          const int nk = (int)min((long long)RD_THREADS, npx - i0p);
+          __syncthreads();
+          if ((int)threadIdx.x < nk) sx[threadIdx.x] = term<KIND>(hxv, __ldg(px + i0p + threadIdx.x));
+          __syncthreads();
+          if (!live) continue;
+          const T* xm = xw + (size_t)(ipy * npx + i0p) * nt * C;
+          for (int k = 0; k < nk; ++k, xm += (size_t)nt * C) {
+            const double cx = sx[k];
+            const double c = three ? cx + cy : cx;
+            if (!isfinite(c)) continue;
+            long long t = first_guess<KIND>(lo, c, nt);
+            while (t > 0 && curve<KIND>(t - 1, cx, cy, three) >= lo) --t;
+            for (; t < nt; ++t) {
+              const double v = curve<KIND>(t, cx, cy, three);
+              if (!(v >= lo)) continue;             // below the range: the estimate was short
+              if (!(v < hi)) break;
+              const T* xs = xm + (size_t)t * C;
+              if (interp) {
+                const long long it = (long long)v;
+                const double d = __dadd_rn(v, -(double)it);
+                const double wt = it == s ? __dadd_rn(1.0, -d) : d;
+#pragma unroll
+                for (int c = 0; c < C; ++c) acc[c] = __dadd_rn(acc[c], __dmul_rn(ld(xs + c), wt));
+              } else {
+#pragma unroll
+                for (int c = 0; c < C; ++c) acc[c] = __dadd_rn(acc[c], ld(xs + c));
+              }
+            }
           }
         }
       }
+      if (WIN) {
+        const T tv = tap ? __ldg(tap + (w * win.len0 + jy) * win.len1 + jx) : T(1);
+#pragma unroll
+        for (int c = 0; c < C; ++c) part[c] = add_rn(part[c], tap ? mul_rn(tv, (T)acc[c]) : (T)acc[c]);
+      } else {
+#pragma unroll
+        for (int c = 0; c < C; ++c) out[c] = (T)acc[c];
+      }
+    }
+    if (WIN) {
+#pragma unroll
+      for (int c = 0; c < C; ++c) out[c] = add_rn(out[c], part[c]);
     }
   }
   if (live) {
 #pragma unroll
-    for (int c = 0; c < C; ++c) y[((size_t)jh * nt + s) * C + c] = (T)acc[c];
+    for (int c = 0; c < C; ++c) y[((size_t)jh * nt + s) * C + c] = out[c];
   }
 }
 
+#define RADON_KERNEL_ARGS                                                                                          \
+  const T *__restrict__ x, T *__restrict__ y, long long nt, long long ntb, long long nhy, long long nhx, long long npy, \
+      long long npx, const double *__restrict__ hy, const double *__restrict__ hx, const double *__restrict__ py,      \
+      const double *__restrict__ px, bool interp, Windows win, const T *__restrict__ tap
+#define RADON_BODY_ARGS x, y, nt, ntb, nhy, nhx, npy, npx, hy, hx, py, px, interp, win, tap
+
+// the one-gather kernels of b2_radon and the windowed ones of b2_radon_windows; the windowed spreading kernel, whose
+// window loops keep more values live, is allowed the registers it needs (no spills) by a minimum of one CTA per SM
 template <typename T, int C, int KIND>
+__global__ void __launch_bounds__(RD_THREADS) radon_stack_kernel(RADON_KERNEL_ARGS) {
+  stack<T, C, KIND, false>(RADON_BODY_ARGS);
+}
+template <typename T, int C, int KIND>
+__global__ void __launch_bounds__(RD_THREADS) radon_spread_kernel(RADON_KERNEL_ARGS) {
+  spread<T, C, KIND, false>(RADON_BODY_ARGS);
+}
+template <typename T, int C, int KIND>
+__global__ void __launch_bounds__(RD_THREADS) radon_stack_windows_kernel(RADON_KERNEL_ARGS) {
+  stack<T, C, KIND, true>(RADON_BODY_ARGS);
+}
+template <typename T, int C, int KIND>
+__global__ void __launch_bounds__(RD_THREADS, 1) radon_spread_windows_kernel(RADON_KERNEL_ARGS) {
+  spread<T, C, KIND, true>(RADON_BODY_ARGS);
+}
+
+// WIN: the windows of win, with taper table tap (NULL: none); else the one gather (win and tap unused)
+template <typename T, int C, int KIND, bool WIN>
 int launch(const void* xv, void* yv, size_t nt, size_t nhy, size_t nhx, size_t npy, size_t npx, const double* hy,
            const double* hx, const double* py, const double* px, bool interp, bool adjoint, size_t blocks,
-           cudaStream_t st) {
+           const Windows& win, const void* tap, cudaStream_t st) {
   const T* x = static_cast<const T*>(xv);
   T* y = static_cast<T*>(yv);
+  const T* tp = static_cast<const T*>(tap);
   const long long ntb = (long long)((nt + RD_THREADS - 1) / RD_THREADS);
-  if (adjoint)
-    radon_stack_kernel<T, C, KIND><<<(unsigned)blocks, RD_THREADS, 0, st>>>(
-        x, y, (long long)nt, ntb, (long long)nhy, (long long)nhx, (long long)npx, hy, hx, py, px, interp);
-  else
-    radon_spread_kernel<T, C, KIND><<<(unsigned)blocks, RD_THREADS, 0, st>>>(
-        x, y, (long long)nt, ntb, (long long)nhx, (long long)npy, (long long)npx, hy, hx, py, px, interp);
+  auto kernel = adjoint ? (WIN ? radon_stack_windows_kernel<T, C, KIND> : radon_stack_kernel<T, C, KIND>)
+                        : (WIN ? radon_spread_windows_kernel<T, C, KIND> : radon_spread_kernel<T, C, KIND>);
+  kernel<<<(unsigned)blocks, RD_THREADS, 0, st>>>(x, y, (long long)nt, ntb, (long long)nhy, (long long)nhx,
+                                                  (long long)npy, (long long)npx, hy, hx, py, px, interp, win, tp);
   B2_LAUNCH_CHECK();
   return B2_OK;
 }
 
-template <typename T, int C>
+template <typename T, int C, bool WIN>
 int launch_kind(int kind, const void* x, void* y, size_t nt, size_t nhy, size_t nhx, size_t npy, size_t npx,
                 const double* hy, const double* hx, const double* py, const double* px, bool interp, bool adjoint,
-                size_t blocks, cudaStream_t st) {
+                size_t blocks, const Windows& win, const void* tap, cudaStream_t st) {
   switch (kind) {
     case B2_RADON_LINEAR:
-      return launch<T, C, B2_RADON_LINEAR>(x, y, nt, nhy, nhx, npy, npx, hy, hx, py, px, interp, adjoint, blocks, st);
+      return launch<T, C, B2_RADON_LINEAR, WIN>(x, y, nt, nhy, nhx, npy, npx, hy, hx, py, px, interp, adjoint, blocks,
+                                                win, tap, st);
     case B2_RADON_PARABOLIC:
-      return launch<T, C, B2_RADON_PARABOLIC>(x, y, nt, nhy, nhx, npy, npx, hy, hx, py, px, interp, adjoint, blocks,
-                                              st);
+      return launch<T, C, B2_RADON_PARABOLIC, WIN>(x, y, nt, nhy, nhx, npy, npx, hy, hx, py, px, interp, adjoint,
+                                                   blocks, win, tap, st);
     default:
-      return launch<T, C, B2_RADON_HYPERBOLIC>(x, y, nt, nhy, nhx, npy, npx, hy, hx, py, px, interp, adjoint, blocks,
-                                               st);
+      return launch<T, C, B2_RADON_HYPERBOLIC, WIN>(x, y, nt, nhy, nhx, npy, npx, hy, hx, py, px, interp, adjoint,
+                                                    blocks, win, tap, st);
   }
+}
+
+// the checks b2_radon and b2_radon_windows share
+bool radon_args(b2_ctx* ctx, const void* x, const void* y, size_t nt, size_t n_inner, size_t nhy, size_t nhx,
+                size_t npy, size_t npx, const double* hy, const double* hx, const double* py, const double* px,
+                int kind) {
+  if (!ctx || !x || !y || x == y || !hx || !px || (hy == nullptr) != (py == nullptr)) return false;
+  if (!hy && (nhy != 1 || npy != 1)) return false;
+  const size_t axis_max = (size_t)1 << 31;
+  for (size_t n : {nt, nhy, nhx, npy, npx})
+    if (n == 0 || n >= axis_max) return false;
+  if (n_inner != 1 && n_inner != 2) return false;
+  return kind == B2_RADON_LINEAR || kind == B2_RADON_PARABOLIC || kind == B2_RADON_HYPERBOLIC;
 }
 
 }  // namespace
@@ -214,22 +309,39 @@ int launch_kind(int kind, const void* x, void* y, size_t nt, size_t nhy, size_t 
 extern "C" int b2_radon(b2_ctx* ctx, const void* x, void* y, size_t nt, size_t n_inner, size_t nhy, size_t nhx,
                         size_t npy, size_t npx, const double* hy, const double* hx, const double* py,
                         const double* px, int kind, int interp, int adjoint, int dtype, void* stream) {
-  if (!ctx || !x || !y || x == y || !hx || !px || (hy == nullptr) != (py == nullptr)) return B2_ERR_ARG;
-  if (!hy && (nhy != 1 || npy != 1)) return B2_ERR_ARG;
-  const size_t axis_max = (size_t)1 << 31;
-  for (size_t n : {nt, nhy, nhx, npy, npx})
-    if (n == 0 || n >= axis_max) return B2_ERR_ARG;
-  if (n_inner != 1 && n_inner != 2) return B2_ERR_ARG;
-  if (kind != B2_RADON_LINEAR && kind != B2_RADON_PARABOLIC && kind != B2_RADON_HYPERBOLIC) return B2_ERR_ARG;
+  if (!radon_args(ctx, x, y, nt, n_inner, nhy, nhx, npy, npx, hy, hx, py, px, kind)) return B2_ERR_ARG;
   // one CTA per RD_THREADS samples of each output trace, in one grid
   const size_t ntb = (nt + RD_THREADS - 1) / RD_THREADS;
   const size_t traces = adjoint ? npy * npx : nhy * nhx;
   if (traces > 0x7fffffffULL / ntb) return B2_ERR_ARG;
   const size_t blocks = traces * ntb;
+  const Windows one{};
   return b2_dispatch_real(dtype, [&](auto t) {
     using T = decltype(t);
-    auto go = n_inner == 1 ? launch_kind<T, 1> : launch_kind<T, 2>;
-    return go(kind, x, y, nt, nhy, nhx, npy, npx, hy, hx, py, px, interp != 0, adjoint != 0, blocks,
+    auto go = n_inner == 1 ? launch_kind<T, 1, false> : launch_kind<T, 2, false>;
+    return go(kind, x, y, nt, nhy, nhx, npy, npx, hy, hx, py, px, interp != 0, adjoint != 0, blocks, one, nullptr,
+              (cudaStream_t)stream);
+  });
+}
+
+extern "C" int b2_radon_windows(b2_ctx* ctx, const void* x, void* y, size_t nt, size_t n_inner, size_t n0, size_t n1,
+                                size_t nhy, size_t nhx, size_t npy, size_t npx, const double* hy, const double* hx,
+                                const double* py, const double* px, int kind, int interp, size_t nwins0,
+                                size_t nwins1, size_t step0, size_t step1, const void* tap, int adjoint, int dtype,
+                                void* stream) {
+  if (!radon_args(ctx, x, y, nt, n_inner, nhy, nhx, npy, npx, hy, hx, py, px, kind)) return B2_ERR_ARG;
+  Windows win;
+  if (!make_windows(n0, n1, nwins0, nwins1, nhy, nhx, step0, step1, win)) return B2_ERR_ARG;
+  // one CTA per RD_THREADS samples of each output trace (adjoint: every window's model traces), in one grid
+  const size_t ntb = (nt + RD_THREADS - 1) / RD_THREADS;
+  const size_t mtr = npy * npx, nw = nwins0 * nwins1;
+  if (adjoint && (nw > 0x7fffffffULL / mtr || nw * mtr > 0x7fffffffULL / ntb)) return B2_ERR_ARG;
+  if (!adjoint && (n0 > 0x7fffffffULL / n1 || n0 * n1 > 0x7fffffffULL / ntb)) return B2_ERR_ARG;
+  const size_t blocks = (adjoint ? nw * mtr : n0 * n1) * ntb;
+  return b2_dispatch_real(dtype, [&](auto t) {
+    using T = decltype(t);
+    auto go = n_inner == 1 ? launch_kind<T, 1, true> : launch_kind<T, 2, true>;
+    return go(kind, x, y, nt, nhy, nhx, npy, npx, hy, hx, py, px, interp != 0, adjoint != 0, blocks, win, tap,
               (cudaStream_t)stream);
   });
 }

@@ -1117,6 +1117,229 @@ class Radon3D(_Radon):
                          name)
 
 
+def _taper(nmask, ntap, tapertype):
+    """pylops.utils.tapers.taper (pylops 2.x as remembered), float64: ``nmask`` samples rising over the first
+    ``ntap`` and falling over the last ``ntap`` (hanning: the first ``ntap`` samples of ``np.hanning(2 * ntap - 1)``;
+    cosine / cosinesquare: of ``(0.5 * (cos((k - c) * pi / c) + 1)) ** e``, ``c = ntap - 1``), ones between; ones
+    for ``None``.  ``ValueError`` for a hanning ``ntap`` above ``nmask / 2``."""
+    if tapertype is None:
+        return np.ones(nmask)
+    if tapertype == "hanning":
+        if ntap > 0 and nmask // ntap < 2:
+            raise ValueError(f"ntap={ntap} must be smaller or equal than {nmask // 2}")
+        rise = np.hanning(2 * ntap - 1)[:ntap]
+    elif tapertype in ("cosine", "cosinesquare"):
+        ntap = 0 if ntap == 1 else ntap
+        c = (2 * ntap - 2) / 2
+        with np.errstate(divide="ignore", invalid="ignore"):
+            rise = ((0.5 * (np.cos((np.arange(2 * ntap - 1) - c) * np.pi / c) + 1.0))
+                    ** (2 if tapertype == "cosinesquare" else 1))[:ntap]
+    else:
+        raise ValueError(f"tapertype={tapertype!r} is not supported (hanning, cosine, cosinesquare or None)")
+    return np.concatenate([rise, np.ones(nmask - 2 * ntap), rise[::-1]])
+
+
+def _slidingsteps(n, nwin, nover):
+    """the first trace of every window of ``nwin`` traces, one every ``nwin - nover``, along an axis of ``n``"""
+    if nwin > n:
+        raise ValueError(f"nwin={nwin} is bigger than ntr={n}...")
+    if not 0 <= nover < nwin:
+        raise ValueError(f"nover={nover} must be in [0, nwin) = [0, {nwin})")
+    return np.arange(0, n - nwin + 1, nwin - nover, dtype=int)
+
+
+def _axis_tapers(nwins, nwin, nover, tapertype, edge):
+    """``(nwins, nwin)`` float64: each window's taper along one axis, the first window's leading ``nover`` samples
+    and the last window's trailing ``nover`` set to ``edge(taper)`` (one window: the trailing ones only)"""
+    tap = _taper(nwin, nover, tapertype)
+    taps = np.tile(tap, (nwins, 1))
+    if nwins > 1:
+        taps[0, :nover] = edge(tap)
+    taps[-1, nwin - nover:] = edge(tap)
+    return taps
+
+
+def sliding2d_design(dimsd, nwin, nover, nop, verb=False):
+    """pylops.signalprocessing.sliding2d_design: ``(nwins, dims, mwins_inends, dwins_inends)`` of a
+    :class:`Sliding2D` on data ``dimsd = (n, nt)`` with windows of ``nwin`` traces overlapping by ``nover`` and an
+    inner operator of model ``nop``: ``dims = (nwins * nop[0], nop[1])``.  Host only."""
+    starts = _slidingsteps(int(dimsd[0]), int(nwin), int(nover))
+    nwins = len(starts)
+    dims = (nwins * int(nop[0]), int(nop[1]))
+    mstarts = np.arange(nwins) * int(nop[0])
+    if verb:
+        print(f"{nwins} windows of {nwin} traces, model {dims}, data {tuple(dimsd)}")
+    return (nwins, dims, ((mstarts, mstarts + int(nop[0])), (0, dims[1])),
+            ((starts, starts + int(nwin)), (0, int(dimsd[-1]))))
+
+
+def sliding3d_design(dimsd, nwin, nover, nop, verb=False):
+    """pylops.signalprocessing.sliding3d_design: ``(nwins, dims, mwins_inends, dwins_inends)`` of a
+    :class:`Sliding3D` on data ``dimsd = (n0, n1, nt)`` with windows ``nwin = (nwin0, nwin1)`` overlapping by
+    ``nover`` and an inner operator of model ``nop``: ``nwins = (nwins0, nwins1)``,
+    ``dims = (nwins0 * nop[0], nwins1 * nop[1], nop[2])``.  Host only."""
+    st = [_slidingsteps(int(dimsd[a]), int(nwin[a]), int(nover[a])) for a in (0, 1)]
+    nwins = (len(st[0]), len(st[1]))
+    dims = (nwins[0] * int(nop[0]), nwins[1] * int(nop[1]), int(nop[2]))
+    m = [np.arange(nwins[a]) * int(nop[a]) for a in (0, 1)]
+    if verb:
+        print(f"{nwins[0]} x {nwins[1]} windows of {tuple(nwin)} traces, model {dims}, data {tuple(dimsd)}")
+    return (nwins, dims, ((m[0], m[0] + int(nop[0])), (m[1], m[1] + int(nop[1])), (0, dims[2])),
+            ((st[0], st[0] + int(nwin[0])), (st[1], st[1] + int(nwin[1])), (0, int(dimsd[2]))))
+
+
+class _Sliding(_KernelOperator):
+    """The shared part of :class:`Sliding2D` / :class:`Sliding3D`: a section ``(n0, n1, inner)`` holding the grid of
+    ``nwins0 x nwins1`` windows of ``nwin0 x nwin1`` traces (Sliding2D: ``n0 = nwin0 = 1``), the per-window taper
+    table ``[nwins][nwin0][nwin1]`` (uploaded once per real dtype, rounded to the inner operator's dtype as pylops'
+    ``Diagonal(taper, dtype=Op.dtype)`` rounds it) and the apply:
+
+    - ``Op`` a :class:`Radon2D` / :class:`Radon3D` whose traces are the window's: one b2_radon_windows launch;
+    - any other kernel operator: ``Op``'s own launch per window into a workspace (allocated once per compute dtype),
+      and one b2_sliding launch to overlap-add (forward) or cut out (adjoint) the windows."""
+
+    def _check_op(self, Op):
+        if not isinstance(Op, _KernelOperator):
+            raise TypeError(f"{type(self).__name__}: Op must be a rank-local kernel operator of this package (not a "
+                            f"product or an adjoint), got {type(Op).__name__}")
+
+    def _setup(self, Op, dims, dimsd, section, nwins, nwin, steps, t0, t1, tapertype, name):
+        self.Op, self.dims, self.dimsd = Op, dims, dimsd
+        self.tapertype, self.name = tapertype, name
+        self.shape = (math.prod(dimsd), math.prod(dims))
+        self.dtype = Op.dtype
+        self._section, self._nwins, self._nwin, self._steps = section, nwins, nwin, steps
+        self._count = nwins[0] * nwins[1]
+        _lib.ctx()
+        self._taps = None
+        if tapertype is not None:
+            real = np.finfo(np.dtype(Op.dtype)).dtype
+            table = (t0[:, None, :, None] * t1[None, :, None, :]).reshape(self._count, *nwin).astype(real)
+            self._taps = {t: torch.as_tensor(np.ascontiguousarray(table, dtype=_lib.numpy_dtype(t))).to("cuda")
+                          for t in (torch.float32, torch.float64)}
+        self._work = {}
+        self._fused = None
+        if isinstance(Op, _Radon):
+            nhy, nhx, npy, npx = Op._geom[:4]
+            if (nhy, nhx) == tuple(nwin) and section[2] == Op._nt:
+                self._fused = Op
+
+    def _compute_dtype(self, xdt):
+        return self.Op._compute_dtype(xdt)
+
+    def _tap_ptr(self, real):
+        return None if self._taps is None else self._taps[real].data_ptr()
+
+    def _workspace(self, dt):
+        if dt not in self._work:
+            self._work[dt] = torch.empty(self._count * self.Op.shape[0], dtype=dt, device="cuda")
+        return self._work[dt]
+
+    def _launch(self, x, y, dt, adjoint):
+        real = _REAL_OF.get(dt, dt)
+        cplx = 2 if dt.is_complex else 1
+        (n0, n1, inner), (nw0, nw1), (l0, l1), (s0, s1) = self._section, self._nwins, self._nwin, self._steps
+        if self._fused is not None:
+            R = self._fused
+            nhy, nhx, npy, npx, hy, hx, py, px, kind, interp = R._geom
+            _lib.check(_lib.lib.b2_radon_windows(_lib.ctx(), x.data_ptr(), y.data_ptr(), R._nt, cplx, n0, n1, nhy,
+                                                 nhx, npy, npx, hy, hx, py, px, kind, interp, nw0, nw1, s0, s1,
+                                                 self._tap_ptr(real), adjoint, _lib.code(real), _lib.stream()),
+                       "b2_radon_windows")
+            return
+        work = self._workspace(dt)
+        nm, nd = self.Op.shape[1], self.Op.shape[0]
+        args = (n0, n1, inner, cplx, nw0, nw1, l0, l1, s0, s1, self._tap_ptr(real))
+        if adjoint:
+            _lib.check(_lib.lib.b2_sliding(_lib.ctx(), x.data_ptr(), work.data_ptr(), *args, 1, _lib.code(real),
+                                           _lib.stream()), "b2_sliding")
+        for w in range(self._count):
+            if adjoint:
+                self.Op._launch(work[w * nd:(w + 1) * nd], y[w * nm:(w + 1) * nm], dt, 1)
+            else:
+                self.Op._launch(x[w * nm:(w + 1) * nm], work[w * nd:(w + 1) * nd], dt, 0)
+        if not adjoint:
+            _lib.check(_lib.lib.b2_sliding(_lib.ctx(), work.data_ptr(), y.data_ptr(), *args, 0, _lib.code(real),
+                                           _lib.stream()), "b2_sliding")
+
+
+class Sliding2D(_Sliding):
+    """Rank-local sliding windows along axis 0 of a section, pylops.signalprocessing.Sliding2D (pylops 2.x as
+    remembered: pylops is not installed here to check it) inside MPIBlockDiag: local slant-stack denoising, slope
+    decomposition and interpolation with ``Op`` a :class:`Radon2D` applied to every window.  The data are
+    ``dimsd = (n, nt)``; windows of ``nwin`` traces start every ``nwin - nover`` traces (``arange(0, n - nwin + 1,
+    nwin - nover)``, so traces past the last window are 0 in the forward and ignored in the adjoint).  ``Op`` maps a
+    window's model of ``nop`` values to its ``(nwin, nt)`` data; the model is ``dims = (nwins * nop[0], nop[1])``,
+    window ``w``'s block contiguous (:func:`sliding2d_design` sizes it)::
+
+        y = sum over w ascending of R_w^T (tap_w * Op x_w),     x_w = Op^H (tap_w * R_w d)
+
+    with ``tap_w`` pylops' ``taper2d(nt, nwin, nover, tapertype)`` (hanning, cosine, cosinesquare or None), the first
+    window's leading and the last window's trailing ``nover`` samples set to 1 (one window: the trailing ones only),
+    rounded to ``Op``'s dtype.  Every product and sum of the overlap-add is in the data's type, in that order.
+
+    ``Op`` is a kernel operator of this package; a :class:`Radon2D` whose ``(nh, nt)`` data are a window's is applied
+    to every window in one b2_radon_windows launch (csrc/radon.cu), equal bit for bit to the per-window route; any other runs
+    its own launch per window, then one b2_sliding launch (csrc/sliding.cu).  Dtype rules, ``out=`` and complex data
+    are ``Op``'s.  ``TypeError`` for any other ``Op`` (products and ``.H`` included); ``ValueError`` for ``nwin > n``,
+    ``nover`` outside ``[0, nwin)``, ``dims`` other than ``(nwins * nop[0], nop[1])``, an ``Op`` whose data are not
+    ``nwin * nt`` values and a hanning ``nover`` above ``nwin / 2``."""
+
+    def __init__(self, Op, dims, dimsd, nwin, nover, tapertype="hanning", name="S"):
+        self._check_op(Op)
+        dims, dimsd = tuple(int(d) for d in dims), tuple(int(d) for d in dimsd)
+        if len(dims) != 2 or len(dimsd) != 2:
+            raise ValueError(f"dims and dimsd must hold two entries; got {dims}, {dimsd}")
+        self.nwin, self.nover = int(nwin), int(nover)
+        starts = _slidingsteps(dimsd[0], self.nwin, self.nover)
+        nwins = len(starts)
+        if nwins * Op.shape[1] // dims[1] != dims[0]:
+            raise ValueError(f"Model shape (dims={dims}) is not consistent with chosen number of windows. Run "
+                             f"sliding2d_design to identify the correct number of windows for the current model size...")
+        if Op.shape[0] != self.nwin * dimsd[1]:
+            raise ValueError(f"Op has {Op.shape[0]} data values; a window has {self.nwin} x {dimsd[1]}")
+        t1 = _axis_tapers(nwins, self.nwin, self.nover, tapertype, lambda t: 1.0)
+        self._setup(Op, dims, dimsd, (1, dimsd[0], dimsd[1]), (1, nwins), (1, self.nwin),
+                    (1, self.nwin - self.nover), np.ones((1, 1)), t1, tapertype, name)
+
+
+class Sliding3D(_Sliding):
+    """Rank-local sliding windows over axes 0 and 1 of a volume, pylops.signalprocessing.Sliding3D (pylops 2.x as
+    remembered) inside MPIBlockDiag: local 3-D slant-stack processing with ``Op`` a :class:`Radon3D`.  The data are
+    ``dimsd = (n0, n1, nt)``; windows of ``nwin = (nwin0, nwin1)`` traces overlap by ``nover = (nover0, nover1)`` and
+    form a grid, window ``w = i0 * nwins1 + i1``.  ``Op`` maps ``nop`` model values to a window's
+    ``(nwin0, nwin1, nt)`` data; the model is ``dims = (nwins0 * nop[0], nwins1 * nop[1], nop[2])`` stored
+    window-major, as BlockDiag orders its blocks (:func:`sliding3d_design` sizes it).  Each trace sums, for each i0
+    ascending, the sum over i1 ascending of its windows' ``tap_w * Op x_w``; the tapers are pylops'
+    ``taper3d(nt, nwin, nover, tapertype)``, with the outer ``nover`` rows / columns of the edge windows set to the
+    taper's middle value (one window along an axis: the trailing ones only).  Apply paths, dtypes and errors as in
+    :class:`Sliding2D` (a :class:`Radon3D` whose traces are a window's takes one b2_radon_windows launch), plus
+    ``ValueError`` for ``dims`` other than the above; ``nproc`` is accepted and ignored."""
+
+    def __init__(self, Op, dims, dimsd, nwin, nover, nop, tapertype="hanning", nproc=1, name="P"):
+        self._check_op(Op)
+        dims, dimsd = tuple(int(d) for d in dims), tuple(int(d) for d in dimsd)
+        self.nwin, self.nover = tuple(int(v) for v in nwin), tuple(int(v) for v in nover)
+        self.nop, self.nproc = tuple(int(v) for v in nop), nproc
+        if len(dims) != 3 or len(dimsd) != 3 or len(self.nwin) != 2 or len(self.nover) != 2 or len(self.nop) != 3:
+            raise ValueError(f"dims, dimsd and nop must hold three entries, nwin and nover two; got {dims}, {dimsd}, "
+                             f"{nop}, {nwin}, {nover}")
+        st = [_slidingsteps(dimsd[a], self.nwin[a], self.nover[a]) for a in (0, 1)]
+        nwins = (len(st[0]), len(st[1]))
+        if nwins[0] * self.nop[0] != dims[0] or nwins[1] * self.nop[1] != dims[1] or self.nop[2] != dims[2]:
+            raise ValueError(f"Model shape (dims={dims}) is not consistent with chosen number of windows. Run "
+                             f"sliding3d_design to identify the correct number of windows for the current model size...")
+        if Op.shape[1] != math.prod(self.nop):
+            raise ValueError(f"Op has {Op.shape[1]} model values; nop is {self.nop}")
+        if Op.shape[0] != self.nwin[0] * self.nwin[1] * dimsd[2]:
+            raise ValueError(f"Op has {Op.shape[0]} data values; a window has {self.nwin[0]} x {self.nwin[1]} x "
+                             f"{dimsd[2]}")
+        t0, t1 = (_axis_tapers(nwins[a], self.nwin[a], self.nover[a], tapertype, lambda t: t[len(t) // 2])
+                  for a in (0, 1))
+        self._setup(Op, dims, dimsd, dimsd, nwins, self.nwin, (self.nwin[0] - self.nover[0],
+                    self.nwin[1] - self.nover[1]), t0, t1, tapertype, name)
+
+
 class FFT(LocalOperator):
     """Rank-local real FFT along ``axis`` of a ``dims`` block -- the role of third-party
     ``pylops.signalprocessing.FFT(dims, axis, real=True, ifftshift_before=..., norm="ortho")`` inside
