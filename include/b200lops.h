@@ -335,6 +335,38 @@ int b2_radon_windows(b2_ctx* ctx, const void* x, void* y, size_t nt, size_t n_in
 int b2_sliding(b2_ctx* ctx, const void* x, void* y, size_t n0, size_t n1, size_t nt, size_t n_inner, size_t nwins0,
                size_t nwins1, size_t nwin0, size_t nwin1, size_t step0, size_t step1, const void* tap, int adjoint,
                int dtype, void* stream);
+/* b2_radon applied to every patch of a section, with the tapered overlap-add of b2_patch, in one launch: the
+ * time-space patch Radon transform of pylops.signalprocessing.Patch2D / Patch3D over Radon2D / Radon3D.  The section
+ * [n0][n1][ns][n_inner] holds nwins0 x nwins1 x nwins2 patches of nhy x nhx traces and nt samples, patch
+ * w = (i0 * nwins1 + i1) * nwins2 + i2 starting at (trace i0 * step0, trace i1 * step1, sample i2 * step2); the model
+ * is [nwins0 * nwins1 * nwins2][npy][npx][nt][n_inner], one b2_radon model block per patch on patch-local time and
+ * the patch-local offsets hy, hx (2-D: hy = py = NULL, nhy = npy = 1).  tap0, tap1, tap2 are b2_patch's per-axis
+ * float64 tapers.  Forward x (model) -> y (section): each section sample sums, as b2_patch's fold, tap * v over the
+ * patches that hold it, v the patch's b2_radon value at the patch-local sample (a float64 sum rounded once to the
+ * dtype); samples no patch holds are 0.  Adjoint x (section) -> y (model): each patch's b2_radon stack of tap * d, the
+ * product rounded to the dtype.  Both directions equal b2_radon per patch plus b2_patch bit for bit.  One launch, no
+ * atomics, no allocation.  dtype F32 / F64.  B2_ERR_ARG: b2_radon's checks, b2_patch's window checks, more CTAs than
+ * one grid holds; B2_ERR_DTYPE: another dtype; y is untouched on every error */
+int b2_radon_patches(b2_ctx* ctx, const void* x, void* y, size_t nt, size_t n_inner, size_t n0, size_t n1, size_t ns,
+                     size_t nhy, size_t nhx, size_t npy, size_t npx, const double* hy, const double* hx,
+                     const double* py, const double* px, int kind, int interp, size_t nwins0, size_t nwins1,
+                     size_t nwins2, size_t step0, size_t step1, size_t step2, const double* tap0, const double* tap1,
+                     const double* tap2, int adjoint, int dtype, void* stream);
+/* tapered overlap-add of time-space patches: the combining stage of pylops.signalprocessing.Patch2D / Patch3D and
+ * Sliding1D.  Windows [nwins0][nwins1][nwins2][nwin0][nwin1][nwin2][n_inner] (n_inner values per sample: 2 for the
+ * (re, im) pairs of complex data in the real dtype), data [n0][n1][nt][n_inner]; window
+ * w = (i0 * nwins1 + i1) * nwins2 + i2 starts at (trace i0 * step0, trace i1 * step1, sample i2 * step2).  tap0
+ * [nwins0][nwin0], tap1 [nwins1][nwin1], tap2 [nwins2][nwin2] are float64 per-axis tapers (NULL: that axis is not
+ * tapered); a window sample's taper is ((tap0 * tap1) * tap2) in float64 rounded once to the dtype.  Forward (fold)
+ * x = windows -> y = data: each sample is the sum over i0 ascending of the sum over i1 ascending of the sum over i2
+ * ascending of tap * window over the windows that hold it, every product and sum rounded to the dtype; samples no
+ * window holds are 0.  Adjoint (unfold) x = data -> y = windows: tap * data.  One launch, no atomics, no allocation.
+ * dtype F32 / F64.  B2_ERR_ARG: a null pointer (the tapers excepted), x == y, a zero size, an axis of 2^31 or more,
+ * windows that leave the section, 2^62 or more values; B2_ERR_DTYPE: another dtype; y is untouched on every error */
+int b2_patch(b2_ctx* ctx, const void* x, void* y, size_t n0, size_t n1, size_t nt, size_t n_inner, size_t nwins0,
+             size_t nwins1, size_t nwins2, size_t nwin0, size_t nwin1, size_t nwin2, size_t step0, size_t step1,
+             size_t step2, const double* tap0, const double* tap1, const double* tap2, int adjoint, int dtype,
+             void* stream);
 /* analytic (constant-velocity) traveltime table of pylops.waveeqprocessing.Kirchhoff, in b2_kirchhoff_chunk's
  * layout: table[p][j] = |grid point i0 + j - point p| / vel for p < n, j < nc (row stride nc).  Axes are float64
  * device arrays; y = NULL for 2-D (ny ignored), where the grid is meshgrid(x, z, indexing="ij") raveled,

@@ -104,6 +104,9 @@ def _load():
         "b2_radon_windows": ([vp, vp, vp, sz, sz, sz, sz, sz, sz, sz, sz, vp, vp, vp, vp, i, i, sz, sz, sz, sz, vp, i,
                               i, vp], i),
         "b2_sliding": ([vp, vp, vp, sz, sz, sz, sz, sz, sz, sz, sz, sz, sz, vp, i, i, vp], i),
+        "b2_radon_patches": ([vp, vp, vp, sz, sz, sz, sz, sz, sz, sz, sz, sz, vp, vp, vp, vp, i, i, sz, sz, sz, sz, sz,
+                              sz, vp, vp, vp, i, i, vp], i),
+        "b2_patch": ([vp, vp, vp, sz, sz, sz, sz, sz, sz, sz, sz, sz, sz, sz, sz, sz, vp, vp, vp, i, i, vp], i),
         "b2_kirchhoff_tables": ([vp, vp, vp, vp, sz, sz, sz, vp, sz, d, sz, sz, vp, vp], i),
         "b2_eikonal_tables": ([vp, vp, sz, sz, sz, d, d, d, vp, sz, sz, vp, vp, vp, vp], i),
         "b2_eikonal_work_bytes": ([sz, sz, sz, sz], sz),

@@ -1188,47 +1188,32 @@ def sliding3d_design(dimsd, nwin, nover, nop, verb=False):
             ((st[0], st[0] + int(nwin[0])), (st[1], st[1] + int(nwin[1])), (0, int(dimsd[2]))))
 
 
-class _Sliding(_KernelOperator):
-    """The shared part of :class:`Sliding2D` / :class:`Sliding3D`: a section ``(n0, n1, inner)`` holding the grid of
-    ``nwins0 x nwins1`` windows of ``nwin0 x nwin1`` traces (Sliding2D: ``n0 = nwin0 = 1``), the per-window taper
-    table ``[nwins][nwin0][nwin1]`` (uploaded once per real dtype, rounded to the inner operator's dtype as pylops'
-    ``Diagonal(taper, dtype=Op.dtype)`` rounds it) and the apply:
+class _Windowed(_KernelOperator):
+    """The shared part of the window operators (:class:`Sliding1D`, :class:`Sliding2D`, :class:`Sliding3D`,
+    :class:`Patch2D`, :class:`Patch3D`): ``Op``, the chosen apply path and the apply:
 
-    - ``Op`` a :class:`Radon2D` / :class:`Radon3D` whose traces are the window's: one b2_radon_windows launch;
+    - ``self._fused`` a :class:`Radon2D` / :class:`Radon3D` whose data are a window's: one fused launch
+      (``_fused_launch``);
     - any other kernel operator: ``Op``'s own launch per window into a workspace (allocated once per compute dtype),
-      and one b2_sliding launch to overlap-add (forward) or cut out (adjoint) the windows."""
+      and one overlap-add launch (``_fold``) to overlap-add (forward) or cut out (adjoint) the windows."""
 
     def _check_op(self, Op):
         if not isinstance(Op, _KernelOperator):
             raise TypeError(f"{type(self).__name__}: Op must be a rank-local kernel operator of this package (not a "
                             f"product or an adjoint), got {type(Op).__name__}")
 
-    def _setup(self, Op, dims, dimsd, section, nwins, nwin, steps, t0, t1, tapertype, name):
+    def _setup(self, Op, dims, dimsd, count, tapertype, name):
         self.Op, self.dims, self.dimsd = Op, dims, dimsd
         self.tapertype, self.name = tapertype, name
         self.shape = (math.prod(dimsd), math.prod(dims))
         self.dtype = Op.dtype
-        self._section, self._nwins, self._nwin, self._steps = section, nwins, nwin, steps
-        self._count = nwins[0] * nwins[1]
-        _lib.ctx()
-        self._taps = None
-        if tapertype is not None:
-            real = np.finfo(np.dtype(Op.dtype)).dtype
-            table = (t0[:, None, :, None] * t1[None, :, None, :]).reshape(self._count, *nwin).astype(real)
-            self._taps = {t: torch.as_tensor(np.ascontiguousarray(table, dtype=_lib.numpy_dtype(t))).to("cuda")
-                          for t in (torch.float32, torch.float64)}
+        self._count = count
         self._work = {}
         self._fused = None
-        if isinstance(Op, _Radon):
-            nhy, nhx, npy, npx = Op._geom[:4]
-            if (nhy, nhx) == tuple(nwin) and section[2] == Op._nt:
-                self._fused = Op
+        _lib.ctx()
 
     def _compute_dtype(self, xdt):
         return self.Op._compute_dtype(xdt)
-
-    def _tap_ptr(self, real):
-        return None if self._taps is None else self._taps[real].data_ptr()
 
     def _workspace(self, dt):
         if dt not in self._work:
@@ -1238,29 +1223,60 @@ class _Sliding(_KernelOperator):
     def _launch(self, x, y, dt, adjoint):
         real = _REAL_OF.get(dt, dt)
         cplx = 2 if dt.is_complex else 1
-        (n0, n1, inner), (nw0, nw1), (l0, l1), (s0, s1) = self._section, self._nwins, self._nwin, self._steps
         if self._fused is not None:
-            R = self._fused
-            nhy, nhx, npy, npx, hy, hx, py, px, kind, interp = R._geom
-            _lib.check(_lib.lib.b2_radon_windows(_lib.ctx(), x.data_ptr(), y.data_ptr(), R._nt, cplx, n0, n1, nhy,
-                                                 nhx, npy, npx, hy, hx, py, px, kind, interp, nw0, nw1, s0, s1,
-                                                 self._tap_ptr(real), adjoint, _lib.code(real), _lib.stream()),
-                       "b2_radon_windows")
+            self._fused_launch(x, y, real, cplx, adjoint)
             return
         work = self._workspace(dt)
         nm, nd = self.Op.shape[1], self.Op.shape[0]
-        args = (n0, n1, inner, cplx, nw0, nw1, l0, l1, s0, s1, self._tap_ptr(real))
         if adjoint:
-            _lib.check(_lib.lib.b2_sliding(_lib.ctx(), x.data_ptr(), work.data_ptr(), *args, 1, _lib.code(real),
-                                           _lib.stream()), "b2_sliding")
+            self._fold(x, work, real, cplx, 1)
         for w in range(self._count):
             if adjoint:
                 self.Op._launch(work[w * nd:(w + 1) * nd], y[w * nm:(w + 1) * nm], dt, 1)
             else:
                 self.Op._launch(x[w * nm:(w + 1) * nm], work[w * nd:(w + 1) * nd], dt, 0)
         if not adjoint:
-            _lib.check(_lib.lib.b2_sliding(_lib.ctx(), work.data_ptr(), y.data_ptr(), *args, 0, _lib.code(real),
-                                           _lib.stream()), "b2_sliding")
+            self._fold(work, y, real, cplx, 0)
+
+
+class _Sliding(_Windowed):
+    """The shared part of :class:`Sliding2D` / :class:`Sliding3D`: a section ``(n0, n1, inner)`` holding the grid of
+    ``nwins0 x nwins1`` windows of ``nwin0 x nwin1`` traces (Sliding2D: ``n0 = nwin0 = 1``), the per-window taper
+    table ``[nwins][nwin0][nwin1]`` (uploaded once per real dtype, rounded to the inner operator's dtype as pylops'
+    ``Diagonal(taper, dtype=Op.dtype)`` rounds it); the fused launch is b2_radon_windows, the overlap-add
+    b2_sliding."""
+
+    def _setup(self, Op, dims, dimsd, section, nwins, nwin, steps, t0, t1, tapertype, name):
+        super()._setup(Op, dims, dimsd, nwins[0] * nwins[1], tapertype, name)
+        self._section, self._nwins, self._nwin, self._steps = section, nwins, nwin, steps
+        self._taps = None
+        if tapertype is not None:
+            real = np.finfo(np.dtype(Op.dtype)).dtype
+            table = (t0[:, None, :, None] * t1[None, :, None, :]).reshape(self._count, *nwin).astype(real)
+            self._taps = {t: torch.as_tensor(np.ascontiguousarray(table, dtype=_lib.numpy_dtype(t))).to("cuda")
+                          for t in (torch.float32, torch.float64)}
+        if isinstance(Op, _Radon):
+            nhy, nhx, npy, npx = Op._geom[:4]
+            if (nhy, nhx) == tuple(nwin) and section[2] == Op._nt:
+                self._fused = Op
+
+    def _tap_ptr(self, real):
+        return None if self._taps is None else self._taps[real].data_ptr()
+
+    def _fused_launch(self, x, y, real, cplx, adjoint):
+        (n0, n1, _), (nw0, nw1), (s0, s1) = self._section, self._nwins, self._steps
+        R = self._fused
+        nhy, nhx, npy, npx, hy, hx, py, px, kind, interp = R._geom
+        _lib.check(_lib.lib.b2_radon_windows(_lib.ctx(), x.data_ptr(), y.data_ptr(), R._nt, cplx, n0, n1, nhy, nhx,
+                                             npy, npx, hy, hx, py, px, kind, interp, nw0, nw1, s0, s1,
+                                             self._tap_ptr(real), adjoint, _lib.code(real), _lib.stream()),
+                   "b2_radon_windows")
+
+    def _fold(self, src, dst, real, cplx, adjoint):
+        (n0, n1, inner), (nw0, nw1), (l0, l1), (s0, s1) = self._section, self._nwins, self._nwin, self._steps
+        _lib.check(_lib.lib.b2_sliding(_lib.ctx(), src.data_ptr(), dst.data_ptr(), n0, n1, inner, cplx, nw0, nw1, l0,
+                                       l1, s0, s1, self._tap_ptr(real), adjoint, _lib.code(real), _lib.stream()),
+                   "b2_sliding")
 
 
 class Sliding2D(_Sliding):
@@ -1338,6 +1354,215 @@ class Sliding3D(_Sliding):
                   for a in (0, 1))
         self._setup(Op, dims, dimsd, dimsd, nwins, self.nwin, (self.nwin[0] - self.nover[0],
                     self.nwin[1] - self.nover[1]), t0, t1, tapertype, name)
+
+
+def _window_design(dimsd, nwin, nover, nop):
+    """``(nwins, dims, mwins_inends, dwins_inends)`` of windows ``nwin`` overlapping by ``nover`` along the leading
+    ``len(nwin)`` axes of ``dimsd``, each window's model ``nop``, window-major"""
+    st = [_slidingsteps(int(dimsd[a]), int(nwin[a]), int(nover[a])) for a in range(len(nwin))]
+    nwins = tuple(len(s) for s in st)
+    dims = tuple(nw * int(n) for nw, n in zip(nwins, nop))
+    m = [np.arange(nw) * int(n) for nw, n in zip(nwins, nop)]
+    return (nwins, dims, tuple((mi, mi + int(n)) for mi, n in zip(m, nop)),
+            tuple((si, si + int(n)) for si, n in zip(st, nwin)))
+
+
+def sliding1d_design(dimd, nwin, nover, nop, verb=False):
+    """pylops.signalprocessing.sliding1d_design: ``(nwins, dim, mwin_inends, dwin_inends)`` of a :class:`Sliding1D`
+    on a signal of ``dimd`` samples with windows of ``nwin`` samples overlapping by ``nover`` and an inner operator of
+    ``nop`` model values: ``dim = nwins * nop``.  Host only."""
+    nwins, dims, m, d = _window_design((dimd,), (nwin,), (nover,), (nop,))
+    if verb:
+        print(f"{nwins[0]} windows of {nwin} samples, model {dims[0]}, data {dimd}")
+    return nwins[0], dims[0], m[0], d[0]
+
+
+def patch2d_design(dimsd, nwin, nover, nop, verb=False):
+    """pylops.signalprocessing.patch2d_design: ``(nwins, dims, mwins_inends, dwins_inends)`` of a :class:`Patch2D`
+    on data ``dimsd = (n, nt)`` with patches ``nwin = (nwin0, nwin1)`` overlapping by ``nover`` and an inner operator
+    of model ``nop``: ``nwins = (nwins0, nwins1)``, ``dims = (nwins0 * nop[0], nwins1 * nop[1])``.  Host only."""
+    out = _window_design(dimsd, nwin, nover, nop)
+    if verb:
+        print(f"{out[0][0]} x {out[0][1]} patches of {tuple(nwin)}, model {out[1]}, data {tuple(dimsd)}")
+    return out
+
+
+def patch3d_design(dimsd, nwin, nover, nop, verb=False):
+    """pylops.signalprocessing.patch3d_design: as :func:`patch2d_design` on data ``dimsd = (ny, nx, nt)`` with three
+    window axes: ``nwins = (nwins0, nwins1, nwins2)``, ``dims = (nwins0 * nop[0], nwins1 * nop[1], nwins2 * nop[2])``.
+    Host only."""
+    out = _window_design(dimsd, nwin, nover, nop)
+    if verb:
+        print(f"{' x '.join(map(str, out[0]))} patches of {tuple(nwin)}, model {out[1]}, data {tuple(dimsd)}")
+    return out
+
+
+def _patch_tapers(nwins, nwin, nover, tapertype):
+    """the float64 per-axis tapers ``[nwins_a][nwin_a]`` of b2_patch's three window axes (an axis with no windows:
+    None; all None for ``tapertype=None``), the one statement of pylops' taper rules as remembered:
+
+    - one axis (Sliding1D): ``taper(nwin, nover)``, the first window's leading and the last window's trailing
+      ``nover`` samples set to 1;
+    - two axes (Patch2D): ``taper2d(nwin[1], nwin[0], nover)``, the outer product of the two axis tapers, with the
+      edge patches' outer ``nover`` rows / columns replaced by the middle row / column;
+    - three axes (Patch3D): ``taper3d(nwin[2], nwin[:2], nover[:2])``, tapered along y and x and constant along t,
+      with the same edge rule on all three axes (a no-op along t).
+
+    An edge replacement by the middle value is, per axis, ``t[:nover] = t[nwin // 2]`` for the first window and
+    ``t[nwin - nover:] = t[nwin // 2]`` for the last (one window: the last only), so the product of the axis tables
+    is pylops' full taper bit for bit."""
+    if tapertype is None:
+        return [None, None, None]
+    mid = lambda t: t[len(t) // 2]                                   # noqa: E731
+    if len(nwin) == 1:
+        return [None, None, _axis_tapers(nwins[0], nwin[0], nover[0], tapertype, lambda t: 1.0)]
+    taps = [_axis_tapers(nwins[a], nwin[a], nover[a], tapertype, mid) for a in range(2)]
+    if len(nwin) == 2:
+        return [None] + taps
+    return taps + [_axis_tapers(nwins[2], nwin[2], nover[2], None, mid)]
+
+
+class _Patch(_Windowed):
+    """The shared part of :class:`Sliding1D` / :class:`Patch2D` / :class:`Patch3D`: a section ``(n0, n1, nt)`` (each
+    sample ``n_inner`` values) holding ``nwins0 x nwins1 x nwins2`` windows of ``nwin0 x nwin1`` traces and ``nwin2``
+    samples, window ``w = (i0 * nwins1 + i1) * nwins2 + i2`` (Patch2D: ``n0 = 1``; Sliding1D: ``n0 = n1 = 1``), and
+    the float64 per-axis tapers of :func:`_patch_tapers`, uploaded once; the fused launch is b2_radon_patches, the
+    overlap-add b2_patch.  Each window's taper is formed on the device from the axis tapers and rounded once to the
+    data's real dtype."""
+
+    def _setup(self, Op, dims, dimsd, section, nwins, nwin, nover, tapertype, scalings, name):
+        if scalings is not None:
+            raise NotImplementedError(f"{type(self).__name__}: scalings={scalings!r} is not supported (None only)")
+        model = math.prod(nwins) * Op.shape[1]
+        if math.prod(dims) != model:
+            raise ValueError(f"Model shape (dims={dims}) is not consistent with chosen number of windows. Run "
+                             f"{type(self).__name__.lower()}_design to identify the correct number of windows for the "
+                             f"current model size...")
+        if Op.shape[0] != math.prod(nwin):
+            raise ValueError(f"Op has {Op.shape[0]} data values; a window has {' x '.join(map(str, nwin))}")
+        k = 3 - len(nwin)
+        taps = _patch_tapers(nwins, nwin, nover, tapertype)
+        super()._setup(Op, dims, dimsd, math.prod(nwins), tapertype, name)
+        self._section = (1,) * k + tuple(section)
+        self._nwins = (1,) * k + tuple(nwins)
+        self._nwin = (1,) * k + tuple(nwin)
+        self._steps = (1,) * k + tuple(w - o for w, o in zip(nwin, nover))
+        self._taps = [None if t is None else torch.as_tensor(np.ascontiguousarray(t, dtype=np.float64)).to("cuda")
+                      for t in taps]
+
+    def _fuse(self, Op):
+        """take the fused path when ``Op`` is a Radon whose traces and samples are a window's"""
+        if isinstance(Op, _Radon) and tuple(Op._geom[:2]) + (Op._nt,) == self._nwin:
+            self._fused = Op
+
+    def _tap_ptrs(self):
+        return [_lib.ptr(t) for t in self._taps]
+
+    def _fused_launch(self, x, y, real, cplx, adjoint):
+        (n0, n1, ns), (nw0, nw1, nw2), (s0, s1, s2) = self._section, self._nwins, self._steps
+        R = self._fused
+        nhy, nhx, npy, npx, hy, hx, py, px, kind, interp = R._geom
+        _lib.check(_lib.lib.b2_radon_patches(_lib.ctx(), x.data_ptr(), y.data_ptr(), R._nt, cplx, n0, n1, ns, nhy,
+                                             nhx, npy, npx, hy, hx, py, px, kind, interp, nw0, nw1, nw2, s0, s1, s2,
+                                             *self._tap_ptrs(), adjoint, _lib.code(real), _lib.stream()),
+                   "b2_radon_patches")
+
+    def _fold(self, src, dst, real, cplx, adjoint):
+        (n0, n1, nt), (nw0, nw1, nw2), (l0, l1, l2), (s0, s1, s2) = (self._section, self._nwins, self._nwin,
+                                                                      self._steps)
+        _lib.check(_lib.lib.b2_patch(_lib.ctx(), src.data_ptr(), dst.data_ptr(), n0, n1, nt, cplx, nw0, nw1, nw2, l0,
+                                     l1, l2, s0, s1, s2, *self._tap_ptrs(), adjoint, _lib.code(real),
+                                     _lib.stream()), "b2_patch")
+
+
+def _ints(name, v, n):
+    v = tuple(int(a) for a in (v if np.ndim(v) else (v,)))
+    if len(v) != n:
+        raise ValueError(f"{name} must hold {n} entries; got {v}")
+    return v
+
+
+class Sliding1D(_Patch):
+    """Rank-local sliding windows along a 1-D signal, pylops.signalprocessing.Sliding1D (pylops 2.x as remembered:
+    pylops is not installed here to check it) inside MPIBlockDiag.  Windows of ``nwin`` samples start every
+    ``nwin - nover`` samples of the ``dimd`` data samples (samples past the last window are 0 in the forward and
+    ignored in the adjoint).  ``Op`` maps a window's model of ``nop`` values to its ``nwin`` samples; the model is
+    ``dim = nwins * nop``, window ``w``'s block contiguous (:func:`sliding1d_design` sizes it)::
+
+        y = sum over w ascending of R_w^T (tap_w * Op x_w),     x_w = Op^H (tap_w * R_w d)
+
+    with ``tap_w`` pylops' ``taper(nwin, nover, tapertype)`` (hanning, cosine, cosinesquare or None), the first
+    window's leading and the last window's trailing ``nover`` samples set to 1 (one window: the trailing ones only),
+    rounded to the data's real dtype.  ``Op`` is a kernel operator of this package, applied by its own launch per
+    window, then one b2_patch launch (csrc/sliding.cu).  Dtype rules, ``out=`` and complex data are ``Op``'s.
+    ``TypeError`` for any other ``Op`` (products and ``.H`` included); ``ValueError`` for ``nwin > dimd``, ``nover``
+    outside ``[0, nwin)``, ``dim`` other than ``nwins * nop``, an ``Op`` whose data are not ``nwin`` values and a
+    hanning ``nover`` above ``nwin / 2``."""
+
+    def __init__(self, Op, dim, dimd, nwin, nover, tapertype="hanning", name="S"):
+        self._check_op(Op)
+        dim, dimd = _ints("dim", dim, 1), _ints("dimd", dimd, 1)
+        self.nwin, self.nover = int(nwin), int(nover)
+        nwins = len(_slidingsteps(dimd[0], self.nwin, self.nover))
+        self._setup(Op, dim, dimd, (dimd[0],), (nwins,), (self.nwin,), (self.nover,), tapertype, None, name)
+
+
+class Patch2D(_Patch):
+    """Rank-local time-space patches of a section, pylops.signalprocessing.Patch2D (pylops 2.x as remembered: pylops
+    is not installed here to check it) inside MPIBlockDiag: local Radon (slope) denoising and interpolation of curved
+    events, with ``Op`` a :class:`Radon2D` applied to every patch.  The data are ``dimsd = (n, nt)``; patches of
+    ``nwin = (nwin0, nwin1)`` (traces, samples) overlap by ``nover`` and form a grid, patch ``w = i0 * nwins1 + i1``
+    starting at ``(i0 * (nwin0 - nover0), i1 * (nwin1 - nover1))`` (traces and samples past the last patch are 0 in
+    the forward and ignored in the adjoint).  ``Op`` maps ``nop`` model values to a patch's ``(nwin0, nwin1)`` data;
+    the model is ``dims = (nwins0 * nop[0], nwins1 * nop[1])`` stored window-major, as BlockDiag orders its blocks
+    (:func:`patch2d_design` sizes it).  Each sample sums, over i0 ascending, the sum over i1 ascending of its patches'
+    ``tap_w * Op x_w``; the tapers are pylops' ``taper2d(nwin1, nwin0, nover, tapertype)``, the outer product of the
+    two axis tapers, with the edge patches' outer ``nover`` rows / columns replaced by the taper's middle row /
+    column (one patch along an axis: the trailing ones only), rounded to the data's real dtype.
+
+    ``Op`` is a kernel operator of this package; a :class:`Radon2D` whose ``(nh, nt)`` data are a patch's is applied to
+    every patch in one b2_radon_patches launch (csrc/radon.cu), equal bit for bit to the per-patch route; any other runs
+    its own launch per patch, then one b2_patch launch (csrc/sliding.cu).  Dtype rules, ``out=`` and complex data are
+    ``Op``'s.  ``TypeError`` for any other ``Op`` (products and ``.H`` included); ``NotImplementedError`` for
+    ``scalings`` other than None; ``ValueError`` for ``nwin > n``, ``nover`` outside ``[0, nwin)``, ``dims`` other than
+    the above, an ``Op`` whose model / data are not ``nop`` / a patch and a hanning ``nover`` above ``nwin / 2``."""
+
+    def __init__(self, Op, dims, dimsd, nwin, nover, nop, tapertype="hanning", scalings=None, name="P"):
+        self._check_op(Op)
+        dims, dimsd = _ints("dims", dims, 2), _ints("dimsd", dimsd, 2)
+        self.nwin, self.nover, self.nop = _ints("nwin", nwin, 2), _ints("nover", nover, 2), _ints("nop", nop, 2)
+        self.scalings = scalings
+        nwins = tuple(len(_slidingsteps(dimsd[a], self.nwin[a], self.nover[a])) for a in (0, 1))
+        if Op.shape[1] != math.prod(self.nop) or dims != tuple(w * n for w, n in zip(nwins, self.nop)):
+            raise ValueError(f"Model shape (dims={dims}) is not consistent with chosen number of windows and Op's "
+                             f"model of {Op.shape[1]} values (nop={self.nop}). Run patch2d_design to identify the "
+                             f"correct number of windows for the current model size...")
+        self._setup(Op, dims, dimsd, dimsd, nwins, self.nwin, self.nover, tapertype, scalings, name)
+        self._fuse(Op)
+
+
+class Patch3D(_Patch):
+    """Rank-local time-space patches of a volume, pylops.signalprocessing.Patch3D (pylops 2.x as remembered) inside
+    MPIBlockDiag: local 3-D Radon processing with ``Op`` a :class:`Radon3D`.  As :class:`Patch2D` over data
+    ``dimsd = (ny, nx, nt)`` with three window axes: patches ``nwin = (nwin0, nwin1, nwin2)`` overlapping by ``nover``,
+    patch ``w = (i0 * nwins1 + i1) * nwins2 + i2``, model ``dims = (nwins0 * nop[0], nwins1 * nop[1], nwins2 * nop[2])``
+    window-major (:func:`patch3d_design` sizes it), each sample summed over i0, of i1, of i2, all ascending.  The tapers
+    are pylops' ``taper3d(nwin2, nwin[:2], nover[:2], tapertype)``: tapered along y and x, constant along t, with the
+    edge rule on all three axes (a no-op along t).  A :class:`Radon3D` whose data are a patch's takes one
+    b2_radon_patches launch.  Apply paths, dtypes and errors as in :class:`Patch2D`."""
+
+    def __init__(self, Op, dims, dimsd, nwin, nover, nop, tapertype="hanning", scalings=None, name="P"):
+        self._check_op(Op)
+        dims, dimsd = _ints("dims", dims, 3), _ints("dimsd", dimsd, 3)
+        self.nwin, self.nover, self.nop = _ints("nwin", nwin, 3), _ints("nover", nover, 3), _ints("nop", nop, 3)
+        self.scalings = scalings
+        nwins = tuple(len(_slidingsteps(dimsd[a], self.nwin[a], self.nover[a])) for a in (0, 1, 2))
+        if Op.shape[1] != math.prod(self.nop) or dims != tuple(w * n for w, n in zip(nwins, self.nop)):
+            raise ValueError(f"Model shape (dims={dims}) is not consistent with chosen number of windows and Op's "
+                             f"model of {Op.shape[1]} values (nop={self.nop}). Run patch3d_design to identify the "
+                             f"correct number of windows for the current model size...")
+        self._setup(Op, dims, dimsd, dimsd, nwins, self.nwin, self.nover, tapertype, scalings, name)
+        self._fuse(Op)
 
 
 class FFT(LocalOperator):
